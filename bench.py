@@ -2,7 +2,7 @@
 """bench.py -- TPC-H Q1 (filter + 2-key group-by, 4 sums, 3 avgs, count) over synthetic SF100 lineitem.
 
 One "step" = one full pass of the hot path over the rank's lineitem partition:
-  HashAggregate(Partial) over [Scan -> Filter -> Project] as ONE fused sm_100a kernel launch per
+  HashAggregate(Partial) over [Scan -> Filter -> Project] as ONE fused sm_90a kernel launch per
   device chunk (+ fold/finalize), then the partial states of all ranks are gathered on rank 0 and
   merged by HashAggregate(Final) (merge_batch semantics) -- the same two plans Spark + Comet run on
   either side of the shuffle (SURVEY.md section 3D).
@@ -11,11 +11,15 @@ One "step" = one full pass of the hot path over the rank's lineitem partition:
 `e2e`    : the same plans through cb200_create_plan / cb200_execute with HOST Arrow buffers handed over
            as an ArrowArrayStream (pinned host memory; H2D inside the timed region; result D2H).
 `roofline`: algorithmic bytes of the fused Q1 kernel / its CUDA-event duration (events recorded by the
-           library on the stream it launches on) against MEASURED_PEAKS.json hbm_gbs.
+           library on the stream it launches on) against MEASURED_PEAKS.json hbm_gbs when present, else the H100 SXM data
+           sheet's 3.35 TB/s.
 `cpu_baseline` / `--impl reference`: the CPU oracle port (oracle/comet_oracle.c, OpenMP, all host
            cores) -- the reference's Rust/DataFusion path cannot be built in this image (no Rust).
 
-Launch: python bench.py [--gpus N --steps K --warmup W]   (torchrun for N>1, one rank per GPU)
+Launch: python bench.py [--gpus N --steps K --warmup W] [--dump-outputs DIR]   (torchrun for N>1, one rank per GPU)
+
+The bench writes nothing into the source tree: pipeline kernels it has to compile go to a temporary cubin cache
+(CB200_CACHE_DIR), the ones the build shipped are read from the tree, and no bytecode is written.
 """
 import argparse
 import json
@@ -27,12 +31,14 @@ import tempfile
 import threading
 import time
 
+sys.dont_write_bytecode = True
 ROOT = os.path.dirname(os.path.abspath(__file__))
 for p in (ROOT, os.path.join(ROOT, "datafusion-comet_b200")):
     if p not in sys.path:
         sys.path.insert(0, p)
 
 SF100_ROWS = 600_037_902
+HBM_SPEC_GBS = 3350.0   # H100 SXM data sheet, HBM3
 METRIC = "rows/sec on TPC-H Q1 filter+agg"
 # bytes the fused kernel must read per row (Arrow layout, dictionary-coded flags):
 #   l_shipdate date32 4 + returnflag/linestatus codes 1+1 + 4 x Decimal128 16  (DESIGN.md "algorithmic bytes")
@@ -44,19 +50,7 @@ def measured_peak():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
-
-
-def profiled_traffic(rows, variant):
-    """dram__bytes_read.sum + dram__bytes_write.sum of ONE bulk launch of the fused kernel, from the committed `ncu --set full`
-    capture of this same workload (profiles/r1_traffic.json, written by tools/summarize_ncu.py); None when the capture was taken
-    at another size / variant."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "r1_traffic.json")) as f:
-            t = json.load(f)["cb_pipeline_agg"]
-        return int(t["dram_bytes"]) if int(t["rows"]) == int(rows) and t["variant"] == variant else None
-    except Exception:
-        return None
+        return HBM_SPEC_GBS, "H100 SXM data sheet (3.35 TB/s), not measured"
 
 
 class ClockSampler:
@@ -414,19 +408,31 @@ def reference_arm(args, rank, world):
 # =====================================================================================================================
 def q1_expected_from_torch(torch, cols, cutoff):
     """All eight Q1 outputs of this rank's partition, exact, from torch int64 arithmetic on the device (independent of the library
-    AND of the oracle): sums as python ints, averages by the reference's HALF_UP rule, per group index 0..5."""
-    keep = cols["l_shipdate"] <= cutoff
-    gid = (cols["l_returnflag"].to(torch.int64) * 2 + cols["l_linestatus"].to(torch.int64))[keep]
-    q, p, dsc, tax = (cols[k][keep] for k in ("l_quantity", "l_extendedprice", "l_discount", "l_tax"))
+    AND of the oracle): sums as python ints, averages by the reference's HALF_UP rule, per group index 0..5.  Runs over 64 Mi-row
+    slices so that its temporaries stay a few GB next to the resident columns on an 80 GB device."""
+    n = cols["l_shipdate"].shape[0]
+    cnt, sq, sp, sd, sdp, sch = ([0] * 6 for _ in range(6))
+    for a in range(0, n, 1 << 26):
+        c = {k: v[a:a + (1 << 26)] for k, v in cols.items()}
+        keep = c["l_shipdate"] <= cutoff
+        gid = (c["l_returnflag"].to(torch.int64) * 2 + c["l_linestatus"].to(torch.int64))[keep]
+        q, p, dsc, tax = (c[k][keep] for k in ("l_quantity", "l_extendedprice", "l_discount", "l_tax"))
 
-    def gsum(v):
-        return torch.zeros(6, dtype=torch.int64, device=v.device).scatter_add_(0, gid, v).cpu().tolist()
-    cnt = torch.bincount(gid, minlength=6).cpu().tolist()
-    sq, sp, sd = gsum(q), gsum(p), gsum(dsc)
-    dp = p * (100 - dsc)                      # d(26,4) unscaled: < 2.1e9 per row
-    sdp = gsum(dp)
-    ch = dp * (100 + tax)                     # d(38,6) unscaled: < 2.3e11 per row; 1.5e8 rows per group overflow int64 -> split
-    sch = [hi * (1 << 20) + lo for hi, lo in zip(gsum(ch >> 20), gsum(ch & ((1 << 20) - 1)))]
+        def gsum(v):
+            return torch.zeros(6, dtype=torch.int64, device=v.device).scatter_add_(0, gid, v).cpu().tolist()
+
+        def acc(total, part):
+            for g in range(6):
+                total[g] += part[g]
+        acc(cnt, torch.bincount(gid, minlength=6).cpu().tolist())
+        acc(sq, gsum(q))
+        acc(sp, gsum(p))
+        acc(sd, gsum(dsc))
+        dp = p * (100 - dsc)                      # d(26,4) unscaled: < 2.1e9 per row
+        acc(sdp, gsum(dp))
+        ch = dp * (100 + tax)                     # d(38,6) unscaled: < 2.3e11 per row; 1.5e8 rows per group overflow int64 -> split
+        acc(sch, [hi * (1 << 20) + lo for hi, lo in zip(gsum(ch >> 20), gsum(ch & ((1 << 20) - 1)))])
+        del c, keep, gid, q, p, dsc, tax, dp, ch
 
     def avg(s, c):                            # avg_decimal.rs:670-689: sum * 10^4 / count, HALF_UP
         qq, r = divmod(abs(s) * 10**4, c)
@@ -461,6 +467,20 @@ def q1_compare(tpch, res, expected):
     return bool(ok)
 
 
+def dump_q1_outputs(tpch, res, out_dir):
+    """The Final plan's result as the caller receives it, one float64 array per output column, rows in the order returned:
+    group.npy = returnflag index * 2 + linestatus index (tpch.RETURNFLAGS / LINESTATUS), the seven decimals by value, count."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    rows = res.to_pylist()
+    cols = {"group": [tpch.RETURNFLAGS.index(r["col_0"]) * 2 + tpch.LINESTATUS.index(r["col_1"]) for r in rows]}
+    for j, name in enumerate(Q1_OUT):
+        cols[name] = [float(r[f"col_{2 + j}"]) for r in rows]
+    cols["count"] = [r["col_9"] for r in rows]
+    for name, v in cols.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), np.asarray(v, dtype=np.float64))
+
+
 def workload_q1(args, env):
     import numpy as np
     import pyarrow as pa
@@ -470,6 +490,7 @@ def workload_q1(args, env):
     variant, n = args.variant, args.rows
     cols = gen_device(torch, n, 42 + rank, device)
     money = build_columns(torch, cols, variant)
+    torch.cuda.empty_cache()   # the generators' temporaries: the library allocates from its own pool, not from torch's cache
     partial_plan, final_plan = tpch.q1_partial_plan(variant), tpch.q1_final_plan(variant)
     chunk_rows = min(args.chunk_rows, 2_000_000_000)
     table = bind_table(native, P, tpch, variant, n, money, cols)   # the resident columns are bound once; every step runs fresh plans over them
@@ -500,6 +521,8 @@ def workload_q1(args, env):
     pipe_launches = sum(o[1]["pipeline_launches"] for o in outs)
     launches = sum(o[1]["kernel_launches"] + (o[2]["kernel_launches"] if o[2] else 0) for o in outs)
     res = outs[-1][0]
+    if rank == 0 and args.dump_outputs:
+        dump_q1_outputs(tpch, res, args.dump_outputs)
 
     # ---- checks (outside the timed region) ---------------------------------------------------------------------------------------
     # (1) every output of every group at FULL size against exact torch int64 arithmetic (rank 0's partition; N = 1 only: the final
@@ -524,6 +547,7 @@ def workload_q1(args, env):
         checks["oracle_all_outputs_rows"] = m
         checks["oracle_all_outputs_ok"] = q1_compare(tpch, res_sub, {g: e for g, e in enumerate(exp) if e is not None})
         del h, t_sub
+        torch.cuda.empty_cache()
 
     # ---- end-to-end leg: HOST buffers -> C ABI -> result (per rank; rank 0 merges) ------------------------------------------------
     e2e, e2e_extra, host = None, {}, None
@@ -630,9 +654,9 @@ def workload_q1(args, env):
                        "parallelism": f"round-robin partitions x{world}; partial states gathered on rank 0 by one NCCL all-gather of a fixed-size buffer (library communicator), merged by the Final plan",
                        "l2": f"inputs ({BYTES_PER_ROW[variant] * n / 1e9:.1f} GB per GPU) exceed L2; no flush needed",
                        "checks": checks},
-            "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": profiled_traffic(n, variant),
+            "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": None,
                          "kernel": "cb_pipeline_agg (fused scan+filter+project+partial aggregate)", "ms_per_launch": ms_per_launch,
-                         "spec_peak": 8000.0, "frac_of_spec_peak": achieved / 8000.0,
+                         "spec_peak": HBM_SPEC_GBS, "frac_of_spec_peak": achieved / HBM_SPEC_GBS,
                          "algorithmic_bytes_per_row": BYTES_PER_ROW[variant], "peak_source": peak_src},
             "gpu_launches": launches, "clocks": clocks, "step_ms": env["step_ms"],
         }
@@ -827,7 +851,7 @@ def workload_groupby(args, env):
                          "peak_source": peak_src},
             "phases_ms": {"partial_kernels": part_ms, "final_kernels": last["st2"]["pipeline_ms"], "exchange_payload": xs["payload_ms"]},
             "exchange": {"bytes_sent_per_gpu": xs["bytes_sent"], "bytes_received_per_gpu": xs["bytes_received"], "payload_ms": xs["payload_ms"],
-                         "GBps_per_gpu": xs["bytes_sent"] / max(xs["payload_ms"], 1e-6) / 1e6, "nvlink_peak_GBps_per_direction": 900.0},
+                         "GBps_per_gpu": xs["bytes_sent"] / max(xs["payload_ms"], 1e-6) / 1e6, "nvlink_peak_GBps_per_direction": 450.0},
             "gpu_launches": sum(o["st"]["kernel_launches"] + o["st2"]["kernel_launches"] for o in outs), "clocks": clocks, "step_ms": env["step_ms"],
         }
         if e2e:
@@ -898,7 +922,7 @@ def workload_select_or_q6(args, env):
                 "config": {"workload": f"{args.workload} over {n} resident rows per GPU, variant {variant}", "rows_per_gpu": n, "rows_out": outs[-1][0], "parallelism": f"replicas x{world}",
                            "l2": "inputs exceed L2; no flush needed"},
                 "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": None, "kernel": kernel,
-                             "ms_pipeline_kernels_per_step": pipe_ms, "spec_peak": 8000.0, "frac_of_spec_peak": achieved / 8000.0, "algorithmic_bytes_per_row": bytes_row,
+                             "ms_pipeline_kernels_per_step": pipe_ms, "spec_peak": HBM_SPEC_GBS, "frac_of_spec_peak": achieved / HBM_SPEC_GBS, "algorithmic_bytes_per_row": bytes_row,
                              "peak_source": peak_src},
                 "gpu_launches": sum(o[1]["kernel_launches"] for o in outs), "clocks": clocks, "step_ms": env["step_ms"]}
         print(json.dumps(line))
@@ -911,7 +935,9 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200")
     ap.add_argument("--workload", default="q1", choices=["q1", "groupby", "config1", "q6"],
-                    help="q1 = BASELINE.json configs[1] (the driver's default); groupby = configs[3] (hash-repartition across GPUs); config1 / q6 = configs[0] / [2] kernels on resident columns")
+                    help="q1 = BASELINE.json configs[1] (the default); groupby = configs[3] (hash-repartition across GPUs); config1 / q6 = configs[0] / [2] kernels on resident columns")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="q1: write the last timed step's result columns to DIR/<name>.npy (float64) for output-for-output comparison of two builds")
     ap.add_argument("--variant", default="dec", choices=["dec", "f64"])
     ap.add_argument("--rows", type=int, default=int(os.environ.get("CB200_BENCH_ROWS", SF100_ROWS)))
     ap.add_argument("--ref-rows", type=int, default=60_000_000)
@@ -931,6 +957,8 @@ def main():
     ap.add_argument("--parquet-compression", default="NONE", choices=["NONE", "SNAPPY"])
     ap.add_argument("--no-cpu", action="store_true")
     args = ap.parse_args()
+    if args.dump_outputs and (args.workload != "q1" or args.impl == "reference"):
+        ap.error("--dump-outputs is implemented for the q1 workload of this implementation")
     if os.environ.get("CB200_BENCH_TRACE_S"):          # debugging aid: dump every thread's Python stack every N seconds to stderr
         import faulthandler
         faulthandler.dump_traceback_later(float(os.environ["CB200_BENCH_TRACE_S"]), repeat=True)
@@ -939,13 +967,15 @@ def main():
     if args.impl == "reference":
         reference_arm(args, rank, world)
         return
-    env = setup(args)
-    if args.workload == "q1":
-        workload_q1(args, env)
-    elif args.workload == "groupby":
-        workload_groupby(args, env)
-    else:
-        workload_select_or_q6(args, env)
+    with tempfile.TemporaryDirectory(prefix="cb200_jitcache_") as jit_dir:
+        os.environ.setdefault("CB200_CACHE_DIR", jit_dir)   # kernels compiled at run time; the shipped cache is still read
+        env = setup(args)
+        if args.workload == "q1":
+            workload_q1(args, env)
+        elif args.workload == "groupby":
+            workload_groupby(args, env)
+        else:
+            workload_select_or_q6(args, env)
     if env["comm"] is not None:
         env["comm"].destroy()
     if env["world"] > 1:

@@ -66,7 +66,8 @@ void start(cb200_plan* p) {
             cuda_check(cudaDeviceGetAttribute(&di.sms, cudaDevAttrMultiProcessorCount, ctx.device), "cudaDeviceGetAttribute");
             di.known = true;
         }
-        if (di.major < 10) throw ExecError(CB200_ERR_CUDA, "", "comet_b200 kernels are built for sm_100a; device is sm_" + std::to_string(di.major * 10 + di.minor));
+        // sm_90a code runs on compute capability 9.0 only: the `a` features (and the cubins) do not carry forward
+        if (di.major != 9 || di.minor != 0) throw ExecError(CB200_ERR_CUDA, "", "comet_b200 kernels are built for sm_90a; device is sm_" + std::to_string(di.major * 10 + di.minor));
         ctx.num_sms = di.sms;
     }
     {
@@ -111,7 +112,7 @@ DType dtype_from_ids(int type_id, int precision, int scale) {
 
 extern "C" {
 
-const char* cb200_version(void) { return "comet_b200 0.1.0 (sm_100a; reference apache/datafusion-comet 1.1.0 @2699f59b)"; }
+const char* cb200_version(void) { return "comet_b200 0.1.0 (sm_90a; reference apache/datafusion-comet 1.1.0 @2699f59b)"; }
 
 int cb200_supports(const uint8_t* op_proto, size_t op_len, cb200_error* why) {
     return cb200_guarded(why, [&]() -> int {

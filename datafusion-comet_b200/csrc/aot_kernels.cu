@@ -1,4 +1,4 @@
-// aot_kernels.cu -- ahead-of-time sm_100a kernels that do not depend on the plan: Arrow buffer
+// aot_kernels.cu -- ahead-of-time sm_90a kernels that do not depend on the plan: Arrow buffer
 // normalisation (bitmap append at arbitrary bit offsets, byte->bitmap packing), dictionary code
 // remapping and the device-side string dictionary builder used to turn Utf8 group keys into dense
 // codes.  (Plan-dependent kernels are JIT-specialised: device/cb_kernels.cuh.)

@@ -1,4 +1,4 @@
-// aot_kernels.h -- host-callable launchers of the plan-independent sm_100a kernels.
+// aot_kernels.h -- host-callable launchers of the plan-independent sm_90a kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>

@@ -1,7 +1,7 @@
-// cb_kernels.cuh -- hand-written sm_100a kernel skeletons for the fused scan -> filter -> project
+// cb_kernels.cuh -- hand-written sm_90a kernel skeletons for the fused scan -> filter -> project
 // -> {compact | aggregate} pipelines.  A pipeline kernel = this file + one generated `cb_prog`
 // block (the plan's expression tree spliced into straight-line code by codegen.cpp) compiled by
-// NVRTC for sm_100a at createPlan time.  Everything that decides performance lives here:
+// NVRTC for sm_90a at createPlan time.  Everything that decides performance lives here:
 //
 //   * persistent CTAs (grid = #SMs x CTAs/SM), each looping over row tiles;
 //   * TMA bulk staging: one elected thread issues `cp.async.bulk.shared::cluster.global` per input

@@ -1,7 +1,7 @@
 // cb_math.h -- integer / decimal / hash arithmetic shared by every comet_b200 kernel.
 //
 // Plain C++ with no includes so that the same text compiles three ways:
-//   * under NVRTC as part of a JIT-specialised pipeline kernel (sm_100a),
+//   * under NVRTC as part of a JIT-specialised pipeline kernel (sm_90a),
 //   * under nvcc for the ahead-of-time kernels (parquet decode, partition, hash table),
 //   * under g++ (CB_HOST_TEST) so tests/ can check every function against the oracle on CPU.
 //
@@ -541,7 +541,7 @@ CB_HD i32 f32_total_key(u32 bits) { i32 b = (i32)bits; return b ^ (i32)(((u32)(b
 
 // Float negation = sign-bit flip, exact for NaN (sign and payload) like Rust's `-x` / arrow-arith `neg`.
 // On the device a plain `-x` (and any xor the optimiser can recognise as fneg) becomes neg.f64, which the
-// hardware executes as an add that returns the canonical +qNaN for NaN inputs (measured on sm_100a) -- so the
+// hardware executes as an add that returns the canonical +qNaN for NaN inputs -- so the
 // flip is done in opaque integer PTX.
 CB_HD double f64_neg(double x) {
 #if defined(__CUDA_ARCH__)

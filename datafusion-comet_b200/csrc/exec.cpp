@@ -60,7 +60,7 @@ BlockCache g_block_cache[64];
 const size_t BLOCK_CACHE_MIN = 1 << 20;
 size_t block_cache_limit() {
     static size_t lim = 0;
-    if (!lim) { const char* e = getenv("CB200_BLOCK_CACHE_BYTES"); lim = e && *e ? (size_t)atoll(e) : (size_t)96 << 30; if (!lim) lim = 1; }
+    if (!lim) { const char* e = getenv("CB200_BLOCK_CACHE_BYTES"); lim = e && *e ? (size_t)atoll(e) : (size_t)32 << 30; if (!lim) lim = 1; }
     return lim;
 }
 size_t size_class(size_t n) {

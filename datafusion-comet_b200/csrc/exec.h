@@ -82,7 +82,7 @@ struct Batch {
 struct ExecContext {
     int device = 0;
     cudaStream_t stream = nullptr;
-    int num_sms = 148;
+    int num_sms = 132;        // H100 SXM; start() reads the device's count
     int64_t chunk_rows = 1ll << 26;
     int hash_threads = 512;   // consumer threads per CTA of the hash-aggregate kernel (tuning knob)
     // Partial hash aggregates over inputs of at least this many rows sample whether equal keys are adjacent and, if so, emit one state

@@ -1,4 +1,4 @@
-// jit.cpp -- NVRTC -> sm_100a cubin -> cudaLibraryLoadData.  The device library and the kernel
+// jit.cpp -- NVRTC -> sm_90a cubin -> cudaLibraryLoadData.  The device library and the kernel
 // skeletons (device/cb_math.h, device/cb_kernels.cuh) are embedded in the .so as strings
 // (device_src.inc, generated at build time) and handed to NVRTC as in-memory headers.
 #include "jit.h"
@@ -34,25 +34,33 @@ cudaKernel_t CompiledModule::kernel(const std::string& name) {
     return k;
 }
 
-std::string jit_cache_dir() {
+std::vector<std::string> jit_cache_dirs() {
+    std::vector<std::string> dirs;
     const char* env = getenv("CB200_CACHE_DIR");
-    if (env && *env) return env;
+    if (env && *env) dirs.push_back(env);
     Dl_info info;
-    if (dladdr((void*)&jit_cache_dir, &info) && info.dli_fname) {
+    if (dladdr((void*)&jit_cache_dirs, &info) && info.dli_fname) {
         std::string p = info.dli_fname;
         size_t s = p.rfind('/');
-        return (s == std::string::npos ? std::string(".") : p.substr(0, s)) + "/.jitcache";
+        dirs.push_back((s == std::string::npos ? std::string(".") : p.substr(0, s)) + "/.jitcache");
     }
-    return "/tmp/cb200_jitcache";
+    if (dirs.empty()) dirs.push_back("/tmp/cb200_jitcache");
+    return dirs;
 }
 
-// cubins depend on the device headers as much as on the generated translation unit
+// --fmad=false: every float expression node rounds once, like the reference's per-node arrays
+static const char* const kNvrtcOpts[] = {"--gpu-architecture=sm_90a", "-std=c++17", "-lineinfo", "--fmad=false"};
+
+// cubins depend on the device headers and the compile options (the target architecture above all) as much as on
+// the generated translation unit
 static std::string headers_tag() {
     static std::string tag;
     if (tag.empty()) {
         uint64_t h = 1469598103934665603ull;
         for (const char* src : {cb_math_src, cb_params_src, cb_kernels_src})
             for (const char* c = src; *c; c++) { h ^= (unsigned char)*c; h *= 1099511628211ull; }
+        for (const char* opt : kNvrtcOpts)
+            for (const char* c = opt; *c; c++) { h ^= (unsigned char)*c; h *= 1099511628211ull; }
         char buf[32];
         snprintf(buf, sizeof(buf), "%016llx", (unsigned long long)h);
         tag = buf;
@@ -69,9 +77,7 @@ static std::vector<char> compile(const GeneratedKernel& g) {
     const char* names[3] = {"cb_math.h", "cb_params.h", "cb_kernels.cuh"};
     if (nvrtcCreateProgram(&prog, g.source.c_str(), ("cb200_" + g.key + ".cu").c_str(), 3, headers, names) != NVRTC_SUCCESS)
         throw JitError("nvrtcCreateProgram failed");
-    // --fmad=false: every float expression node rounds once, like the reference's per-node arrays
-    const char* opts[] = {"--gpu-architecture=sm_100a", "-std=c++17", "-lineinfo", "--fmad=false"};
-    nvrtcResult r = nvrtcCompileProgram(prog, 4, opts);
+    nvrtcResult r = nvrtcCompileProgram(prog, (int)(sizeof(kNvrtcOpts) / sizeof(kNvrtcOpts[0])), kNvrtcOpts);
     if (r != NVRTC_SUCCESS) {
         size_t n = 0;
         nvrtcGetProgramLogSize(prog, &n);
@@ -83,7 +89,7 @@ static std::vector<char> compile(const GeneratedKernel& g) {
     size_t n = 0;
     if (nvrtcGetCUBINSize(prog, &n) != NVRTC_SUCCESS || n == 0) {
         nvrtcDestroyProgram(&prog);
-        throw JitError("NVRTC produced no cubin (sm_100a not supported by this NVRTC?)");
+        throw JitError("NVRTC produced no cubin (sm_90a not supported by this NVRTC?)");
     }
     std::vector<char> cubin(n);
     nvrtcGetCUBIN(prog, cubin.data());
@@ -98,12 +104,16 @@ std::shared_ptr<CompiledModule> jit_get(const GeneratedKernel& g, bool load) {
     if (it != g_cache.end()) m = it->second;
     if (!m) {
         m = std::make_shared<CompiledModule>();
-        std::string dir = jit_cache_dir(), path = dir + "/" + g.key + "_" + headers_tag() + ".cubin";
-        std::ifstream in(path, std::ios::binary);
-        if (in) {
-            m->cubin.assign(std::istreambuf_iterator<char>(in), std::istreambuf_iterator<char>());
+        const std::vector<std::string> dirs = jit_cache_dirs();
+        const std::string file = "/" + g.key + "_" + headers_tag() + ".cubin";
+        for (const std::string& d : dirs) {
+            std::ifstream in(d + file, std::ios::binary);
+            if (in) m->cubin.assign(std::istreambuf_iterator<char>(in), std::istreambuf_iterator<char>());
+            if (!m->cubin.empty()) break;
         }
         if (m->cubin.empty()) {
+            const std::string& dir = dirs.front();
+            const std::string path = dir + file;
             m->cubin = compile(g);
             mkdir(dir.c_str(), 0755);
             std::string tmp = path + ".tmp" + std::to_string((long)getpid());

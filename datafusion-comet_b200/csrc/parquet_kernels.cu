@@ -1,4 +1,4 @@
-// parquet_kernels.cu -- Parquet page decode on sm_100a.
+// parquet_kernels.cu -- Parquet page decode on sm_90a.
 //
 // Encodings per the Apache Parquet specification (Encodings.md): PLAIN for fixed-width physical types,
 // RLE/bit-packed hybrid for dictionary indices (RLE_DICTIONARY: 1 byte bit width, then runs) and for
@@ -719,7 +719,7 @@ template <int W> __global__ void k_pq_scatter(const u8* valid, const u32* idx, c
 }
 void launch_pq_scatter(const unsigned char* valid, const unsigned* idx, const void* dense, void* out, unsigned* bitmap, long long total, int width, cudaStream_t st) {
     if (total <= 0) return;
-    const int blocks = (int)std::min<long long>((total + 255) / 256, 148 * 16);
+    const int blocks = (int)std::min<long long>((total + 255) / 256, 132 * 16); // grid-stride: 16 CTAs per H100 SM
     if (width == 4) k_pq_scatter<4><<<blocks, 256, 0, st>>>(valid, idx, (const u8*)dense, (u8*)out, bitmap, total);
     else if (width == 8) k_pq_scatter<8><<<blocks, 256, 0, st>>>(valid, idx, (const u8*)dense, (u8*)out, bitmap, total);
     else k_pq_scatter<16><<<blocks, 256, 0, st>>>(valid, idx, (const u8*)dense, (u8*)out, bitmap, total);

@@ -1,5 +1,5 @@
 /*
- * comet_b200.h -- C ABI of libcomet_b200.so: the B200-native drop-in for the hot path of
+ * comet_b200.h -- C ABI of libcomet_b200.so: the H100-native drop-in for the hot path of
  * apache/datafusion-comet's native layer (scan -> filter -> project -> hash aggregate).
  *
  * The entry points are exactly what the reference's JNI surface binds for this path; each one names
@@ -192,7 +192,7 @@ int cb200_plan_stats(cb200_plan* plan, cb200_stats* out);
  * pools are host-side, native/core/src/execution/memory_pools/). */
 int64_t cb200_release_cached_memory(int32_t device_ordinal);
 
-/* Build-time: generate and NVRTC-compile (sm_100a; needs no GPU) every pipeline kernel the plan would
+/* Build-time: generate and NVRTC-compile (sm_90a; needs no GPU) every pipeline kernel the plan would
  * use for null-free inputs; cubins land in the JIT cache that ships with the library.  Writes the
  * comma-separated kernel keys to `keys_out`.  Returns the number of kernels, <0 on error. */
 int cb200_compile_plan(const uint8_t* op_proto, size_t op_len, char* keys_out, size_t keys_cap, cb200_error* err);

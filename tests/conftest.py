@@ -10,7 +10,7 @@ for p in (ROOT, os.path.join(ROOT, "datafusion-comet_b200")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90a); run with -m gpu")
 
 
 @pytest.fixture(scope="session")

@@ -1,5 +1,5 @@
 """GPU parity: TPC-H Q1 / Q6 / Config 1 through the C ABI vs the CPU oracle (bit-exact for decimals,
-1 ULP of the exact sum for float aggregates).  `pytest -m gpu` on a B200."""
+1 ULP of the exact sum for float aggregates).  `pytest -m gpu` on an H100."""
 import math
 
 import numpy as np

@@ -1,7 +1,7 @@
 """Pin the CPU oracle against the reference's own in-file known-answer tests.
 
-Each test names the reference file:line holding the vector (paths under
-/root/reference/native/).  These run on CPU (`-m "not gpu"`).
+Each test names the reference file:line holding the vector (paths under native/ of
+apache/datafusion-comet).  These run on CPU (`-m "not gpu"`).
 """
 import numpy as np
 import pytest
