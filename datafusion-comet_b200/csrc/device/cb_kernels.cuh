@@ -266,7 +266,7 @@ struct Acc {
             if (__any_sync(0xffffffffu, fresh)) {
                 int gn = alloc_gids(fresh);
                 if (fresh) {
-                    if (gn < 0) { atomicOr(p->hflags, 2); gn = p->max_groups; shared_g = true; } // out of state rows: the host grows the arrays and repeats the launch
+                    if (gn < 0) { atomicOr(p->hflags, CB_HF_FULL); gn = p->max_groups; shared_g = true; } // out of state rows: the host grows the arrays and repeats the launch
                     else {
 #pragma unroll
                         for (int i = 0; i < CB_KEY_WORDS; i++) p->hkey_of_gid[(size_t)gn * CB_KEY_WORDS + i] = kw[i];
@@ -279,7 +279,7 @@ struct Acc {
 #endif
         bool unresolved = want;
         if (want && null_group) { g = p->max_groups + 1; unresolved = false; }           // reserved group of the NULL key
-        if (CB_KEY_WORDS == 1 && unresolved && kw[0] == CB_EMPTY_KEY) { atomicOr(p->hflags, 1); g = p->max_groups; unresolved = false; } // the key equal to the empty pattern
+        if (CB_KEY_WORDS == 1 && unresolved && kw[0] == CB_EMPTY_KEY) { atomicOr(p->hflags, CB_HF_SENTINEL); g = p->max_groups; unresolved = false; } // the key equal to the empty pattern
         const u64 tag = CB_KEY_WORDS == 1 ? kw[0] : key_tag(kw);
         u32 s = (CB_KEY_WORDS == 1 ? (u32)mix64(tag) : (u32)(tag ^ (tag >> 32))) & mask;
         u32 probes = 0;
@@ -287,7 +287,7 @@ struct Acc {
             bool claimed = false, pending = false;
             if (unresolved) {
                 while (true) {
-                    if (probes++ > mask) { atomicOr(p->hflags, 2); g = p->max_groups; unresolved = false; break; } // table full: cannot happen (host sizes it)
+                    if (probes++ > mask) { atomicOr(p->hflags, CB_HF_FULL); g = p->max_groups; unresolved = false; break; } // table full: cannot happen (host sizes it)
 #if CB_CAS_FIRST
                     // merging state rows: most keys are new, so claim first and look second -- one L2 / HBM round trip instead of two
                     ulonglong2 slot;
@@ -315,7 +315,7 @@ struct Acc {
             if (__any_sync(0xffffffffu, claimed)) {
                 int gn = alloc_gids(claimed);
                 if (claimed) {
-                    if (gn < 0) { atomicOr(p->hflags, 2); gn = p->max_groups; } // cannot happen: host sizes max_groups >= rows
+                    if (gn < 0) { atomicOr(p->hflags, CB_HF_FULL); gn = p->max_groups; } // cannot happen: host sizes max_groups >= rows
                     else {
 #pragma unroll
                         for (int i = 0; i < CB_KEY_WORDS; i++) p->hkey_of_gid[(size_t)gn * CB_KEY_WORDS + i] = kw[i];

@@ -464,7 +464,7 @@ CB_HD i64 i64_div_checked(i64 a, i64 b, int bits, int& err) {
 // The reference adds row by row and nulls the sum as soon as a running prefix leaves the precision
 // (agg_funcs/sum_decimal.rs:418-439).  A parallel sum reproduces that exactly whenever no ordering
 // of the addends can overflow: n * max|v| <= 10^p - 1.
-// host certificate h (exec.cpp AggNode::certificate, from the observed input ranges):
+// host certificate h (agg.cpp AggNode::certificate, from the observed input ranges):
 //   0: n * max|v| <= 10^p - 1          -> no ordering can overflow, the exact total is the answer
 //   1: n * max|v| <  2^127             -> the 128-bit total is exact; if IT is out of range every ordering
 //                                         overflows (the last prefix is the total), otherwise order-dependent

@@ -1,11 +1,11 @@
 // cb_params.h -- kernel parameter blocks shared by the device skeletons (cb_kernels.cuh) and the host
-// executor (exec.cpp).  Plain structs over the cb_math.h typedefs so both sides agree on layout.
+// executor (exec.cpp, agg.cpp).  Plain structs over the cb_math.h typedefs so both sides agree on layout.
 #ifndef CB_PARAMS_H
 #define CB_PARAMS_H
 #include "cb_math.h"
 namespace cb {
 
-// pipeline kernels (filled by exec.cpp; passed __grid_constant__)
+// pipeline kernels (filled by exec.cpp / agg.cpp; passed __grid_constant__)
 #define CB_MAX_COLS 24
 #define CB_MAX_OUT 24
 #define CB_MAX_KEYS 4
@@ -53,6 +53,11 @@ struct PipeParams {
 #define CB_GID_RANGES 64
 #define CB_HFLAG_CTR 16
 #define CB_HFLAG_WORDS (CB_HFLAG_CTR + CB_GID_RANGES)
+// hflags[0] bits
+#define CB_HF_SENTINEL 1    // a key equal to the empty-slot pattern was seen (reserved group max_groups)
+#define CB_HF_FULL 2        // out of group ids / key table full
+#define CB_HF_WIDE_KEY 4    // a decimal(p > 18) key does not fit the 64-bit packing
+#define CB_HF_NULL_GROUP 8  // the NULL-key group (reserved group max_groups + 1) was used
 
 
 // fold / finalize kernels of aggregate pipelines

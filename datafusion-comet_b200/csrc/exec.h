@@ -93,7 +93,6 @@ struct ExecContext {
     int* d_err = nullptr;   // device error flags
     int* h_err = nullptr;   // pinned host mirror
     int64_t kernel_launches = 0;
-    std::string last_kernel_key;
     // measurement (bench.py / cb200_plan_stats): CUDA events around each fused pipeline kernel, on the
     // stream the kernel is launched on
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;

@@ -4,7 +4,7 @@
 // the exact arithmetic the kernels perform.  Used twice:
 //   * codegen.cpp: with ASSUMED (and in-kernel validated) column bounds, to pick 64-bit arithmetic and
 //     drop checks that provably never fire (CheckOverflow, i128 overflow, wide-decimal bound);
-//   * exec.cpp: with OBSERVED column bounds (OR-masks the kernels accumulate over every valid input
+//   * agg.cpp: with OBSERVED column bounds (OR-masks the kernels accumulate over every valid input
 //     value), to certify that a parallel decimal SUM cannot overflow for any row order, which is what
 //     makes it bit-identical to the reference's row-by-row accumulation
 //     (native/spark-expr/src/agg_funcs/sum_decimal.rs:418-439).

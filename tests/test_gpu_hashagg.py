@@ -193,6 +193,30 @@ def test_dense_to_hash_migration_mid_stream(cb):
     assert {r["col_0"]: [r["col_1"], r["col_2"]] for r in res.to_pylist()} == exp
 
 
+def test_dense_regroup_when_dictionary_grows_and_gains_nulls(cb):
+    """A dictionary key stays on the dense path while its plan-global dictionary grows from 3 to 10 values and NULL keys appear
+    in a later batch: the accumulated totals move to each wider group layout, the NULL slot staying the last one of its key."""
+    P = cb.proto
+    rng = np.random.default_rng(47)
+    names = [f"k{i}" for i in range(10)]
+    batches, exp = [], {}
+    for n_values, null_frac in ((3, 0.0), (6, 0.0), (9, 0.15), (10, 0.1)):
+        n = 5000
+        codes = rng.integers(0, n_values, n).astype(np.int32)
+        vals = rng.integers(-10**9, 10**9, n)
+        nulls = rng.random(n) < null_frac
+        for c, v, isnull in zip(codes.tolist(), vals.tolist(), nulls.tolist()):
+            e = exp.setdefault(None if isnull else names[c], [0, 0])
+            e[0] += v
+            e[1] += 1
+        keys = pa.DictionaryArray.from_arrays(pa.array(codes, mask=nulls if null_frac else None), pa.array(names[:n_values]))
+        batches.append(pa.RecordBatch.from_arrays([keys, pa.array(vals)], names=["k", "v"]))
+    plan = P.hash_agg(P.scan([P.STRING, P.INT64]), [P.bound(0, P.STRING)], [P.agg_sum(P.bound(1, P.INT64), P.INT64), P.agg_count([P.literal(1, P.INT32)])], P.PARTIAL)
+    out = run(cb, plan, [batches], 5000)                                   # one device chunk per batch
+    assert out.num_rows == len(exp) == 11                                  # dense: every group exactly once, NULL included
+    assert {r["col_0"]: [r["col_1"], r["col_2"]] for r in out.to_pylist()} == exp
+
+
 # ---- stream mode (CB_STREAM): Partial aggregates over clustered keys emit one state row per run, no key table --------------------
 def run_cfg(cb, plan, inputs, cfg):
     with cb.native.Plan(plan, inputs, config={k: str(v) for k, v in cfg.items()}) as p:
