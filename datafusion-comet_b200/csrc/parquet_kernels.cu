@@ -75,7 +75,7 @@ __global__ void __launch_bounds__(SN_WARPS * 32) k_pq_snappy(PqPage* pages, int 
     if (lane == 0) pre = snappy_preamble(in, n, ulen64);
     pre = __shfl_sync(0xffffffffu, pre, 0);
     ulen64 = __shfl_sync(0xffffffffu, ulen64, 0);
-    if (pre < 0 || ulen64 != (u64)pg.body_bytes) { if (lane == 0) atomicOr(err, 8); return; }
+    if (pre < 0 || ulen64 != (u64)pg.body_bytes) { if (lane == 0) atomicOr(err, PQ_ERR_SNAPPY); return; }
     const u32 ulen = (u32)ulen64;
     // the window holds input bytes [wbase, wbase + SN_WIN) where wbase is `in`-relative and 16-byte aligned in memory
     const u32 misalign = (u32)((size_t)in & 15);
@@ -158,7 +158,7 @@ __global__ void __launch_bounds__(SN_WARPS * 32) k_pq_snappy(PqPage* pages, int 
         __syncwarp(); // the next element may read what this one wrote
         o += len;
     }
-    if ((bad || o != ulen) && lane == 0) atomicOr(err, 8);
+    if ((bad || o != ulen) && lane == 0) atomicOr(err, PQ_ERR_SNAPPY);
 }
 // ---- Snappy, segmented ------------------------------------------------------------------------------------------------------------
 // One warp per page leaves most of the GPU idle (a batch has a few hundred pages) and a page of small elements -- PLAIN INT64
@@ -220,7 +220,7 @@ __global__ void __launch_bounds__(SXI_WARPS * 32) k_pq_snappy_index(PqPage* page
     if (lane == 0) pre = snappy_preamble(in, n, ulen64);
     pre = __shfl_sync(0xffffffffu, pre, 0);
     ulen64 = __shfl_sync(0xffffffffu, ulen64, 0);
-    if (pre < 0 || ulen64 != (u64)pg.body_bytes) { if (lane == 0) { atomicOr(err, 8); atomicOr(&pages[warp].flags, PQ_PAGE_SN_BAD); } return; }
+    if (pre < 0 || ulen64 != (u64)pg.body_bytes) { if (lane == 0) { atomicOr(err, PQ_ERR_SNAPPY); atomicOr(&pages[warp].flags, PQ_PAGE_SN_BAD); } return; }
     u32* ck = ckpt + pg.seg_base;
     const u32 misalign = (u32)((size_t)in & 15);
     const u32 body = (u32)pg.body_bytes;
@@ -297,7 +297,7 @@ __global__ void __launch_bounds__(SXI_WARPS * 32) k_pq_snappy_index(PqPage* page
     }
     if (status == 0 && (o != body || k != pg.n_segs)) status = (o == body && pos == n && k < pg.n_segs) ? 1 : 2;
     if (lane == 0) {
-        if (status == 2) { atomicOr(err, 8); atomicOr(&pages[warp].flags, PQ_PAGE_SN_BAD); }
+        if (status == 2) { atomicOr(err, PQ_ERR_SNAPPY); atomicOr(&pages[warp].flags, PQ_PAGE_SN_BAD); }
         else if (status == 1) atomicOr(&pages[warp].flags, PQ_PAGE_SN_SERIAL);
     }
 }
@@ -422,7 +422,7 @@ __global__ void __launch_bounds__(SX_WARPS * 32) k_pq_snappy_seg(PqPage* pages, 
     }
     if (status == 0 && o != oend) status = 2;
     if (lane == 0) {
-        if (status == 2) { atomicOr(err, 8); atomicOr(&pages[lo].flags, PQ_PAGE_SN_BAD); }
+        if (status == 2) { atomicOr(err, PQ_ERR_SNAPPY); atomicOr(&pages[lo].flags, PQ_PAGE_SN_BAD); }
         else if (status == 1) atomicOr(&pages[lo].flags, PQ_PAGE_SN_SERIAL);
     }
 }
@@ -440,13 +440,6 @@ void launch_pq_snappy_segmented(PqPage* pages, int n_pages, unsigned* ckpt, int 
     const int smem1 = SN_WARPS * (SN_RING + SN_WIN);
     cudaFuncSetAttribute(k_pq_snappy, cudaFuncAttributeMaxDynamicSharedMemorySize, smem1);
     k_pq_snappy<<<(n_pages + SN_WARPS - 1) / SN_WARPS, SN_WARPS * 32, smem1, st>>>(pages, n_pages, err, 1); // irregular pages only
-}
-
-void launch_pq_snappy(PqPage* pages, int n_pages, int* err, cudaStream_t st) {
-    if (n_pages <= 0) return;
-    const int smem = SN_WARPS * (SN_RING + SN_WIN);
-    cudaFuncSetAttribute(k_pq_snappy, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); // per device, idempotent
-    k_pq_snappy<<<(n_pages + SN_WARPS - 1) / SN_WARPS, SN_WARPS * 32, smem, st>>>(pages, n_pages, err, 0);
 }
 
 // ---- locate levels / values inside the page body ------------------------------------------------------------------------
@@ -477,17 +470,15 @@ template <int CONV> __global__ void k_pq_plain(const PqPage* pages, int flba_len
     const PqPage pg = pages[blockIdx.y];
     if (pg.encoding != 0) return; // dictionary-encoded page: decoded by k_pq_rle_decode
     const u8* src = pg.values;
-    const int w = CONV == PQ_COPY32 || CONV == PQ_I32_TO_I64 || CONV == PQ_I32_TO_I128 ? 4 : CONV == PQ_COPY64 || CONV == PQ_I64_TO_I128 ? 8 : flba_len;
+    const int w = CONV == PQ_COPY32 || CONV == PQ_I32_TO_I64 ? 4 : CONV == PQ_COPY64 ? 8 : flba_len;
     const int have = w > 0 ? pg.values_bytes / w : 0;   // never read beyond the page, whatever the header claims
     const int count = pg.nonnull < have ? pg.nonnull : have;
-    if (pg.nonnull > have && blockIdx.x == 0 && threadIdx.x == 0) atomicOr(err, 16); // short page: the rows it cannot fill must not pass silently
+    if (pg.nonnull > have && blockIdx.x == 0 && threadIdx.x == 0) atomicOr(err, PQ_ERR_TRUNCATED); // short page: the rows it cannot fill must not pass silently
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < count; i += gridDim.x * blockDim.x) {
         long long row = pg.dst_row + i;
         if (CONV == PQ_COPY32) ((u32*)out)[row] = load_u32_unaligned(src + (size_t)i * 4);
         else if (CONV == PQ_COPY64) ((u64*)out)[row] = load_u64_unaligned(src + (size_t)i * 8);
         else if (CONV == PQ_I32_TO_I64) ((i64*)out)[row] = (i64)(i32)load_u32_unaligned(src + (size_t)i * 4);
-        else if (CONV == PQ_I64_TO_I128) ((i128*)out)[row] = i128_from_i64((i64)load_u64_unaligned(src + (size_t)i * 8));
-        else if (CONV == PQ_I32_TO_I128) ((i128*)out)[row] = i128_from_i64((i64)(i32)load_u32_unaligned(src + (size_t)i * 4));
         else { // FIXED_LEN_BYTE_ARRAY: big-endian two's complement of flba_len bytes
             const u8* b = src + (size_t)i * flba_len;
             u64 hi = (b[0] & 0x80) ? ~0ull : 0ull, lo = hi;
@@ -507,8 +498,6 @@ void launch_pq_plain(const PqPage* pages, int n_pages, int conv, int flba_len, v
     case PQ_COPY32: k_pq_plain<PQ_COPY32><<<grid, block, 0, st>>>(pages, flba_len, (u8*)out, err); break;
     case PQ_COPY64: k_pq_plain<PQ_COPY64><<<grid, block, 0, st>>>(pages, flba_len, (u8*)out, err); break;
     case PQ_I32_TO_I64: k_pq_plain<PQ_I32_TO_I64><<<grid, block, 0, st>>>(pages, flba_len, (u8*)out, err); break;
-    case PQ_I64_TO_I128: k_pq_plain<PQ_I64_TO_I128><<<grid, block, 0, st>>>(pages, flba_len, (u8*)out, err); break;
-    case PQ_I32_TO_I128: k_pq_plain<PQ_I32_TO_I128><<<grid, block, 0, st>>>(pages, flba_len, (u8*)out, err); break;
     case PQ_FLBA_TO_I64: k_pq_plain<PQ_FLBA_TO_I64><<<grid, block, 0, st>>>(pages, flba_len, (u8*)out, err); break;
     default: k_pq_plain<PQ_FLBA_TO_I128><<<grid, block, 0, st>>>(pages, flba_len, (u8*)out, err); break;
     }
@@ -578,8 +567,8 @@ template <bool LEVELS> __global__ void k_pq_rle_scan(const PqPage* pages, int n_
         n++;
         row += count;
     });
-    if (n > cap || seen != want) atomicOr(err, 1);
-    if (truncated) atomicOr(err, 16);
+    if (n > cap || seen != want) atomicOr(err, PQ_ERR_RLE);
+    if (truncated) atomicOr(err, PQ_ERR_TRUNCATED);
     run_counts[pi] = n < cap ? n : cap;
 }
 void launch_pq_rle_scan(const PqPage* pages, int n_pages, PqRun* runs, int* run_counts, int* err, cudaStream_t st) {
@@ -587,7 +576,7 @@ void launch_pq_rle_scan(const PqPage* pages, int n_pages, PqRun* runs, int* run_
 }
 
 template <int DW> __device__ __forceinline__ void store_dict(const void* dict, int dict_size, u32 idx, void* out, long long row, int* err) {
-    if ((int)idx >= dict_size) { atomicOr(err, 4); idx = 0; }
+    if ((int)idx >= dict_size) { atomicOr(err, PQ_ERR_DICT_INDEX); idx = 0; }
     if (DW == 4) ((u32*)out)[row] = ((const u32*)dict)[idx];
     else if (DW == 8) ((u64*)out)[row] = ((const u64*)dict)[idx];
     else ((ulonglong2*)out)[row] = ((const ulonglong2*)dict)[idx];
@@ -643,8 +632,8 @@ __global__ void k_pq_check_def(const PqPage* pages, int n_pages, int* err) {
         if (!packed) { if (value != 1u) bad = true; }
         else for (int i = 0; i < count && data + (i >> 3) < end; i++) if (!((data[i >> 3] >> (i & 7)) & 1)) { bad = true; break; }
     });
-    if (bad) atomicOr(err, 2);
-    if (seen != pg.num_values) atomicOr(err, 1);
+    if (bad) atomicOr(err, PQ_ERR_NULL_ON_FAST_PATH);
+    if (seen != pg.num_values) atomicOr(err, PQ_ERR_RLE);
 }
 void launch_pq_check_def_levels(const PqPage* pages, int n_pages, int* err, cudaStream_t st) {
     if (n_pages > 0) k_pq_check_def<<<(n_pages + 63) / 64, 64, 0, st>>>(pages, n_pages, err);

@@ -1,61 +1,18 @@
 // parquet_kernels.h -- device-side Parquet page decode: Snappy decompression, PLAIN, RLE_DICTIONARY, definition
 // levels (validity + NULL scatter).
 #pragma once
+#include "parquet_pages.h"
+
 #include <cuda_runtime.h>
-#include <cstdint>
+#include <cstddef>
 
 namespace cb200 {
-
-// PqPage::flags.  V1_LEVELS: body starts with [u32 byte length][RLE definition levels] (DataPage v1 of an optional column).  SN_*: set by the
-// Snappy index / segment kernels (the page needs the serial decoder / is malformed).  HOSTDEC (host bookkeeping only): the body was produced
-// on the host -- decompressed (csrc/host_codecs.h) or PLAIN strings turned into dictionary codes -- and travels with the page tables.
-enum { PQ_PAGE_V1_LEVELS = 1, PQ_PAGE_SN_SERIAL = 2, PQ_PAGE_SN_BAD = 4, PQ_PAGE_HOSTDEC = 8 };
-
-// One page of a column chunk resident on the device.  The host fills what the page HEADER tells it; everything
-// that lives inside the (possibly compressed) page body is resolved on the device by k_pq_resolve.
-struct PqPage {
-    unsigned char* body;          // v1: page body (levels + values); v2: the values section.  Snappy pages: where the decompressor writes
-    int body_bytes;               // uncompressed size of `body`
-    const unsigned char* comp;    // Snappy-compressed source, nullptr when `body` already holds the bytes
-    int comp_bytes;
-    int flags;
-    const unsigned char* def_ptr; // definition levels (RLE/bit-packed hybrid, bit width 1); v2: set by the host
-    int def_bytes;
-    const unsigned char* values;  // resolved: encoded values (non-null values only)
-    int values_bytes;
-    long long dst_row;            // first output row of this page
-    int num_values;               // rows of the page (incl. NULLs)
-    int nonnull;                  // resolved: encoded values present
-    int encoding;                 // 0 PLAIN, 8 RLE_DICTIONARY (2 PLAIN_DICTIONARY is the same on the wire)
-    long long run_base;           // value runs: first entry of this page in the run table, capacity
-    int max_runs;
-    long long def_run_base;       // definition-level runs (NULL-aware path)
-    int def_max_runs;
-    long long dict_off;           // element offset of this page's dictionary inside the column's combined dictionary buffer
-    int dict_size;
-    int seg_base;                 // Snappy pages: first entry of this page in the column's checkpoint table (one entry per 64 KB of output)
-    int n_segs;
-};
-
-struct PqRun {              // one run of the RLE / bit-packed hybrid
-    long long out_row;      // absolute output row of the run's first value
-    const unsigned char* src; // packed data (bit-packed runs)
-    int count;              // values in the run
-    unsigned value;         // RLE runs: the repeated value
-    int bit_packed;
-    int bit_width;
-};
-
-enum PqConv { PQ_COPY32, PQ_COPY64, PQ_I32_TO_I64, PQ_FLBA_TO_I64, PQ_FLBA_TO_I128, PQ_I64_TO_I128, PQ_I32_TO_I128 };
-// err bits: 1 malformed / pathological RLE stream, 2 NULL found on the no-NULL fast path, 4 dictionary index out of range, 8 malformed Snappy page, 16 truncated page (fewer encoded values than the header declares)
 
 // dst[0, bytes) = src[0, bytes) with SM loads/stores (bytes a multiple of 16, both 16-byte aligned).  `src` may be mapped pinned
 // host memory: small tables reach the device without queueing on a copy engine.
 void launch_pq_copy(void* dst, const void* src, size_t bytes, cudaStream_t st);
-// Snappy: one warp per compressed page (pages with comp == nullptr are skipped)
-void launch_pq_snappy(PqPage* pages_dev, int n_pages, int* err, cudaStream_t st);
-// segmented decoder: `ckpt` has room for n_segs_total entries (sum of PqPage::n_segs, n_segs = ceil(body_bytes / PQ_SNAPPY_SEG))
-constexpr int PQ_SNAPPY_SEG = 65536;
+// Snappy, segmented: `ckpt` has room for n_segs_total entries (sum of PqPage::n_segs, n_segs = ceil(body_bytes / PQ_SNAPPY_SEG)); pages
+// with comp == nullptr are skipped
 void launch_pq_snappy_segmented(PqPage* pages_dev, int n_pages, unsigned* ckpt_dev, int n_segs_total, int* err, cudaStream_t st);
 // locate levels / values inside every page body; nonnull = num_values
 void launch_pq_resolve(PqPage* pages_dev, int n_pages, cudaStream_t st);
@@ -67,7 +24,7 @@ void launch_pq_rle_scan(const PqPage* pages_dev, int n_pages, PqRun* runs, int* 
 void launch_pq_rle_decode(const PqPage* pages_dev, int n_pages, const PqRun* runs, const int* run_counts, const void* dict, int dict_width, void* out, int* err,
                           cudaStream_t st);
 // definition levels of flat optional columns (max level 1)
-//   fast path (statistics promise no NULLs): verify it (err bit 2 otherwise)
+//   fast path (statistics promise no NULLs): verify it (PQ_ERR_NULL_ON_FAST_PATH otherwise)
 void launch_pq_check_def_levels(const PqPage* pages_dev, int n_pages, int* err, cudaStream_t st);
 //   NULL-aware path: valid[row] = level, idx[row] = dst_row(page) + number of non-null rows before `row` in its page, pages[].nonnull
 void launch_pq_def_levels(PqPage* pages_dev, int n_pages, PqRun* runs, int* run_counts, unsigned char* valid, unsigned* idx, int* err, cudaStream_t st);

@@ -1,8 +1,8 @@
 // scan_parquet.cpp -- native Parquet scan (NativeScan -> DataSourceExec(ParquetSource),
-// native/core/src/parquet/parquet_exec.rs:60-200).
+// native/core/src/parquet/parquet_exec.rs:60-200): the device pipeline over the host plans of scan_plan.cpp.
 //
-// Footers and page headers are parsed on the host (parquet.cpp); encoded pages cross PCIe as they sit in the file and every
-// value byte is decoded on the device (parquet_kernels.cu).  d(p<=18) / INT64 decimals stay 8 bytes wide in HBM (the Parquet
+// Footers and page headers are parsed on the host (parquet.cpp, scan_plan.cpp); encoded pages cross PCIe as they sit in the file and
+// every value byte is decoded on the device (parquet_kernels.cu).  d(p<=18) / INT64 decimals stay 8 bytes wide in HBM (the Parquet
 // physical width) and the fused kernels read them as such.
 //
 // Memory.  A scan owns two SLOTS that alternate between consecutive batches, so that batch k+1's encoded bytes cross PCIe
@@ -17,56 +17,16 @@
 // framework that holds most of HBM -- the end-to-end step time was hostage to it.)
 #include "exec.h"
 
-#include "device/cb_snappy.h"
-#include "parquet.h"
 #include "parquet_kernels.h"
-#include "host_codecs.h"
+#include "scan_plan.h"
 
 #include <algorithm>
 #include <cstdlib>
 #include <cstring>
 #include <map>
 #include <mutex>
-#include <unordered_map>
 
 namespace cb200 {
-
-// =================================================================================================
-// memory files
-// =================================================================================================
-static std::mutex g_memfile_mu;
-static std::map<std::string, std::pair<const uint8_t*, size_t>> g_memfiles;
-void register_memory_file(const std::string& name, const uint8_t* p, size_t n) {
-    std::lock_guard<std::mutex> lk(g_memfile_mu);
-    if (p) g_memfiles[name] = {p, n};
-    else g_memfiles.erase(name);
-}
-static bool lookup_memory_file(const std::string& path, const uint8_t** p, size_t* n) {
-    const std::string pre = "memory://";
-    if (path.compare(0, pre.size(), pre) != 0) return false;
-    std::lock_guard<std::mutex> lk(g_memfile_mu);
-    auto it = g_memfiles.find(path.substr(pre.size()));
-    if (it == g_memfiles.end()) throw ExecError(3, "", "parquet: memory file '" + path + "' is not registered");
-    *p = it->second.first;
-    *n = it->second.second;
-    return true;
-}
-static std::string strip_file_scheme(const std::string& p) { return p.compare(0, 7, "file://") == 0 ? p.substr(7) : p; }
-
-static pq::FileMeta open_parquet(const std::string& path, const uint8_t** mem, size_t* mem_len) {
-    *mem = nullptr;
-    *mem_len = 0;
-    if (lookup_memory_file(path, mem, mem_len)) return pq::parse_footer(*mem, *mem_len);
-    int64_t sz = 0;
-    return pq::read_footer(strip_file_scheme(path), &sz);
-}
-
-std::string describe_parquet(const std::string& path) {
-    const uint8_t* mem;
-    size_t len;
-    pq::FileMeta m = open_parquet(path, &mem, &len);
-    return pq::describe(m);
-}
 
 // =================================================================================================
 // block cache: device / pinned blocks survive their scan and are handed to the next one
@@ -185,99 +145,6 @@ void release_res(int device, const ScanRes& r) {
     g_res_pool[device].push_back(r);
 }
 
-size_t align_up(size_t n, size_t a) { return (n + a - 1) / a * a; }
-
-// ---- conjuncts `column <op> literal` of the pushed-down filters, evaluated against chunk statistics --------------------------
-// (parquet_exec.rs:143-196: the reference builds a pruning predicate from the same data_filters; row groups whose
-//  min/max statistics prove that no row can pass are never read.)
-struct PruneTerm {
-    int col;          // index into required_schema
-    ExprKind op;      // Eq, Lt, LtEq, Gt, GtEq (column on the left), IsNotNull
-    bool is_float = false;
-    __int128 ival = 0;
-    double fval = 0;
-};
-
-void collect_prune_terms(const ExprP& e, std::vector<PruneTerm>& out) {
-    if (e->kind == ExprKind::And) {
-        for (auto& c : e->children) collect_prune_terms(c, out);
-        return;
-    }
-    if (e->kind == ExprKind::IsNotNull && e->children[0]->kind == ExprKind::Bound) {
-        PruneTerm t;
-        t.col = e->children[0]->index;
-        t.op = ExprKind::IsNotNull;
-        out.push_back(t);
-        return;
-    }
-    ExprKind k = e->kind;
-    if (!(k == ExprKind::Eq || k == ExprKind::Lt || k == ExprKind::LtEq || k == ExprKind::Gt || k == ExprKind::GtEq)) return;
-    const Expr *l = e->children[0].get(), *r = e->children[1].get();
-    if (l->kind == ExprKind::Literal && r->kind == ExprKind::Bound) { // literal <op> column: mirror
-        std::swap(l, r);
-        k = k == ExprKind::Lt ? ExprKind::Gt : k == ExprKind::LtEq ? ExprKind::GtEq : k == ExprKind::Gt ? ExprKind::Lt : k == ExprKind::GtEq ? ExprKind::LtEq : k;
-    }
-    if (l->kind != ExprKind::Bound || r->kind != ExprKind::Literal || r->lit_null) return;
-    PruneTerm t;
-    t.col = l->index;
-    t.op = k;
-    const DType& ty = l->type;
-    if (ty.is_integer() || ty.id == TypeId::Date || ty.id == TypeId::Timestamp || ty.id == TypeId::TimestampNtz) t.ival = r->lit_i64;
-    else if (ty.is_decimal() && r->type.is_decimal() && r->type.scale == ty.scale) t.ival = (__int128)r->lit_dec;
-    else if (ty.id == TypeId::Float64 || ty.id == TypeId::Float32) { t.is_float = true; t.fval = r->lit_f64; if (t.fval != t.fval) return; }
-    else return;
-    out.push_back(t);
-}
-
-// decode a statistics value (PLAIN-encoded single value) of a leaf; false = cannot use it
-bool stat_value(const pq::SchemaElement& se, const std::string& raw, bool* is_float, __int128* iv, double* fv) {
-    *is_float = false;
-    switch (se.type) {
-    case pq::INT32: { if (raw.size() != 4) return false; int32_t v; memcpy(&v, raw.data(), 4); *iv = v; return true; }
-    case pq::INT64: { if (raw.size() != 8) return false; int64_t v; memcpy(&v, raw.data(), 8); *iv = v; return true; }
-    case pq::FLOAT: { if (raw.size() != 4) return false; float v; memcpy(&v, raw.data(), 4); *is_float = true; *fv = v; return v == v; }
-    case pq::DOUBLE: { if (raw.size() != 8) return false; double v; memcpy(&v, raw.data(), 8); *is_float = true; *fv = v; return v == v; }
-    case pq::FIXED_LEN_BYTE_ARRAY: { // big-endian two's complement decimal
-        if (raw.empty() || raw.size() > 16) return false;
-        __int128 v = (signed char)raw[0] < 0 ? -1 : 0;
-        for (unsigned char ch : raw) v = (v << 8) | ch;
-        *iv = v;
-        return true;
-    }
-    default: return false;
-    }
-}
-
-// true = the statistics prove that no row of the chunk satisfies the term
-bool term_excludes(const PruneTerm& t, const pq::SchemaElement& se, const pq::ColumnChunkMeta& cc) {
-    if (t.op == ExprKind::IsNotNull) return cc.null_count >= 0 && cc.null_count == cc.num_values && cc.num_values > 0;
-    if (!cc.has_min_max) return false;
-    bool fmin, fmax;
-    __int128 imin = 0, imax = 0;
-    double dmin = 0, dmax = 0;
-    if (!stat_value(se, cc.min_value, &fmin, &imin, &dmin) || !stat_value(se, cc.max_value, &fmax, &imax, &dmax)) return false;
-    if (fmin != t.is_float) return false;
-    if (t.is_float) {
-        // float statistics may be written with -0.0 / +0.0 either way; comparisons below treat them as equal, which is safe
-        switch (t.op) {
-        case ExprKind::Eq: return t.fval < dmin || t.fval > dmax;
-        case ExprKind::Lt: return !(dmin < t.fval);
-        case ExprKind::LtEq: return !(dmin <= t.fval);
-        case ExprKind::Gt: return !(dmax > t.fval);
-        case ExprKind::GtEq: return !(dmax >= t.fval);
-        default: return false;
-        }
-    }
-    switch (t.op) {
-    case ExprKind::Eq: return t.ival < imin || t.ival > imax;
-    case ExprKind::Lt: return !(imin < t.ival);
-    case ExprKind::LtEq: return !(imin <= t.ival);
-    case ExprKind::Gt: return !(imax > t.ival);
-    case ExprKind::GtEq: return !(imax >= t.ival);
-    default: return false;
-    }
-}
-
 } // namespace
 
 // =================================================================================================
@@ -290,50 +157,24 @@ struct NativeScanSource : ExecNode {
     std::vector<StructField> fields;
     std::vector<ExprP> data_filters;
 
-    struct OpenFile {
-        pq::FileMeta meta;
-        const uint8_t* mem = nullptr;
-        size_t mem_len = 0;
-        FILE* fh = nullptr;
-        std::vector<int> leaf_of; // per output column: leaf index in this file
-    };
-    struct Unit { size_t file, rg; int64_t rows, row0; };
-    struct ChunkLoc { const uint8_t* host; unsigned char* dev; }; // one column chunk of a batch: its bytes on the host and where they land on the device
-    std::vector<OpenFile> open_files;
+    std::vector<ScanFile> open_files;
+    std::vector<FILE*> fh;                  // per file: its handle when the bytes are read from disk
     std::vector<Unit> all_units;
-    std::vector<std::pair<size_t, size_t>> batches; // [first unit, end unit) of every batch
+    BatchPlan plan;
     size_t next_batch = 0;
     bool opened = false;
-    std::vector<DictionaryP> dicts;
-    std::vector<std::unordered_map<std::string, int32_t>> dict_index; // value -> code of dicts[c] (PLAIN string pages: one lookup per row)
-    int64_t pruned_row_groups = 0, pruned_rows = 0;
+    std::vector<StringInterner> strings;    // per column
 
     struct Slot {
         ScanBlockP chunk, work, meta, staging;
         size_t work_used = 0, meta_used = 0;
         bool used = false;
+        uint8_t* meta_dev = nullptr;        // the current batch's device mirror of the pinned page tables (in the work block)
+        int* derr = nullptr;                // the current batch's decode error bits (PqErr)
     };
     Slot slots[2];
     ScanRes res;
     bool have_res = false;
-    size_t chunk_need = 0, work_estimate = 0; // per slot, from the footers
-
-    // host-side description of one column of one batch (phase A), then its device buffers (phase B)
-    struct ColPlan {
-        int conv = 0, out_w = 0, type_length = 0, phys_type = 0;
-        std::vector<PqPage> pages;   // data pages, then fixed-width dictionary pages
-        size_t n_data = 0, n_dict_pages = 0;
-        std::vector<int32_t> remap;  // string columns: combined code remap tables
-        int64_t run_base = 0, def_run_base = 0, dict_elems = 0;
-        size_t unc_bytes = 0;
-        int64_t n_segs_total = 0;    // Snappy: 64 KB output segments over all compressed pages (checkpoint table entries)
-        std::vector<uint8_t> hostdec; // bodies of the pages decompressed on the host (ZSTD / LZ4 / GZIP), 16-byte aligned each; shipped with the page tables
-        bool optional = false, null_aware = false, any_compressed = false;
-        // device buffers (offsets into the slot's work block while planning, pointers after bind)
-        uint8_t *out = nullptr, *dunc = nullptr, *dpd = nullptr, *ddict = nullptr, *dense = nullptr, *dvalid = nullptr, *didx = nullptr, *druns = nullptr,
-                *dcounts = nullptr, *validity = nullptr, *runs = nullptr, *counts = nullptr, *dckpt = nullptr;
-        size_t out_bytes = 0, validity_bytes = 0;
-    };
 
     struct Prepared {
         Batch batch;
@@ -343,7 +184,6 @@ struct NativeScanSource : ExecNode {
     };
     std::unique_ptr<Prepared> pending;
     int64_t n_issued = 0;
-    double t_pages = 0, t_h2d = 0, t_launch = 0; // CB200_TRACE: host milliseconds per issue()
 
     void push_filters(const std::vector<ExprP>& preds) override {
         if (!opened) for (auto& p : preds) data_filters.push_back(p);
@@ -356,12 +196,7 @@ struct NativeScanSource : ExecNode {
             release_res(ctx->device, res);
         }
         pending.reset();
-        for (auto& f : open_files) if (f.fh) fclose(f.fh);
-    }
-
-    const pq::ColumnChunkMeta& chunk_meta(const Unit& u, size_t c) const {
-        const OpenFile& f = open_files[u.file];
-        return f.meta.row_groups[u.rg].columns[(size_t)f.leaf_of[c]];
+        for (FILE* f : fh) if (f) fclose(f);
     }
 
     // ---- open: footers, pruning, batch plan, block sizes ---------------------------------------------------------------------
@@ -370,95 +205,20 @@ struct NativeScanSource : ExecNode {
         std::vector<PruneTerm> terms;
         const bool prune = getenv("CB200_NO_PRUNE") ? atoi(getenv("CB200_NO_PRUNE")) == 0 : true;
         if (prune) for (auto& f : data_filters) collect_prune_terms(f, terms);
-        for (size_t fi = 0; fi < files.size(); fi++) {
-            const std::string& path = files[fi];
-            OpenFile of;
-            of.meta = open_parquet(path, &of.mem, &of.mem_len);
-            if (!of.mem) {
-                of.fh = fopen(strip_file_scheme(path).c_str(), "rb");
-                if (!of.fh) throw ExecError(3, "", "parquet: cannot open " + path);
-            }
-            for (auto& f : fields) {
-                int li = of.meta.leaf_index(f.name);
-                if (li < 0) throw Unsupported("parquet: column '" + f.name + "' missing from " + path + " (schema evolution / default values are out of scope)");
-                of.leaf_of.push_back(li);
-            }
-            const int64_t r0 = fi < file_start.size() ? file_start[fi] : 0, rl = fi < file_length.size() ? file_length[fi] : 0;
-            for (size_t g = 0; g < of.meta.row_groups.size(); g++) {
-                const pq::RowGroupMeta& rg = of.meta.row_groups[g];
-                if (rg.num_rows <= 0 || rg.columns.empty()) continue;
-                if (rl > 0) { // a file split owns the row groups that START inside it (DataFusion's range rule for ParquetSource)
-                    const int64_t off = rg.columns[0].start();
-                    if (off < r0 || off >= r0 + rl) continue;
-                }
-                bool excluded = false;
-                for (auto& t : terms) {
-                    if (t.col < 0 || t.col >= (int)fields.size()) continue;
-                    const int leaf = of.leaf_of[(size_t)t.col];
-                    if (term_excludes(t, of.meta.leaf(leaf), rg.columns[(size_t)leaf])) { excluded = true; break; }
-                }
-                if (excluded) { pruned_row_groups++; pruned_rows += rg.num_rows; continue; }
-                all_units.push_back({open_files.size(), g, rg.num_rows, 0});
-            }
-            open_files.push_back(std::move(of));
+        for (auto& path : files) {
+            open_files.push_back(open_scan_file(path, fields));
+            fh.push_back(open_files.back().mem ? nullptr : fopen(strip_file_scheme(path).c_str(), "rb"));
+            if (!open_files.back().mem && !fh.back()) throw ExecError(3, "", "parquet: cannot open " + path);
         }
-        dicts.assign(fields.size(), nullptr);
-        plan_batches();
+        Selection sel = select_row_groups(open_files, file_start, file_length, fields.size(), terms);
+        all_units = std::move(sel.units);
+        strings.resize(fields.size());
+        plan = plan_batches(all_units, open_files, fields, ctx->chunk_rows);
         if (trace_on()) fprintf(stderr, "[cb200 trace]   parquet scan: %zu row groups in %zu batches (%lld pruned by statistics), chunk block %.1f MB, work block %.1f MB per slot\n",
-                                all_units.size(), batches.size(), (long long)pruned_row_groups, chunk_need / 1e6, work_estimate / 1e6);
-        ctx->scan_pruned_row_groups += pruned_row_groups;
-        ctx->scan_pruned_rows += pruned_rows;
+                                all_units.size(), plan.batches.size(), (long long)sel.pruned_row_groups, plan.chunk_need / 1e6, plan.work_estimate / 1e6);
+        ctx->scan_pruned_row_groups += sel.pruned_row_groups;
+        ctx->scan_pruned_rows += sel.pruned_rows;
         opened = true;
-    }
-
-    void plan_batches() {
-        // greedy fill up to chunk_rows; the FIRST batch is a sixteenth of that: nothing overlaps its upload, so it should be short
-        // (the blocks are sized for the largest batch, so batches of different sizes cost nothing)
-        static const bool ramp = getenv("CB200_SCAN_RAMP") ? atoi(getenv("CB200_SCAN_RAMP")) != 0 : true;
-        size_t u = 0;
-        int64_t total_rows = 0;
-        for (auto& x : all_units) total_rows += x.rows;
-        while (u < all_units.size()) {
-            int64_t cap = ctx->chunk_rows;
-            if (ramp && batches.empty() && total_rows > 2 * ctx->chunk_rows) cap = std::max<int64_t>(ctx->chunk_rows / 16, 1);
-            size_t e = u;
-            int64_t rows = 0;
-            while (e < all_units.size() && (e == u || rows + all_units[e].rows <= cap)) rows += all_units[e++].rows;
-            batches.push_back({u, e});
-            u = e;
-        }
-        // block sizes: encoded bytes exactly (from the chunk metadata), decoded bytes + temporaries as an estimate that
-        // bind() re-checks (a slot grows once if the estimate was short)
-        for (auto& b : batches) {
-            size_t enc = 0, work = 4096;
-            int64_t rows = 0;
-            for (size_t i = b.first; i < b.second; i++) rows += all_units[i].rows;
-            for (size_t i = b.first; i < b.second; i++) {
-                for (size_t c = 0; c < fields.size(); c++) {
-                    const pq::ColumnChunkMeta& cc = chunk_meta(all_units[i], c);
-                    enc += align_up((size_t)std::max<int64_t>(cc.total_compressed, 0), 256) + 256;
-                    if (cc.codec != pq::UNCOMPRESSED) work += (size_t)std::max<int64_t>(cc.total_uncompressed, 0) + 64 * 1024;
-                }
-            }
-            for (size_t c = 0; c < fields.size(); c++) {
-                const DType& t = fields[c].type;
-                const size_t w = t.is_decimal() ? (t.precision <= 18 ? 8 : 16) : t.is_string() ? 4 : (size_t)std::max(t.arrow_width(), 1);
-                bool nulls = false;
-                for (size_t i = b.first; i < b.second; i++) {
-                    const OpenFile& of = open_files[all_units[i].file];
-                    if (of.meta.leaf(of.leaf_of[c]).repetition == 1 && chunk_meta(all_units[i], c).null_count != 0) nulls = true;
-                }
-                bool dict_encoded = false;
-                for (size_t i = b.first; i < b.second && !dict_encoded; i++)
-                    for (int enc : chunk_meta(all_units[i], c).encodings) if (enc == pq::RLE_DICTIONARY || enc == pq::PLAIN_DICTIONARY) dict_encoded = true;
-                work += (size_t)rows * w + 4096;                                  // decoded column
-                work += (b.second - b.first) * 96 * 1024;                         // page tables / dictionaries
-                if (dict_encoded) work += (size_t)rows * 4 + (b.second - b.first) * 16 * 2048; // run table: (values / 8 + 64) runs of 32 bytes per page
-                if (nulls) work += (size_t)rows * (w + 5 + 4) + 65536;            // dense values + validity bytes + indices + level runs
-            }
-            chunk_need = std::max(chunk_need, enc + 65536);
-            work_estimate = std::max(work_estimate, work + work / 16);
-        }
     }
 
     void ensure_resources() {
@@ -468,8 +228,8 @@ struct NativeScanSource : ExecNode {
         // a cached block may have been released by another plan whose last kernels are still in flight on ITS stream
         cuda_check(cudaDeviceSynchronize(), "scan start sync");
         for (auto& sl : slots) {
-            sl.chunk = block_cache().acquire(ctx->device, false, chunk_need);
-            sl.work = block_cache().acquire(ctx->device, false, work_estimate);
+            sl.chunk = block_cache().acquire(ctx->device, false, plan.chunk_need);
+            sl.work = block_cache().acquire(ctx->device, false, plan.work_estimate);
             sl.meta = block_cache().acquire(ctx->device, true, (size_t)4 << 20);
         }
     }
@@ -484,57 +244,53 @@ struct NativeScanSource : ExecNode {
 
     // ---- one batch ----------------------------------------------------------------------------------------------------------------
     std::unique_ptr<Prepared> issue() {
-        if (next_batch >= batches.size()) return nullptr;
+        if (next_batch >= plan.batches.size()) return nullptr;
         TraceSpan ts("parquet.issue");
         ensure_resources();
         auto pr = std::make_unique<Prepared>();
         pr->slot = (int)(n_issued++ & 1);
         const int si = pr->slot;
         Slot& sl = slots[si];
-        std::vector<Unit> units;
-        int64_t total = 0;
-        for (size_t i = batches[next_batch].first; i < batches[next_batch].second; i++) {
-            Unit u = all_units[i];
-            u.row0 = total;
-            total += u.rows;
-            units.push_back(u);
-        }
-        next_batch++;
+        const std::vector<Unit> units = batch_units(all_units, plan.batches[next_batch++]);
+        const int64_t total = units.back().row0 + units.back().rows;
         Batch& out = pr->batch;
         out.n_rows = total;
-        out.cols.clear();
-        out.cols.resize(fields.size());
-        // Upload plan: per row group, the selected column chunks sorted by file offset and merged into byte ranges (gaps of
-        // unselected columns up to 64 KB ride along) -- PCIe moves few large copies faster than many chunk-sized ones
-        // (measured: 49 GB/s at 1.8 MB per copy, 54 GB/s at 12 MB).
-        struct Range { size_t file; int64_t start, end; size_t dev_off; };
-        std::vector<Range> ranges;
-        std::vector<std::vector<ChunkLoc>> loc(fields.size(), std::vector<ChunkLoc>(units.size()));
-        std::vector<std::vector<size_t>> range_of(fields.size(), std::vector<size_t>(units.size(), 0));
-        bool any_file = false;
-        for (size_t u = 0; u < units.size(); u++) {
-            const OpenFile& of = open_files[units[u].file];
-            if (!of.mem) any_file = true;
-            std::vector<std::pair<int64_t, size_t>> items; // (file offset, column)
-            for (size_t c = 0; c < fields.size(); c++) {
-                const pq::ColumnChunkMeta& cc = chunk_meta(units[u], c);
-                if (cc.total_compressed < 0 || cc.start() < 0) throw PlanError("parquet: negative column chunk offset / size");
-                if (of.mem && (size_t)cc.start() + (size_t)cc.total_compressed > of.mem_len) throw PlanError("parquet: column chunk beyond the end of the file image");
-                items.push_back({cc.start(), c});
-            }
-            std::sort(items.begin(), items.end());
-            bool open_range = false;
-            for (auto& it : items) {
-                const int64_t st0 = it.first, en0 = st0 + chunk_meta(units[u], it.second).total_compressed;
-                if (open_range && st0 >= ranges.back().end && st0 - ranges.back().end <= 65536) ranges.back().end = std::max(ranges.back().end, en0);
-                else if (open_range && st0 < ranges.back().end) ranges.back().end = std::max(ranges.back().end, en0); // overlapping chunks (same column projected twice)
-                else { ranges.push_back({units[u].file, st0, en0, 0}); open_range = true; }
-                range_of[it.second][u] = ranges.size() - 1;
-            }
+        out.cols.assign(fields.size(), Column());
+        const UploadPlan up = plan_uploads(units, open_files, fields.size());
+        reuse_slot(si, up);
+        if (trace_on()) {
+            for (auto& e : pr->tr) cuda_check(cudaEventCreate(&e), "event");
+            cuda_check(cudaEventRecord(pr->tr[0], res.copy_stream), "event record");
+            cuda_check(cudaEventRecord(pr->tr[2], res.decode_stream), "event record");
         }
-        size_t dev_total = 0;
-        for (auto& r : ranges) { r.dev_off = dev_total; dev_total += align_up((size_t)(r.end - r.start), 256); }
-        // ---- slot reuse: everything queued on this slot two batches ago must be done with its blocks --------------------------
+        double tt = now_ms();
+        const std::vector<std::vector<ChunkLoc>> loc = upload(up, si);
+        const double t_h2d = now_ms() - tt;
+        // phase A: page tables on the host (reads only page headers)
+        tt = now_ms();
+        std::vector<ColPlan> plans;
+        for (size_t c = 0; c < fields.size(); c++) plans.push_back(plan_column(open_files, fields[c], c, units, total, loc[c], strings[c]));
+        bind_buffers(plans, total, sl);
+        const double t_pages = now_ms() - tt;
+        // phase B: decode kernels
+        tt = now_ms();
+        launch(plans, total, out, si);
+        const double t_launch = now_ms() - tt;
+        if (trace_on()) fprintf(stderr, "[cb200 trace]   issue breakdown: h2d enqueue (%zu ranges) %.3f  page tables %.3f  launches %.3f ms; work %.1f MB\n", up.ranges.size(), t_h2d, t_pages, t_launch, sl.work_used / 1e6);
+        cuda_check(cudaEventRecord(res.decoded[si], res.decode_stream), "event record");
+        if (trace_on()) {
+            cuda_check(cudaEventRecord(pr->tr[1], res.copy_stream), "event record");
+            cuda_check(cudaEventRecord(pr->tr[3], res.decode_stream), "event record");
+        }
+        sl.used = true;
+        cuda_check(cudaMemcpyAsync(&res.h_flags[si], sl.derr, 4, cudaMemcpyDeviceToHost, res.decode_stream), "parquet err");
+        cuda_check(cudaEventRecord(res.done[si], res.decode_stream), "event record");
+        return pr;
+    }
+
+    // everything queued on the slot two batches ago must be done with its blocks; the chunk / staging blocks must hold this batch
+    void reuse_slot(int si, const UploadPlan& up) {
+        Slot& sl = slots[si];
         if (sl.used) {
             cuda_check(cudaEventSynchronize(res.decoded[si]), "slot reuse"); // page tables / staging on the host side; long done (two batches back)
             cuda_check(cudaStreamWaitEvent(res.copy_stream, res.decoded[si], 0), "stream wait");
@@ -543,56 +299,50 @@ struct NativeScanSource : ExecNode {
         // when it is finished with batch k-1): order the decode stream behind them
         cuda_check(cudaEventRecord(res.consumer, ctx->stream), "event record");
         cuda_check(cudaStreamWaitEvent(res.decode_stream, res.consumer, 0), "stream wait");
-        if (dev_total + 64 > sl.chunk->cap) { // cannot happen when the footers are honest; grow rather than fail
+        if (up.dev_total + 64 > sl.chunk->cap) { // cannot happen when the footers are honest; grow rather than fail
             cuda_check(cudaStreamSynchronize(res.copy_stream), "chunk growth");
-            sl.chunk = block_cache().acquire(ctx->device, false, dev_total + dev_total / 8 + 65536);
+            sl.chunk = block_cache().acquire(ctx->device, false, up.dev_total + up.dev_total / 8 + 65536);
         }
-        if (any_file) {
-            if (!sl.staging || sl.staging->cap < dev_total) sl.staging = block_cache().acquire(ctx->device, true, dev_total + dev_total / 8);
-        }
+        bool any_file = false;
+        for (auto& r : up.ranges) if (!open_files[r.file].mem) any_file = true;
+        if (any_file && (!sl.staging || sl.staging->cap < up.dev_total)) sl.staging = block_cache().acquire(ctx->device, true, up.dev_total + up.dev_total / 8);
         sl.meta_used = 0;
         sl.work_used = 0;
-        t_pages = t_h2d = t_launch = 0;
-        if (trace_on()) {
-            for (auto& e : pr->tr) cuda_check(cudaEventCreate(&e), "event");
-            cuda_check(cudaEventRecord(pr->tr[0], res.copy_stream), "event record");
-            cuda_check(cudaEventRecord(pr->tr[2], res.decode_stream), "event record");
-        }
-        double tt = now_ms();
-        for (auto& r : ranges) {
-            const OpenFile& of = open_files[r.file];
+    }
+
+    // the batch's byte ranges onto the copy stream (ranges of files on disk are read into the pinned staging block first);
+    // returns where every column chunk sits, [column][unit]
+    std::vector<std::vector<ChunkLoc>> upload(const UploadPlan& up, int si) {
+        Slot& sl = slots[si];
+        auto host_of = [&](const UploadRange& r) -> const uint8_t* {
+            const ScanFile& f = open_files[r.file];
+            return f.mem ? f.mem + r.start : sl.staging->ptr + r.dev_off;
+        };
+        for (auto& r : up.ranges) {
             const size_t len = (size_t)(r.end - r.start);
-            const uint8_t* host;
-            if (of.mem) host = of.mem + r.start;
-            else {
-                uint8_t* dst = sl.staging->ptr + r.dev_off;
-                if (fseeko(of.fh, (off_t)r.start, SEEK_SET) != 0 || fread(dst, 1, len, of.fh) != len) throw ExecError(3, "", "parquet: short read");
-                host = dst;
-            }
-            cuda_check(cudaMemcpyAsync(sl.chunk->ptr + r.dev_off, host, len, cudaMemcpyHostToDevice, res.copy_stream), "H2D parquet range");
+            FILE* f = fh[r.file];
+            if (f && (fseeko(f, (off_t)r.start, SEEK_SET) != 0 || fread(sl.staging->ptr + r.dev_off, 1, len, f) != len)) throw ExecError(3, "", "parquet: short read");
+            cuda_check(cudaMemcpyAsync(sl.chunk->ptr + r.dev_off, host_of(r), len, cudaMemcpyHostToDevice, res.copy_stream), "H2D parquet range");
             ctx->h2d_bytes += (int64_t)len;
         }
         cuda_check(cudaEventRecord(res.uploaded[si], res.copy_stream), "event record");
+        std::vector<std::vector<ChunkLoc>> loc(fields.size());
         for (size_t c = 0; c < fields.size(); c++)
-            for (size_t u = 0; u < units.size(); u++) {
-                const Range& r = ranges[range_of[c][u]];
-                const int64_t off = chunk_meta(units[u], c).start() - r.start;
-                const OpenFile& of = open_files[r.file];
-                loc[c][u].host = (of.mem ? of.mem + r.start : sl.staging->ptr + r.dev_off) + off;
-                loc[c][u].dev = sl.chunk->ptr + r.dev_off + off;
+            for (const ChunkAt& at : up.chunk_at[c]) {
+                const UploadRange& r = up.ranges[at.range];
+                loc[c].push_back({host_of(r) + at.off, sl.chunk->ptr + r.dev_off + at.off});
             }
-        t_h2d += now_ms() - tt;
-        // ---- phase A: page tables on the host (reads only page headers) ------------------------------------------------------------
-        tt = now_ms();
-        std::vector<ColPlan> plans(fields.size());
-        for (size_t c = 0; c < fields.size(); c++) plan_column(c, units, total, loc[c], out.cols[c], plans[c]);
-        // ---- work block: one bump allocation per buffer, sized now that every page is known ----------------------------------
+        return loc;
+    }
+
+    // one bump allocation in the work block per device buffer, sized now that every page is known; page tables into the pinned block
+    void bind_buffers(std::vector<ColPlan>& plans, int64_t total, Slot& sl) {
         size_t need = 1024, meta_need = 4096;
         for (auto& p : plans) meta_need += align_up(p.pages.size() * sizeof(PqPage), 64) + align_up(p.remap.size() * 4, 64) + align_up(p.hostdec.size(), 64) + 192;
         std::vector<std::pair<uint8_t**, size_t>> reqs;
-        uint8_t *derr_p = nullptr, *meta_dev = nullptr; // meta_dev: device mirror of the slot's pinned page tables / remap tables
-        reqs.push_back({&derr_p, 64});
-        reqs.push_back({&meta_dev, meta_need});
+        uint8_t* derr = nullptr;
+        reqs.push_back({&derr, 64});
+        reqs.push_back({&sl.meta_dev, meta_need});
         for (auto& p : plans) buffer_requests(p, total, reqs);
         for (auto& r : reqs) need += align_up(r.second, 256) + 256;
         if (need > sl.work->cap) {
@@ -600,61 +350,65 @@ struct NativeScanSource : ExecNode {
             // as long as a batch handed to the consumer still points into it.
             if (trace_on()) fprintf(stderr, "[cb200 trace]   work block grows %.1f -> %.1f MB\n", sl.work->cap / 1e6, (need + need / 8) / 1e6);
             sl.work = block_cache().acquire(ctx->device, false, need + need / 8);
-            work_estimate = std::max(work_estimate, need + need / 8);
+            plan.work_estimate = std::max(plan.work_estimate, need + need / 8);
         }
         if (meta_need > sl.meta->cap) sl.meta = block_cache().acquire(ctx->device, true, meta_need + meta_need / 4);
-        {
-            size_t off = 0;
-            for (auto& r : reqs) { *r.first = sl.work->ptr + off; off += align_up(r.second, 256) + 256; }
-            sl.work_used = off;
-        }
+        size_t off = 0;
+        for (auto& r : reqs) { *r.first = sl.work->ptr + off; off += align_up(r.second, 256) + 256; }
+        sl.work_used = off;
+        sl.derr = (int*)derr;
         // tables: staged in the pinned block, pulled into the device mirror by ONE kernel that reads the mapped host memory.  (An
         // H2D memcpy would share the copy engine with the bulk transfer of the NEXT batch, which is already queued: measured,
         // every batch's decode then started a whole transfer late -- 17.7 ms per batch instead of the 14.75 ms the bytes take.)
-        for (auto& p : plans) stage_tables(p, sl, meta_dev);
-        t_pages += now_ms() - tt;
-        // ---- phase B: decode kernels -----------------------------------------------------------------------------------------------
-        tt = now_ms();
-        int* derr = (int*)derr_p;
-        cuda_check(cudaMemsetAsync(derr, 0, 64, res.decode_stream), "memset parquet err");
+        for (auto& p : plans) stage_tables(p, sl);
+    }
+
+    // `bytes` into the slot's pinned block; returns their address in the device mirror
+    uint8_t* stage(Slot& sl, const void* p, size_t bytes) {
+        uint8_t* pin = meta_take(sl, bytes);
+        memcpy(pin, p, bytes);
+        return sl.meta_dev + (pin - sl.meta->ptr);
+    }
+
+    // host-produced page bodies, page descriptors and the string dictionary remap of one column
+    void stage_tables(ColPlan& cp, Slot& sl) {
+        if (cp.pages.empty()) return;
+        uint8_t* hostdec_dev = cp.hostdec.empty() ? nullptr : stage(sl, cp.hostdec.data(), cp.hostdec.size());
+        std::vector<uint8_t>().swap(cp.hostdec);
+        resolve_bodies(cp, hostdec_dev);
+        cp.dpd = stage(sl, cp.pages.data(), cp.pages.size() * sizeof(PqPage));
+        if (!cp.remap.empty()) cp.ddict = stage(sl, cp.remap.data(), cp.remap.size() * 4);
+    }
+
+    void launch(std::vector<ColPlan>& plans, int64_t total, Batch& out, int si) {
+        Slot& sl = slots[si];
+        cuda_check(cudaMemsetAsync(sl.derr, 0, 64, res.decode_stream), "memset parquet err");
         void* meta_host_dev = nullptr;
         cuda_check(cudaHostGetDevicePointer(&meta_host_dev, sl.meta->ptr, 0), "cudaHostGetDevicePointer");
-        launch_pq_copy(meta_dev, meta_host_dev, align_up(sl.meta_used, 16), res.decode_stream);
+        launch_pq_copy(sl.meta_dev, meta_host_dev, align_up(sl.meta_used, 16), res.decode_stream);
         ctx->kernel_launches++;
         cuda_check(cudaStreamWaitEvent(res.decode_stream, res.uploaded[si], 0), "stream wait"); // decode kernels start when the batch has landed
-        {   // compressed columns first, spread over the side streams; the decode stream carries on when all of them are done
-            bool used[ScanRes::N_SIDE] = {false, false, false, false};
-            int n_comp = 0;
-            for (auto& cp : plans) if (cp.any_compressed && !cp.pages.empty()) n_comp++;
-            if (n_comp > 0) {
-                cuda_check(cudaEventRecord(res.side_begin, res.decode_stream), "event record");
-                int k = 0;
-                for (auto& cp : plans) {
-                    if (!cp.any_compressed || cp.pages.empty()) continue;
-                    const int sid = k++ % ScanRes::N_SIDE;
-                    if (!used[sid]) { cuda_check(cudaStreamWaitEvent(res.side[sid], res.side_begin, 0), "stream wait"); used[sid] = true; }
-                    launch_pq_snappy_segmented((PqPage*)cp.dpd, (int)cp.pages.size(), (unsigned*)cp.dckpt, (int)cp.n_segs_total, derr, res.side[sid]);
-                    ctx->kernel_launches += 3;
-                }
-                for (int i = 0; i < ScanRes::N_SIDE; i++) {
-                    if (!used[i]) continue;
-                    cuda_check(cudaEventRecord(res.side_done[i], res.side[i]), "event record");
-                    cuda_check(cudaStreamWaitEvent(res.decode_stream, res.side_done[i], 0), "stream wait");
-                }
-            }
+        launch_snappy(plans, sl.derr);
+        for (size_t c = 0; c < fields.size(); c++) launch_column(c, plans[c], total, out.cols[c], sl);
+    }
+
+    // compressed columns first, spread over the side streams; the decode stream carries on when all of them are done
+    void launch_snappy(std::vector<ColPlan>& plans, int* derr) {
+        bool used[ScanRes::N_SIDE] = {false, false, false, false};
+        int k = 0;
+        for (auto& cp : plans) {
+            if (!cp.any_compressed || cp.pages.empty()) continue;
+            if (k == 0) cuda_check(cudaEventRecord(res.side_begin, res.decode_stream), "event record");
+            const int sid = k++ % ScanRes::N_SIDE;
+            if (!used[sid]) { cuda_check(cudaStreamWaitEvent(res.side[sid], res.side_begin, 0), "stream wait"); used[sid] = true; }
+            launch_pq_snappy_segmented((PqPage*)cp.dpd, (int)cp.pages.size(), (unsigned*)cp.dckpt, (int)cp.n_segs_total, derr, res.side[sid]);
+            ctx->kernel_launches += 3;
         }
-        for (size_t c = 0; c < fields.size(); c++) bind_and_launch(c, plans[c], total, out.cols[c], derr, sl);
-        t_launch += now_ms() - tt;
-        if (trace_on()) fprintf(stderr, "[cb200 trace]   issue breakdown: h2d enqueue (%zu ranges) %.3f  page tables %.3f  launches %.3f ms; work %.1f MB\n", ranges.size(), t_h2d, t_pages, t_launch, sl.work_used / 1e6);
-        cuda_check(cudaEventRecord(res.decoded[si], res.decode_stream), "event record");
-        if (trace_on()) {
-            cuda_check(cudaEventRecord(pr->tr[1], res.copy_stream), "event record");
-            cuda_check(cudaEventRecord(pr->tr[3], res.decode_stream), "event record");
+        for (int i = 0; i < ScanRes::N_SIDE; i++) {
+            if (!used[i]) continue;
+            cuda_check(cudaEventRecord(res.side_done[i], res.side[i]), "event record");
+            cuda_check(cudaStreamWaitEvent(res.decode_stream, res.side_done[i], 0), "stream wait");
         }
-        sl.used = true;
-        cuda_check(cudaMemcpyAsync(&res.h_flags[si], derr, 4, cudaMemcpyDeviceToHost, res.decode_stream), "parquet err");
-        cuda_check(cudaEventRecord(res.done[si], res.decode_stream), "event record");
-        return pr;
     }
 
     bool next(Batch& out) override {
@@ -674,360 +428,37 @@ struct NativeScanSource : ExecNode {
                     (long long)cur->batch.n_rows, h2d, dec, lag);
         }
         const int perr = res.h_flags[cur->slot];
-        if (perr & 2) throw PlanError("parquet: a column chunk whose statistics say null_count = 0 contains NULLs (corrupt statistics)");
-        if (perr & 8) throw PlanError("parquet: malformed Snappy page");
-        if (perr & 4) throw ExecError(3, "", "parquet: dictionary index out of range (corrupt page)");
-        if (perr & 16) throw PlanError("parquet: truncated page (fewer encoded values than the page header declares)");
-        if (perr & 1) throw Unsupported("parquet: malformed RLE stream, or one with more than n/8 + 64 runs per page");
+        if (perr & PQ_ERR_NULL_ON_FAST_PATH) throw PlanError("parquet: a column chunk whose statistics say null_count = 0 contains NULLs (corrupt statistics)");
+        if (perr & PQ_ERR_SNAPPY) throw PlanError("parquet: malformed Snappy page");
+        if (perr & PQ_ERR_DICT_INDEX) throw ExecError(3, "", "parquet: dictionary index out of range (corrupt page)");
+        if (perr & PQ_ERR_TRUNCATED) throw PlanError("parquet: truncated page (fewer encoded values than the page header declares)");
+        if (perr & PQ_ERR_RLE) throw Unsupported("parquet: malformed RLE stream, or one with more than n/8 + 64 runs per page");
         out = std::move(cur->batch);
         return true;
     }
 
-    // ---- phase A ---------------------------------------------------------------------------------------------------------------------
-    void check_annotations(const pq::SchemaElement& se, const DType& t) const {
-        // SchemaElement.converted_type / logicalType decide what the physical bytes MEAN; a mismatch must not be read silently
-        const int ct = se.converted_type;
-        if (t.id == TypeId::Timestamp || t.id == TypeId::TimestampNtz) {
-            const bool millis = ct == 9 || se.ts_unit == 1, nanos = se.ts_unit == 3;
-            if (millis || nanos) throw Unsupported(std::string("parquet: TIMESTAMP_") + (millis ? "MILLIS" : "NANOS") + " column '" + se.name + "' (only microsecond timestamps are decoded; unit conversion is out of scope)");
-        }
-        if (ct == 13 || ct == 14 || (se.int_bits >= 32 && se.int_signed == 0)) throw Unsupported("parquet: unsigned 32/64-bit integer column '" + se.name + "'");
-        if ((ct == 11 || ct == 12 || (se.int_bits > 0 && se.int_bits < 32 && se.int_signed == 0)) && !(t.id == TypeId::Int32 || t.id == TypeId::Int64 || t.id == TypeId::Int16))
-            throw Unsupported("parquet: unsigned 8/16-bit integer column '" + se.name + "' read as " + t.str());
-        if (t.is_decimal()) {
-            if (se.scale != t.scale) throw Unsupported("parquet decimal scale differs from the requested type (schema adapter casts are out of scope)");
-            if (se.precision > 0 && se.precision > t.precision) throw Unsupported("parquet: decimal(" + std::to_string(se.precision) + ") column '" + se.name + "' read as " + t.str());
-            if (ct != 5 && !se.logical_decimal) throw Unsupported("parquet: column '" + se.name + "' carries no DECIMAL annotation but is read as " + t.str());
-        }
-    }
-
-    void plan_column(size_t c, const std::vector<Unit>& units, int64_t total, const std::vector<ChunkLoc>& loc, Column& col, ColPlan& cp) {
-        const DType& t = fields[c].type;
-        const pq::SchemaElement& se = open_files[units[0].file].meta.leaf(open_files[units[0].file].leaf_of[c]);
-        col.type = t;
-        col.null_count = 0;
-        cp.phys_type = se.type;
-        cp.type_length = se.type_length;
-        switch (se.type) {
-        case pq::INT32:
-            if (!(t.is_integer() || t.id == TypeId::Date || (t.is_decimal() && t.precision <= 9))) throw Unsupported("parquet INT32 -> " + t.str());
-            if (t.id == TypeId::Int64) { cp.conv = PQ_I32_TO_I64; cp.out_w = 8; col.phys = Phys::I64; }
-            else { cp.conv = PQ_COPY32; cp.out_w = 4; col.phys = Phys::I32; }
-            break;
-        case pq::INT64:
-            if (!(t.id == TypeId::Int64 || t.id == TypeId::Timestamp || t.id == TypeId::TimestampNtz || (t.is_decimal() && t.precision <= 18)))
-                throw Unsupported("parquet INT64 -> " + t.str());
-            cp.conv = PQ_COPY64; cp.out_w = 8; col.phys = Phys::I64;
-            break;
-        case pq::FLOAT: if (t.id != TypeId::Float32) throw Unsupported("parquet FLOAT -> " + t.str()); cp.conv = PQ_COPY32; cp.out_w = 4; col.phys = Phys::F32; break;
-        case pq::DOUBLE: if (t.id != TypeId::Float64) throw Unsupported("parquet DOUBLE -> " + t.str()); cp.conv = PQ_COPY64; cp.out_w = 8; col.phys = Phys::F64; break;
-        case pq::FIXED_LEN_BYTE_ARRAY:
-            if (!t.is_decimal() || se.type_length > 16) throw Unsupported("parquet FIXED_LEN_BYTE_ARRAY -> " + t.str());
-            if (t.precision <= 18) { cp.conv = PQ_FLBA_TO_I64; cp.out_w = 8; col.phys = Phys::I64; }
-            else { cp.conv = PQ_FLBA_TO_I128; cp.out_w = 16; col.phys = Phys::I128; }
-            break;
-        case pq::BYTE_ARRAY:
-            if (!t.is_string()) throw Unsupported("parquet BYTE_ARRAY -> " + t.str());
-            cp.conv = -1; cp.out_w = 4; col.phys = Phys::I32; col.is_dict = true;
-            if (!dicts[c]) dicts[c] = std::make_shared<Dictionary>();
-            col.dict = dicts[c];
-            break;
-        default: throw Unsupported("parquet physical type " + std::to_string(se.type));
-        }
-        check_annotations(se, t);
-        std::vector<PqPage>& dpages = cp.pages;
-        std::vector<PqPage> dict_pages;                // fixed-width dictionary pages (decoded into the combined dictionary)
-        bool nulls_possible = false;
-        std::vector<uint8_t> host_scratch;
-        // compressed page bodies are decompressed into `dunc`; its offsets are assigned here and turned into pointers in bind
-        // codec: pq::UNCOMPRESSED (or an uncompressed v2 values section), pq::SNAPPY (device), or a host codec
-        auto place_body = [&](PqPage& d, const unsigned char* src, const uint8_t* host_src, int comp_bytes, int unc, int codec) {
-            const bool compressed = codec == pq::SNAPPY;
-            if (codec != pq::UNCOMPRESSED && codec != pq::SNAPPY) {
-                if (unc < 0 || comp_bytes < 0) throw PlanError("parquet: negative page size");
-                const size_t off = cp.hostdec.size();
-                cp.hostdec.resize(off + (((size_t)unc + 31) / 16) * 16, 0); // 16-byte aligned, >= 8 spare bytes for the unaligned-word loads
-                host_decompress(codec, host_src, (size_t)comp_bytes, cp.hostdec.data() + off, (size_t)unc);
-                d.comp = nullptr;
-                d.comp_bytes = 0;
-                d.body = (unsigned char*)(uintptr_t)off; // offset for now (stage_tables turns it into the device address)
-                d.body_bytes = unc;
-                d.n_segs = 0;
-                d.flags |= PQ_PAGE_HOSTDEC;
-                return;
-            }
-            if (compressed) {
-                d.comp = src;
-                d.comp_bytes = comp_bytes;
-                d.body = (unsigned char*)(uintptr_t)cp.unc_bytes; // offset for now
-                d.body_bytes = unc;
-                d.n_segs = (unc + PQ_SNAPPY_SEG - 1) / PQ_SNAPPY_SEG; // checkpoint entries of the segmented Snappy decoder
-                cp.unc_bytes += ((size_t)unc + 31) / 16 * 16;     // 16-byte aligned, >= 8 spare bytes for the unaligned-word loads
-                cp.any_compressed = true;
-            } else {
-                d.comp = nullptr;
-                d.comp_bytes = 0;
-                d.body = (unsigned char*)src;
-                d.body_bytes = comp_bytes;
-                d.n_segs = 0;
-            }
-        };
-        // PLAIN-encoded string page (a writer's dictionary fallback).  Strings live on the device as codes of the plan-wide dictionary
-        // only, so the host -- which already parses every string dictionary page -- turns the page's values into codes: the page
-        // the device sees is [levels as written][int32 codes], PLAIN.  `vals` = the uncompressed value section on the host.
-        auto place_plain_strings = [&](PqPage& d, const uint8_t* prefix, size_t prefix_len, const uint8_t* vals, size_t vals_len) {
-            if (dict_index.size() < fields.size()) dict_index.resize(fields.size());
-            Dictionary& gd = *dicts[c];
-            auto& index = dict_index[c];
-            if (index.size() != gd.values.size()) { index.clear(); for (size_t k = 0; k < gd.values.size(); k++) index.emplace(gd.values[k], (int32_t)k); }
-            const size_t off = cp.hostdec.size();
-            cp.hostdec.resize(off + prefix_len, 0);
-            if (prefix_len) memcpy(cp.hostdec.data() + off, prefix, prefix_len);
-            size_t n_vals = 0;
-            const uint8_t *p = vals, *e = vals + vals_len;
-            while (p < e) {
-                if (p + 4 > e) throw PlanError("parquet: truncated PLAIN string page");
-                uint32_t len;
-                memcpy(&len, p, 4);
-                p += 4;
-                if (len > (size_t)(e - p)) throw PlanError("parquet: truncated PLAIN string page");
-                std::string v((const char*)p, len);
-                p += len;
-                auto it = index.find(v);
-                int32_t code;
-                if (it == index.end()) {
-                    if (gd.values.size() >= (size_t)INT32_MAX) throw Unsupported("parquet: more than 2^31 distinct strings in one column");
-                    code = (int32_t)gd.values.size();
-                    gd.values.push_back(v);
-                    index.emplace(std::move(v), code);
-                } else code = it->second;
-                const size_t at = cp.hostdec.size();
-                cp.hostdec.resize(at + 4);
-                memcpy(cp.hostdec.data() + at, &code, 4);
-                n_vals++;
-            }
-            const size_t body_bytes = cp.hostdec.size() - off;
-            cp.hostdec.resize(off + ((body_bytes + 31) / 16) * 16, 0);
-            d.comp = nullptr;
-            d.comp_bytes = 0;
-            d.body = (unsigned char*)(uintptr_t)off;
-            d.body_bytes = (int)body_bytes;
-            d.n_segs = 0;
-            d.flags |= PQ_PAGE_HOSTDEC;
-            d.encoding = 0;
-            cp.conv = PQ_COPY32; // k_pq_plain copies the codes of PLAIN pages; dictionary pages of the same column go through k_pq_rle_decode
-            (void)n_vals;
-        };
-        // uncompressed bytes of a page section on the host (any codec), valid until the next call
-        auto host_section = [&](const uint8_t* p, int comp, int unc, int codec_) -> const uint8_t* {
-            if (codec_ == pq::UNCOMPRESSED) return p;
-            host_scratch.assign((size_t)unc + 16, 0);
-            if (codec_ == pq::SNAPPY) {
-                if (cb::snappy_decode_serial(p, comp, host_scratch.data(), unc) != unc) throw PlanError("parquet: malformed Snappy page");
-            } else host_decompress(codec_, p, (size_t)comp, host_scratch.data(), (size_t)unc);
-            return host_scratch.data();
-        };
-        for (size_t u = 0; u < units.size(); u++) {
-            const OpenFile& of = open_files[units[u].file];
-            const pq::SchemaElement& use = of.meta.leaf(of.leaf_of[c]);
-            if (use.type != se.type || use.type_length != se.type_length) throw Unsupported("parquet: column '" + fields[c].name + "' changes physical type between files");
-            if (&use != &se) check_annotations(use, t);
-            const bool opt_u = use.repetition == 1;
-            cp.optional = cp.optional || opt_u;
-            const pq::ColumnChunkMeta& cc = chunk_meta(units[u], c);
-            if (opt_u && cc.null_count != 0) nulls_possible = true; // unknown (-1) counts as possible
-            if (cc.codec != pq::UNCOMPRESSED && cc.codec != pq::SNAPPY && !host_codec_supported(cc.codec))
-                throw Unsupported("parquet codec " + std::to_string(cc.codec) + " (UNCOMPRESSED and SNAPPY are decompressed on the device, ZSTD / LZ4 / LZ4_RAW / GZIP on the host; BROTLI / LZO are not read)");
-            const bool snappy = cc.codec == pq::SNAPPY;
-            const int codec = cc.codec;
-            if (cc.num_values != units[u].rows) throw Unsupported("parquet: repeated column (num_values != num_rows)");
-            const size_t clen = (size_t)cc.total_compressed;
-            const uint8_t* host = loc[u].host;
-            unsigned char* const dc = loc[u].dev;
-            std::vector<pq::PageInfo> pages = pq::walk_pages(host, clen, cc.num_values);
-            int64_t row = units[u].row0, this_dict_off = -1;
-            int this_dict_size = 0;
-            for (auto& pg : pages) {
-                if (pg.type == pq::DICTIONARY_PAGE) {
-                    this_dict_size = (int)pg.num_values;
-                    this_dict_off = cp.dict_elems;
-                    if (se.type == pq::BYTE_ARRAY) {
-                        // strings: parse on the host, unify with the plan-global dictionary, ship the code remap table
-                        const uint8_t* p = host + pg.data_offset;
-                        const uint8_t* e = p + pg.compressed_size;
-                        if (snappy) {
-                            host_scratch.assign((size_t)pg.uncompressed_size + 16, 0);
-                            if (cb::snappy_decode_serial(p, pg.compressed_size, host_scratch.data(), pg.uncompressed_size) != pg.uncompressed_size)
-                                throw PlanError("parquet: malformed Snappy dictionary page");
-                            p = host_scratch.data();
-                            e = p + pg.uncompressed_size;
-                        } else if (codec != pq::UNCOMPRESSED) {
-                            host_scratch.assign((size_t)pg.uncompressed_size + 16, 0);
-                            host_decompress(codec, p, (size_t)pg.compressed_size, host_scratch.data(), (size_t)pg.uncompressed_size);
-                            p = host_scratch.data();
-                            e = p + pg.uncompressed_size;
-                        }
-                        Dictionary& gd = *dicts[c];
-                        for (int k = 0; k < this_dict_size; k++) {
-                            if (p + 4 > e) throw PlanError("parquet: truncated dictionary page");
-                            uint32_t len;
-                            memcpy(&len, p, 4);
-                            p += 4;
-                            if (len > (size_t)(e - p)) throw PlanError("parquet: truncated dictionary page");
-                            std::string v((const char*)p, len);
-                            p += len;
-                            auto it = std::find(gd.values.begin(), gd.values.end(), v);
-                            if (it == gd.values.end()) { cp.remap.push_back((int32_t)gd.values.size()); gd.values.push_back(v); }
-                            else cp.remap.push_back((int32_t)(it - gd.values.begin()));
-                        }
-                    } else {
-                        PqPage dp;
-                        memset(&dp, 0, sizeof(dp));
-                        place_body(dp, dc + pg.data_offset, host + pg.data_offset, pg.compressed_size, pg.uncompressed_size, codec);
-                        dp.num_values = this_dict_size;
-                        dp.dst_row = cp.dict_elems; // decoded into the combined dictionary at this element offset
-                        dict_pages.push_back(dp);
-                    }
-                    cp.dict_elems += this_dict_size;
-                    continue;
-                }
-                if (pg.type != pq::DATA_PAGE && pg.type != pq::DATA_PAGE_V2) continue;
-                PqPage d;
-                memset(&d, 0, sizeof(d));
-                d.dst_row = row;
-                d.num_values = (int)pg.num_values;
-                const unsigned char* body = dc + pg.data_offset;
-                const bool plain_str = se.type == pq::BYTE_ARRAY && pg.encoding == pq::PLAIN;
-                if (plain_str && pg.type == pq::DATA_PAGE) {
-                    if (opt_u) d.flags |= PQ_PAGE_V1_LEVELS;
-                    const uint8_t* b = host_section(host + pg.data_offset, pg.compressed_size, pg.uncompressed_size, codec);
-                    size_t pre = 0;
-                    if (opt_u) { // [u32 byte length][RLE definition levels] stay as they are
-                        if (pg.uncompressed_size < 4) throw PlanError("parquet: data page shorter than its level header");
-                        uint32_t ll;
-                        memcpy(&ll, b, 4);
-                        if ((size_t)ll + 4 > (size_t)pg.uncompressed_size) throw PlanError("parquet: definition levels exceed the page");
-                        pre = 4 + ll;
-                    }
-                    place_plain_strings(d, b, pre, b + pre, (size_t)pg.uncompressed_size - pre);
-                } else if (plain_str) {
-                    const int lv = pg.rep_levels_bytes + pg.def_levels_bytes;
-                    if (lv > pg.compressed_size || lv > pg.uncompressed_size) throw PlanError("parquet: data page v2 level sizes exceed the page");
-                    d.def_ptr = body + pg.rep_levels_bytes;
-                    d.def_bytes = pg.def_levels_bytes;
-                    const uint8_t* b = host_section(host + pg.data_offset + lv, pg.compressed_size - lv, pg.uncompressed_size - lv, pg.v2_compressed ? codec : (int)pq::UNCOMPRESSED);
-                    place_plain_strings(d, nullptr, 0, b, (size_t)(pg.uncompressed_size - lv));
-                } else if (pg.type == pq::DATA_PAGE) {
-                    // v1: [u32 length + definition levels (optional columns)] [values], compressed as one block
-                    if (opt_u) d.flags |= PQ_PAGE_V1_LEVELS;
-                    place_body(d, body, host + pg.data_offset, pg.compressed_size, pg.uncompressed_size, codec);
-                } else {
-                    // v2: repetition + definition levels sit uncompressed in front of the (optionally compressed) values
-                    const int lv = pg.rep_levels_bytes + pg.def_levels_bytes;
-                    if (lv > pg.compressed_size || lv > pg.uncompressed_size) throw PlanError("parquet: data page v2 level sizes exceed the page");
-                    d.def_ptr = body + pg.rep_levels_bytes;
-                    d.def_bytes = pg.def_levels_bytes;
-                    place_body(d, body + lv, host + pg.data_offset + lv, pg.compressed_size - lv, pg.uncompressed_size - lv, pg.v2_compressed ? codec : (int)pq::UNCOMPRESSED);
-                }
-                if (pg.encoding == pq::PLAIN) {
-                    d.encoding = 0;
-                } else if (pg.encoding == pq::RLE_DICTIONARY || pg.encoding == pq::PLAIN_DICTIONARY) {
-                    if (this_dict_off < 0) throw PlanError("parquet: dictionary-encoded page without a dictionary page");
-                    d.encoding = 8;
-                    d.run_base = cp.run_base;
-                    d.max_runs = (int)(pg.num_values / 8 + 64);
-                    d.dict_off = this_dict_off;
-                    d.dict_size = this_dict_size;
-                    cp.run_base += d.max_runs;
-                } else throw Unsupported("parquet value encoding " + std::to_string(pg.encoding) + " (DELTA_* / BYTE_STREAM_SPLIT are next-row work)");
-                if (opt_u) {
-                    d.def_run_base = cp.def_run_base;
-                    d.def_max_runs = (int)(pg.num_values / 8 + 64);
-                    cp.def_run_base += d.def_max_runs;
-                }
-                row += pg.num_values;
-                dpages.push_back(d);
-            }
-            if (row != units[u].row0 + units[u].rows) throw PlanError("parquet: data pages of column '" + fields[c].name + "' do not add up to the row group's row count");
-        }
-        cp.n_data = dpages.size();
-        cp.n_dict_pages = dict_pages.size();
-        dpages.insert(dpages.end(), dict_pages.begin(), dict_pages.end()); // one upload for every descriptor of this column
-        // definition levels: the statistics' null_count == 0 selects the verify-only fast path; otherwise values are decoded
-        // densely and scattered to their rows
-        cp.null_aware = cp.optional && nulls_possible;
-        if (cp.null_aware && total >= (int64_t)1 << 32) throw Unsupported("parquet: NULL-aware decode of more than 2^32 rows per batch (lower spark.comet.b200.chunkRows)");
-    }
-
-    // every device buffer of a column, as (where the pointer goes, bytes)
-    static void buffer_requests(ColPlan& cp, int64_t total, std::vector<std::pair<uint8_t**, size_t>>& reqs) {
-        const size_t n = (size_t)std::max<int64_t>(total, 1);
-        cp.out_bytes = n * (size_t)cp.out_w;
-        reqs.push_back({&cp.out, cp.out_bytes});
-        if (cp.pages.empty()) return;
-        if (cp.any_compressed) {
-            reqs.push_back({&cp.dunc, cp.unc_bytes + 64});
-            cp.n_segs_total = 0;
-            for (auto& d : cp.pages) { d.seg_base = (int)cp.n_segs_total; cp.n_segs_total += d.comp ? d.n_segs : 0; if (!d.comp) d.n_segs = 0; }
-            reqs.push_back({&cp.dckpt, (size_t)(cp.n_segs_total + 1) * 4});
-        }
-        if (cp.dict_elems > 0 && cp.remap.empty()) reqs.push_back({&cp.ddict, (size_t)cp.dict_elems * (size_t)cp.out_w + 16}); // string dictionaries: the remap table in the mirror IS the dictionary
-        if (cp.null_aware) {
-            reqs.push_back({&cp.dense, n * (size_t)cp.out_w});
-            reqs.push_back({&cp.dvalid, n + 64});
-            reqs.push_back({&cp.didx, n * 4 + 64});
-            reqs.push_back({&cp.druns, (size_t)std::max<int64_t>(cp.def_run_base, 1) * sizeof(PqRun)});
-            reqs.push_back({&cp.dcounts, cp.n_data * 4 + 16});
-            cp.validity_bytes = (n + 31) / 32 * 4 + 16;
-            reqs.push_back({&cp.validity, cp.validity_bytes});
-        }
-        if (cp.run_base > 0) {
-            reqs.push_back({&cp.runs, (size_t)cp.run_base * sizeof(PqRun)});
-            reqs.push_back({&cp.counts, cp.n_data * 4 + 16});
-        }
-    }
-
-    // ---- phase B ---------------------------------------------------------------------------------------------------------------------
     DeviceBufP view(const Slot& sl, void* p, size_t bytes) const {
         auto b = std::make_shared<DeviceBuf>(p, bytes);
         b->owner = sl.work; // the block lives as long as a batch points into it
         return b;
     }
 
-    // page descriptors (+ string dictionary remap) of one column into the slot's pinned block; device addresses point into the mirror
-    void stage_tables(ColPlan& cp, Slot& sl, uint8_t* meta_dev) {
-        if (cp.pages.empty()) return;
-        if (cp.any_compressed) for (auto& d : cp.pages) if (d.comp) d.body = cp.dunc + (size_t)(uintptr_t)d.body;
-        if (!cp.hostdec.empty()) { // host-decompressed page bodies ride in the pinned block; the pages point at its device mirror
-            uint8_t* pin_body = meta_take(sl, cp.hostdec.size());
-            memcpy(pin_body, cp.hostdec.data(), cp.hostdec.size());
-            uint8_t* dev_body = meta_dev + (pin_body - sl.meta->ptr);
-            for (auto& d : cp.pages) if (d.flags & PQ_PAGE_HOSTDEC) d.body = dev_body + (size_t)(uintptr_t)d.body;
-            std::vector<uint8_t>().swap(cp.hostdec);
-        }
-        uint8_t* pin_pages = meta_take(sl, cp.pages.size() * sizeof(PqPage));
-        memcpy(pin_pages, cp.pages.data(), cp.pages.size() * sizeof(PqPage));
-        cp.dpd = meta_dev + (pin_pages - sl.meta->ptr);
-        if (!cp.remap.empty()) {
-            uint8_t* pin_remap = meta_take(sl, cp.remap.size() * 4);
-            memcpy(pin_remap, cp.remap.data(), cp.remap.size() * 4);
-            cp.ddict = meta_dev + (pin_remap - sl.meta->ptr);
-        }
-    }
-
-    void bind_and_launch(size_t c, ColPlan& cp, int64_t total, Column& col, int* derr, Slot& sl) {
+    void launch_column(size_t c, ColPlan& cp, int64_t total, Column& col, Slot& sl) {
+        col.type = fields[c].type;
+        col.phys = cp.phys;
+        col.is_dict = cp.dict != nullptr;
+        col.dict = cp.dict;
         col.data = view(sl, cp.out, cp.out_bytes);
         if (cp.pages.empty()) return;
         const cudaStream_t ds = res.decode_stream;
-        std::vector<PqPage>& dpages = cp.pages;
-        const int n_all = (int)dpages.size(), n_data = (int)cp.n_data;
-        PqPage* all_pages = (PqPage*)cp.dpd;
-        PqPage* data_pages = all_pages;
-        const PqPage* dict_pages_dev = data_pages + n_data;
+        int* derr = sl.derr;
+        const int n_all = (int)cp.pages.size(), n_data = (int)cp.n_data;
+        PqPage* data_pages = (PqPage*)cp.dpd;
+        const PqPage* dict_pages = data_pages + n_data;
         uint8_t* dense = cp.null_aware ? cp.dense : cp.out;
-        launch_pq_resolve(all_pages, n_all, ds);
+        launch_pq_resolve(data_pages, n_all, ds);
         ctx->kernel_launches++;
-        if (cp.n_dict_pages) { launch_pq_plain(dict_pages_dev, (int)cp.n_dict_pages, cp.conv, cp.type_length, cp.ddict, derr, ds); ctx->kernel_launches++; }
+        if (cp.n_dict_pages) { launch_pq_plain(dict_pages, (int)cp.n_dict_pages, cp.conv, cp.type_length, cp.ddict, derr, ds); ctx->kernel_launches++; }
         if (cp.optional && !cp.null_aware) { launch_pq_check_def_levels(data_pages, n_data, derr, ds); ctx->kernel_launches++; }
         if (cp.null_aware) {
             launch_pq_def_levels(data_pages, n_data, (PqRun*)cp.druns, (int*)cp.dcounts, cp.dvalid, (unsigned*)cp.didx, derr, ds);
@@ -1045,7 +476,6 @@ struct NativeScanSource : ExecNode {
             launch_pq_scatter(cp.dvalid, (const unsigned*)cp.didx, dense, cp.out, (unsigned*)cp.validity, total, cp.out_w, ds);
             ctx->kernel_launches++;
         }
-        (void)c;
     }
 };
 

@@ -133,3 +133,159 @@ def test_host_codecs_decompress_what_pyarrow_compressed():
         out = C.create_string_buffer(len(raw))
         f(codec_id, comp, len(comp), out, len(raw))
         assert out.raw == raw, name
+
+
+# ---- the scan planner (csrc/scan_plan.cpp) without a GPU ------------------------------------------------------------------------
+@pytest.fixture(scope="module")
+def planner(tmp_path_factory):
+    """csrc/scan_plan_test.cpp linked with the planner and the host parsers only: -Wl,--no-undefined proves they need no CUDA runtime."""
+    import ctypes as C
+    import json
+    import os
+    import subprocess
+    csrc = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "datafusion-comet_b200", "csrc")
+    cuda = os.environ.get("CUDA", "/usr/local/cuda")
+    so = str(tmp_path_factory.mktemp("scanplan") / "libcb200_scanplan.so")
+    srcs = [os.path.join(csrc, f) for f in ("scan_plan_test.cpp", "scan_plan.cpp", "parquet.cpp", "host_codecs.cpp", "plan.cpp")]
+    subprocess.check_call(["/usr/bin/g++", "-O1", "-std=c++17", "-fPIC", "-shared", f"-I{cuda}/include", "-o", so, *srcs, "-Wl,--no-undefined", "-lz", "-ldl"])
+    lib = C.CDLL(so)
+    lib.sp_plan.restype = C.c_char_p
+    lib.sp_plan.argtypes = [C.c_char_p, C.c_size_t, C.c_longlong]
+
+    def plan(scan_bytes, chunk_rows=1 << 26):
+        out = json.loads(lib.sp_plan(scan_bytes, len(scan_bytes), chunk_rows))
+        assert "error" not in out, bytes.fromhex(out["error"]).decode()
+        out["dictionaries"] = [[bytes.fromhex(v).decode() for v in d] for d in out["dictionaries"]]
+        return out
+    return plan
+
+
+def _chunk_pages(raw, col):
+    """(header, body offset) of every page of a column chunk, read by oracle/parquet_oracle.py"""
+    from oracle import parquet_oracle as po
+    pos = col.dictionary_page_offset if col.has_dictionary_page and col.dictionary_page_offset else col.data_page_offset
+    pos, end = min(pos, col.data_page_offset), min(pos, col.data_page_offset) + col.total_compressed_size
+    out = []
+    while pos < end:
+        h, body = po.page_header(raw, pos)
+        out.append((h, body))
+        pos = body + h["compressed"]
+    return out
+
+
+@pytest.mark.parametrize("compression,version,dictionary", [("NONE", "1.0", False), ("SNAPPY", "1.0", True), ("SNAPPY", "2.0", False), ("NONE", "2.0", True),
+                                                            ("ZSTD", "1.0", True), ("ZSTD", "2.0", False)])
+def test_planner_pages_tile_every_row_group(cb, planner, tmp_path, compression, version, dictionary):
+    """Each column's data pages cover its row groups' rows exactly, in order, with the page headers' value counts and encodings."""
+    import decimal
+    import pyarrow as pa
+    P = cb.proto
+    rng = np.random.default_rng(6)
+    n = 30_000
+    mask = lambda: rng.random(n) < 0.15
+    words = np.array(["AIR", "MAIL", "SHIP", "", "TRUCK", "ünï"])[rng.integers(0, 6, n)]
+    tbl = pa.table({"i64": pa.array(rng.integers(-2**60, 2**60, n), mask=mask()), "low": pa.array(rng.integers(0, 30, n).astype(np.int32)),
+                    "d12": pa.array([decimal.Decimal(int(v)).scaleb(-2) for v in rng.integers(-10**11, 10**11, n)], type=pa.decimal128(12, 2)),
+                    "word": pa.array(words.tolist(), mask=mask()).cast(pa.string())})
+    path = str(tmp_path / "p.parquet")
+    pq.write_table(tbl, path, row_group_size=7_000, compression=compression, use_dictionary=dictionary, data_page_version=version, data_page_size=4096)
+    fields = [("i64", P.INT64, True), ("low", P.INT32, True), ("d12", P.DECIMAL(12, 2), True), ("word", P.STRING, True)]
+    out = planner(P.native_scan(fields, fields, [path]), chunk_rows=15_000)
+    raw = open(path, "rb").read()
+    md = pq.ParquetFile(path).metadata
+    assert [u[1] for b in out["batches"] for u in b["units"]] == list(range(md.num_row_groups))
+    for b in out["batches"]:
+        for ci, col in enumerate(b["columns"]):
+            data = col["pages"][:col["n_data"]]
+            row = 0
+            for _, rg, rows, row0 in b["units"]:
+                assert row0 == row
+                pages = [(h, off) for h, off in _chunk_pages(raw, md.row_group(rg).column(ci)) if h["type"] in (0, 3)]
+                mine, data = data[:len(pages)], data[len(pages):]
+                assert len(mine) == len(pages)
+                for p, (h, _) in zip(mine, pages):
+                    assert p["dst_row"] == row and p["num_values"] == h["num_values"]
+                    assert p["encoding"] == (0 if h["encoding"] == 0 else 8)
+                    lv = h["rep_bytes"] + h["def_bytes"] if h["type"] == 3 else 0
+                    assert p["def_bytes"] == (h["def_bytes"] if h["type"] == 3 else 0)
+                    if not p["flags"] & 8 or p["encoding"] != 0 or ci != 3:             # everything but host-encoded PLAIN strings: the page's own bytes
+                        assert p["body_bytes"] == h["uncompressed"] - lv
+                    row += p["num_values"]
+                assert row == row0 + rows
+            assert data == []
+
+
+@pytest.mark.parametrize("compression,version", [("SNAPPY", "1.0"), ("NONE", "2.0")])
+def test_planner_codes_plain_and_dictionary_strings_alike(cb, planner, tmp_path, compression, version):
+    """A PLAIN file and a dictionary file of one string column: every value gets the same code, the dictionary holds it once."""
+    import pyarrow as pa
+    from oracle import parquet_oracle as po
+    P = cb.proto
+    rng = np.random.default_rng(4)
+    n = 20_000
+    words = np.array([f"w{i:04d}" for i in range(900)] + ["", "ünï", "a" * 300])[rng.integers(0, 903, n)]
+    tbl = pa.table({"word": pa.array(words.tolist(), mask=rng.random(n) < 0.1).cast(pa.string())})
+    p1, p2 = str(tmp_path / "plain.parquet"), str(tmp_path / "dict.parquet")
+    pq.write_table(tbl, p1, row_group_size=8_000, compression=compression, use_dictionary=False, data_page_version=version, data_page_size=4096)
+    pq.write_table(tbl, p2, row_group_size=8_000, compression=compression, use_dictionary=True, data_page_version=version)
+    fields = [("word", P.STRING, True)]
+    out = planner(P.native_scan(fields, fields, [p1, p2]), chunk_rows=n)
+    dictionary = out["dictionaries"][0]
+    want = [w for w in tbl.column("word").to_pylist() if w is not None]
+    assert len(set(dictionary)) == len(dictionary) and set(dictionary) == set(want)
+    code = {v: i for i, v in enumerate(dictionary)}
+    plain_codes, remap = [], []
+    for b in out["batches"]:
+        col = b["columns"][0]
+        if b["units"][0][0] == 0:
+            assert col["remap"] == [] and all(p["flags"] & 8 and p["encoding"] == 0 for p in col["pages"])
+            plain_codes += [c for p in col["pages"] for c in p["codes"]]
+        else:
+            assert all(p["encoding"] == 8 for p in col["pages"])
+            remap += col["remap"]
+    assert [dictionary[c] for c in plain_codes] == want
+    raw = open(p2, "rb").read()
+    md = pq.ParquetFile(p2).metadata
+    dict_values = []
+    for rg in range(md.num_row_groups):
+        h, body = _chunk_pages(raw, md.row_group(rg).column(0))[0]
+        data = raw[body:body + h["compressed"]]
+        data = po.snappy_decompress(data) if compression == "SNAPPY" else data
+        dict_values += [v.decode() for v in po.plain(data, "BYTE_ARRAY", h["num_values"])]
+    assert remap == [code[v] for v in dict_values]
+
+
+@pytest.mark.parametrize("variant", ["dec", "f64"])
+def test_planner_prunes_q6_row_groups_by_min_max(cb, planner, tmp_path, variant):
+    """The row groups the GPU test test_q6_row_groups_pruned_by_min_max expects to be read: those whose l_shipdate range meets 1994."""
+    t = cb.tpch
+    n = 400_000
+    cols = t.gen_lineitem(n, seed=41)
+    order = np.argsort(cols["l_shipdate"], kind="stable")
+    cols = {k: v[order] for k, v in cols.items()}
+    path = t.write_lineitem_parquet(cols, str(tmp_path / f"q6_{variant}.parquet"), variant, row_group_size=16_384, columns=t.Q6_COLUMNS)
+    out = planner(t.q6_native_scan(variant, [path]), chunk_rows=60_000)
+    ship = cols["l_shipdate"]
+    groups = [(g, ship[g * 16_384:(g + 1) * 16_384]) for g in range((n + 16_383) // 16_384)]
+    exp = [g for g, s in groups if s.max() >= t.DATE_1994_01_01 and s.min() < t.DATE_1995_01_01]
+    assert [u[1] for b in out["batches"] for u in b["units"]] == exp
+    assert out["pruned_row_groups"] == len(groups) - len(exp) >= len(groups) * 0.8
+    assert out["pruned_rows"] == n - sum(len(s) for g, s in groups if g in exp)
+
+
+def test_planner_file_splits_own_the_row_groups_that_start_inside_them(cb, planner, tmp_path):
+    """Two splits of one file cut in the middle of a row group: each row group belongs to the split it starts in."""
+    import os
+    t = cb.tpch
+    P = cb.proto
+    path = t.write_lineitem_parquet(t.gen_lineitem(100_000, seed=45), str(tmp_path / "split.parquet"), "dec", row_group_size=10_000)
+    size = os.path.getsize(path)
+    md = pq.ParquetFile(path).metadata
+    starts = [md.row_group(g).column(0).dictionary_page_offset or md.row_group(g).column(0).data_page_offset for g in range(md.num_row_groups)]
+    cut = starts[4] + 1
+    fields = list(zip(t.Q1_COLUMNS, t.q1_scan_fields("dec"), [True] * 7))
+    got = []
+    for lo, ln in ((0, cut), (cut, size - cut)):
+        out = planner(P.native_scan(fields, fields, [(path, lo, ln, size)]))
+        got.append([u[1] for b in out["batches"] for u in b["units"]])
+    assert got == [[g for g in range(md.num_row_groups) if starts[g] < cut], [g for g in range(md.num_row_groups) if starts[g] >= cut]]
