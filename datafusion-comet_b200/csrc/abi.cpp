@@ -354,6 +354,7 @@ int cb200_plan_stats(cb200_plan* plan, cb200_stats* out) {
     out->d2h_bytes = c.d2h_bytes;
     out->scan_pruned_row_groups = c.scan_pruned_row_groups;
     out->scan_pruned_rows = c.scan_pruned_rows;
+    out->agg_strategies = c.agg_strategies;
     return 0;
 }
 

@@ -3,6 +3,7 @@
 //   table:  a key table in HBM hands out group ids; state rows addressed by id (device/cb_kernels.cuh CB_HASH)
 //   stream: Partial over clustered keys: one state row per run of equal adjacent keys, no key table (CB_STREAM)
 #include "exec_internal.h"
+#include "../../include/comet_b200.h"
 
 #include "aot_kernels.h"
 #include "ranges.h"
@@ -579,8 +580,12 @@ struct AggNode : FusedBase {
         key_has_null = hn;
         if (observed_bits.empty()) observed_bits.assign(child->schema.size(), -1);
         if (strategy == Strategy::Undecided || (strategy == Strategy::Dense && needs_hash)) {
-            if (strategy == Strategy::Dense) leave_dense();
+            if (strategy == Strategy::Dense) {
+                leave_dense();
+                ctx->agg_strategies |= CB200_AGG_MIGRATED;
+            }
             strategy = !needs_hash ? Strategy::Dense : sample_stream(b) ? Strategy::Stream : Strategy::Table;
+            ctx->agg_strategies |= strategy == Strategy::Dense ? CB200_AGG_DENSE : strategy == Strategy::Stream ? CB200_AGG_STREAM : CB200_AGG_TABLE;
         }
         if (strategy == Strategy::Dense) consume_dense(b, nc, n_groups);
         else if (strategy == Strategy::Table) consume_table(b);

@@ -925,7 +925,9 @@ GeneratedKernel generate_pipeline_uncached(const PipelineSpec& spec) {
                 if (kt.is_decimal()) {
                     if (kv.narrow) raw = "(cb::u64)" + kv.v;
                     else {
-                        em.body << "    if (keep_ && !cb::i128_fits_i64(" << kv.v << ")) atomicOr(p.hflags, 4);\n";
+                        // a NULL key packs as 0 whatever bytes its slot holds (Arrow leaves them unspecified): only valid keys count
+                        const std::string valid = kv.n.empty() ? "" : " && !" + kv.n;
+                        em.body << "    if (keep_" << valid << " && !cb::i128_fits_i64(" << kv.v << ")) atomicOr(p.hflags, 4);\n";
                         raw = kv.v + ".lo";
                     }
                 } else if (kt.id == TypeId::Bool) raw = "(" + kv.v + " ? 1ull : 0ull)";
@@ -1123,13 +1125,16 @@ GeneratedKernel generate_pipeline_uncached(const PipelineSpec& spec) {
                         upd("wrap", "!" + cnull, L.w_cnt, c.v);
                         upd("count", "(" + snull + " || " + cnull + ")", L.w_bad);
                         upd("i128", "!" + snull, L.w_sum, Emitter::W(s));
-                    } else { // avg.rs:279-309
+                    } else { // avg.rs:165-175 (ungrouped), :279-309 (grouped)
+                        // A NULL partial sum or count adds nothing: the ungrouped accumulator merges with arrow's null-skipping
+                        // `sum`, and its Partial emits a NULL sum for a partition that saw no batch (avg.rs:148-153).  The bytes
+                        // under a NULL slot are unspecified in Arrow, so they are never read.
                         Val s = col(0), c = col(1);
                         L.is_f64_sum = true;
                         L.w_sum = slots.add(W_DD_HI, tag + "sum", 2);
                         L.w_cnt = slots.add(W_WRAP64, tag + "cnt");
-                        upd("f64", "true", L.w_sum, s.v);
-                        upd("wrap", "true", L.w_cnt, c.v);
+                        upd("f64", s.n.empty() ? "true" : "!" + s.n, L.w_sum, s.v);
+                        upd("wrap", c.n.empty() ? "true" : "!" + c.n, L.w_cnt, c.v);
                     }
                     break;
                 case AggKind::Min: case AggKind::Max: {

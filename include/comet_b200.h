@@ -183,7 +183,12 @@ typedef struct cb200_stats {
     int64_t d2h_bytes;         /* device->host bytes copied by cb200_execute */
     int64_t scan_pruned_row_groups; /* Parquet row groups skipped because their statistics rule the pushed filters out */
     int64_t scan_pruned_rows;
+    int64_t agg_strategies;    /* OR of CB200_AGG_* over the plan's aggregates: which accumulation strategies ran */
 } cb200_stats;
+#define CB200_AGG_DENSE 1      /* thread-private accumulators over dictionary / bool key codes (and ungrouped aggregates) */
+#define CB200_AGG_TABLE 2      /* global key table */
+#define CB200_AGG_STREAM 4     /* one state row per run of equal keys */
+#define CB200_AGG_MIGRATED 8   /* a dense aggregate outgrew its group limit and moved to hashing mid-stream */
 int cb200_plan_stats(cb200_plan* plan, cb200_stats* out);
 
 /* The library recycles device blocks >= 1 MiB on a per-device free list instead of returning them to the driver (a query step

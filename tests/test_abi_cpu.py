@@ -25,6 +25,17 @@ def test_library_exports_every_declared_symbol(cb):
     assert set(cb.native.EXPORTED) <= declared
 
 
+def test_stats_struct_matches_the_header(cb):
+    """native.Stats mirrors cb200_stats field by field (the binding reads it by position), incl. agg_strategies and its bits."""
+    hdr = open(os.path.join(ROOT, "include", "comet_b200.h")).read()
+    body = hdr[hdr.index("typedef struct cb200_stats {"):hdr.index("} cb200_stats;")]
+    fields = re.findall(r"^\s*(?:int64_t|double)\s+([a-z_0-9]+);", body, re.M)
+    assert fields == [f for f, _ in cb.native.Stats._fields_]
+    bits = dict(re.findall(r"#define CB200_AGG_([A-Z]+) (\d+)", hdr))
+    n = cb.native
+    assert {k: int(v) for k, v in bits.items()} == {"DENSE": n.AGG_DENSE, "TABLE": n.AGG_TABLE, "STREAM": n.AGG_STREAM, "MIGRATED": n.AGG_MIGRATED}
+
+
 def test_version(cb):
     assert "sm_90a" in cb.native.version()
 
