@@ -1,12 +1,13 @@
 // parquet_kernels.cu -- Parquet page decode on sm_90a.
 //
-// Encodings per the Apache Parquet specification (Encodings.md): PLAIN for fixed-width physical types,
-// RLE/bit-packed hybrid for dictionary indices (RLE_DICTIONARY: 1 byte bit width, then runs) and for
-// definition levels.  The reference reaches the third-party `parquet` crate for this
+// Encodings per the Apache Parquet specification (Encodings.md): PLAIN and BYTE_STREAM_SPLIT for fixed-width physical
+// types, DELTA_BINARY_PACKED for INT32 / INT64, RLE/bit-packed hybrid for dictionary indices (RLE_DICTIONARY: 1 byte bit
+// width, then runs) and for definition levels.  The reference reaches the third-party `parquet` crate for this
 // (native/core/src/parquet/parquet_exec.rs:139-141); its source is not under the reference tree, so the
 // decoders follow the format specification and are checked against pyarrow-written files.
 #include "parquet_kernels.h"
 #include "device/cb_math.h"
+#include "device/cb_delta.h"
 #include "device/cb_snappy.h"
 #include <algorithm>
 
@@ -465,30 +466,53 @@ void launch_pq_resolve(PqPage* pages, int n_pages, cudaStream_t st) {
     if (n_pages > 0) k_pq_resolve<<<(n_pages + 127) / 128, 128, 0, st>>>(pages, n_pages);
 }
 
-// ---- PLAIN ---------------------------------------------------------------------------------------------------
+// ---- PLAIN / BYTE_STREAM_SPLIT ---------------------------------------------------------------------------------
+// One conversion for every layout: byte(k) returns byte k of the value being converted (little-endian for the numeric types,
+// big-endian two's complement of flba_len bytes for FIXED_LEN_BYTE_ARRAY decimals).
+template <int CONV, typename B> __device__ __forceinline__ void pq_store(u8* out, long long row, int flba_len, B byte) {
+    if (CONV == PQ_COPY32 || CONV == PQ_I32_TO_I64) {
+        const u32 v = (u32)byte(0) | ((u32)byte(1) << 8) | ((u32)byte(2) << 16) | ((u32)byte(3) << 24);
+        if (CONV == PQ_COPY32) ((u32*)out)[row] = v;
+        else ((i64*)out)[row] = (i64)(i32)v;
+    } else if (CONV == PQ_COPY64) {
+        u64 v = 0;
+        for (int k = 0; k < 8; k++) v |= (u64)byte(k) << (8 * k);
+        ((u64*)out)[row] = v;
+    } else {
+        u64 hi = (byte(0) & 0x80) ? ~0ull : 0ull, lo = hi;
+        for (int k = 0; k < flba_len; k++) {
+            hi = (hi << 8) | (lo >> 56);
+            lo = (lo << 8) | byte(k);
+        }
+        if (CONV == PQ_FLBA_TO_I64) ((i64*)out)[row] = (i64)lo;
+        else ((i128*)out)[row] = mk128(lo, (i64)hi);
+    }
+}
+
+// PLAIN: value i at values[i * w, i * w + w).  BYTE_STREAM_SPLIT: byte k of value i at values[k * N + i], N = the page's non-null values.
 template <int CONV> __global__ void k_pq_plain(const PqPage* pages, int flba_len, u8* out, int* err) {
     const PqPage pg = pages[blockIdx.y];
-    if (pg.encoding != 0) return; // dictionary-encoded page: decoded by k_pq_rle_decode
+    const bool bss = pg.encoding == PQ_ENC_BSS;
+    if (pg.encoding != PQ_ENC_PLAIN && !bss) return; // dictionary / delta pages have their own kernels
     const u8* src = pg.values;
     const int w = CONV == PQ_COPY32 || CONV == PQ_I32_TO_I64 ? 4 : CONV == PQ_COPY64 ? 8 : flba_len;
-    const int have = w > 0 ? pg.values_bytes / w : 0;   // never read beyond the page, whatever the header claims
-    const int count = pg.nonnull < have ? pg.nonnull : have;
-    if (pg.nonnull > have && blockIdx.x == 0 && threadIdx.x == 0) atomicOr(err, PQ_ERR_TRUNCATED); // short page: the rows it cannot fill must not pass silently
+    const long long n = pg.nonnull;
+    int count;
+    if (bss) { // the streams' length follows from N: any other size is malformed and is not read at all
+        if (n * w != (long long)pg.values_bytes) { if (blockIdx.x == 0 && threadIdx.x == 0) atomicOr(err, PQ_ERR_BSS); return; }
+        count = (int)n;
+    } else {
+        const int have = w > 0 ? pg.values_bytes / w : 0;   // never read beyond the page, whatever the header claims
+        count = pg.nonnull < have ? pg.nonnull : have;
+        if (pg.nonnull > have && blockIdx.x == 0 && threadIdx.x == 0) atomicOr(err, PQ_ERR_TRUNCATED); // short page: the rows it cannot fill must not pass silently
+    }
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < count; i += gridDim.x * blockDim.x) {
         long long row = pg.dst_row + i;
-        if (CONV == PQ_COPY32) ((u32*)out)[row] = load_u32_unaligned(src + (size_t)i * 4);
+        if (bss) pq_store<CONV>(out, row, flba_len, [&](int k) -> u8 { return src[(size_t)k * (size_t)n + (size_t)i]; });
+        else if (CONV == PQ_COPY32) ((u32*)out)[row] = load_u32_unaligned(src + (size_t)i * 4);
         else if (CONV == PQ_COPY64) ((u64*)out)[row] = load_u64_unaligned(src + (size_t)i * 8);
         else if (CONV == PQ_I32_TO_I64) ((i64*)out)[row] = (i64)(i32)load_u32_unaligned(src + (size_t)i * 4);
-        else { // FIXED_LEN_BYTE_ARRAY: big-endian two's complement of flba_len bytes
-            const u8* b = src + (size_t)i * flba_len;
-            u64 hi = (b[0] & 0x80) ? ~0ull : 0ull, lo = hi;
-            for (int k = 0; k < flba_len; k++) {
-                hi = (hi << 8) | (lo >> 56);
-                lo = (lo << 8) | b[k];
-            }
-            if (CONV == PQ_FLBA_TO_I64) ((i64*)out)[row] = (i64)lo;
-            else ((i128*)out)[row] = mk128(lo, (i64)hi);
-        }
+        else { const u8* b = src + (size_t)i * flba_len; pq_store<CONV>(out, row, flba_len, [&](int k) -> u8 { return b[k]; }); }
     }
 }
 void launch_pq_plain(const PqPage* pages, int n_pages, int conv, int flba_len, void* out, int* err, cudaStream_t st) {
@@ -501,6 +525,130 @@ void launch_pq_plain(const PqPage* pages, int n_pages, int conv, int flba_len, v
     case PQ_FLBA_TO_I64: k_pq_plain<PQ_FLBA_TO_I64><<<grid, block, 0, st>>>(pages, flba_len, (u8*)out, err); break;
     default: k_pq_plain<PQ_FLBA_TO_I128><<<grid, block, 0, st>>>(pages, flba_len, (u8*)out, err); break;
     }
+}
+
+// ---- DELTA_BINARY_PACKED ---------------------------------------------------------------------------------------------
+// (1) walk   one thread per page reads only the block headers (device/cb_delta.h) into the page's miniblock table; entry 0 is the
+//            first value as a delta from zero
+// (2) sum    warp per entry: sum of its deltas (min delta + packed)
+// (3) carry  block per page: exclusive scan of the sums -> each entry's carry
+// (4) decode warp per entry: unpack again, warp prefix sum + carry, convert, store into the same dense buffer PLAIN pages use
+// The packed bytes are read twice and the values written once; all arithmetic wraps in 64 bits, an INT32 page keeps the low 32.
+
+// the i-th packed delta of an entry: two aligned words when 16 bytes of the body remain, else byte by byte (cb_delta.h)
+__device__ __forceinline__ u64 dbp_get(const PqMiniblock& m, int i) {
+    const int bw = m.bit_width;
+    if (bw == 0) return 0;
+    const long long bit = (long long)i * bw, byte = bit >> 3;
+    if (byte + 16 > m.nbytes) return dbp_unpack(m.src, m.nbytes, i, bw);
+    const int sh = (int)(bit & 7);
+    const u64 lo = load_u64_unaligned(m.src + byte); // aligned words inside [body - 7, body + nbytes): the page's own bytes
+    const u64 hi = m.src[byte + 8];
+    const u64 v = (lo >> sh) | (sh ? hi << (64 - sh) : 0ull);
+    return bw == 64 ? v : v & ((1ull << bw) - 1ull);
+}
+
+__global__ void k_pq_dbp_walk(PqPage* pages, int n_pages, PqMiniblock* table, int type_bits, int* err) {
+    const int pi = blockIdx.x * blockDim.x + threadIdx.x;
+    if (pi >= n_pages) return;
+    const PqPage pg = pages[pi];
+    if (pg.encoding != PQ_ENC_DBP) return;
+    PqMiniblock* t = table + pg.mb_base;
+    const int cap = pg.mb_cap;
+    const u8* end = pg.values + pg.values_bytes;
+    DbpHeader h;
+    int n = 0;
+    bool bad = dbp_header(pg.values, end, h) != 0 || h.total != (long long)pg.nonnull; // the header must count exactly the non-null values
+    if (!bad && h.total > 0) {
+        PqMiniblock first;
+        first.src = nullptr; first.min_delta = (i64)h.first; first.carry = 0; first.out_idx = 0; first.count = 1; first.bit_width = 0; first.nbytes = 0;
+        if (cap > 0) t[0] = first;
+        n = 1;
+        const u8* e = dbp_walk(h, end, type_bits, [&](long long idx, long long cnt, int bw, u64 min_delta, const u8* src, long long nbytes) {
+            if (n < cap) {
+                PqMiniblock m;
+                m.src = src; m.min_delta = (i64)min_delta; m.carry = 0; m.out_idx = (int)idx; m.count = (int)cnt; m.bit_width = bw; m.nbytes = (int)nbytes;
+                t[n] = m;
+            }
+            n++;
+        });
+        bad = e == nullptr || n > cap;
+    }
+    if (bad) { atomicOr(err, PQ_ERR_DELTA); n = 0; }
+    pages[pi].mb_count = n;
+}
+
+__global__ void k_pq_dbp_sum(const PqPage* pages, PqMiniblock* table) {
+    const PqPage pg = pages[blockIdx.y];
+    if (pg.encoding != PQ_ENC_DBP) return;
+    PqMiniblock* t = table + pg.mb_base;
+    const int lane = threadIdx.x & 31, warps_per_block = blockDim.x >> 5;
+    for (int e = blockIdx.x * warps_per_block + (threadIdx.x >> 5); e < pg.mb_count; e += gridDim.x * warps_per_block) {
+        const PqMiniblock m = t[e];
+        u64 s = 0;
+        for (int i = lane; i < m.count; i += 32) s += (u64)m.min_delta + dbp_get(m, i);
+        for (int d = 16; d > 0; d >>= 1) s += __shfl_xor_sync(0xffffffffu, s, d);
+        if (lane == 0) t[e].carry = (i64)s;
+    }
+}
+
+__global__ void k_pq_dbp_carry(const PqPage* pages, PqMiniblock* table) {
+    const PqPage pg = pages[blockIdx.x];
+    if (pg.encoding != PQ_ENC_DBP) return;
+    __shared__ u64 warp_sums[8];
+    PqMiniblock* t = table + pg.mb_base;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    u64 carry = 0;
+    for (int base = 0; base < pg.mb_count; base += 256) {
+        const int e = base + threadIdx.x;
+        const u64 s = e < pg.mb_count ? (u64)t[e].carry : 0ull;
+        u64 incl = s;
+        for (int d = 1; d < 32; d <<= 1) { const u64 x = __shfl_up_sync(0xffffffffu, incl, d); if (lane >= d) incl += x; }
+        if (lane == 31) warp_sums[warp] = incl;
+        __syncthreads();
+        u64 wbase = 0, total = 0;
+        for (int w = 0; w < 8; w++) { if (w < warp) wbase += warp_sums[w]; total += warp_sums[w]; }
+        if (e < pg.mb_count) t[e].carry = (i64)(carry + wbase + incl - s);
+        carry += total;
+        __syncthreads();
+    }
+}
+
+template <int CONV> __global__ void k_pq_dbp_decode(const PqPage* pages, const PqMiniblock* table, u8* out) {
+    const PqPage pg = pages[blockIdx.y];
+    if (pg.encoding != PQ_ENC_DBP) return;
+    const PqMiniblock* t = table + pg.mb_base;
+    const int lane = threadIdx.x & 31, warps_per_block = blockDim.x >> 5;
+    for (int e = blockIdx.x * warps_per_block + (threadIdx.x >> 5); e < pg.mb_count; e += gridDim.x * warps_per_block) {
+        const PqMiniblock m = t[e];
+        u64 run = (u64)m.carry;
+        for (int base = 0; base < m.count; base += 32) {
+            const int i = base + lane;
+            const u64 d = i < m.count ? (u64)m.min_delta + dbp_get(m, i) : 0ull;
+            u64 incl = d;
+            for (int k = 1; k < 32; k <<= 1) { const u64 x = __shfl_up_sync(0xffffffffu, incl, k); if (lane >= k) incl += x; }
+            if (i < m.count) {
+                const u64 v = run + incl;
+                const long long row = pg.dst_row + m.out_idx + i;
+                if (CONV == PQ_COPY32) ((u32*)out)[row] = (u32)v;
+                else if (CONV == PQ_COPY64) ((u64*)out)[row] = v;
+                else ((i64*)out)[row] = (i64)(i32)(u32)v; // PQ_I32_TO_I64: wraps at 2^32, then widens
+            }
+            run += __shfl_sync(0xffffffffu, incl, 31);
+        }
+    }
+}
+
+void launch_pq_dbp(PqPage* pages, int n_pages, PqMiniblock* table, int conv, void* out, int* err, cudaStream_t st) {
+    if (n_pages <= 0) return;
+    const int type_bits = conv == PQ_COPY64 ? 64 : 32;
+    k_pq_dbp_walk<<<(n_pages + 63) / 64, 64, 0, st>>>(pages, n_pages, table, type_bits, err);
+    const dim3 grid(32, (unsigned)n_pages), block(256);
+    k_pq_dbp_sum<<<grid, block, 0, st>>>(pages, table);
+    k_pq_dbp_carry<<<n_pages, 256, 0, st>>>(pages, table);
+    if (conv == PQ_COPY32) k_pq_dbp_decode<PQ_COPY32><<<grid, block, 0, st>>>(pages, table, (u8*)out);
+    else if (conv == PQ_COPY64) k_pq_dbp_decode<PQ_COPY64><<<grid, block, 0, st>>>(pages, table, (u8*)out);
+    else k_pq_dbp_decode<PQ_I32_TO_I64><<<grid, block, 0, st>>>(pages, table, (u8*)out);
 }
 
 // ---- RLE / bit-packed hybrid ------------------------------------------------------------------------------------------
@@ -541,7 +689,7 @@ template <bool LEVELS> __global__ void k_pq_rle_scan(const PqPage* pages, int n_
     int pi = blockIdx.x * blockDim.x + threadIdx.x;
     if (pi >= n_pages) return;
     const PqPage pg = pages[pi];
-    if (LEVELS ? pg.def_bytes <= 0 : pg.encoding == 0) { run_counts[pi] = 0; return; }
+    if (LEVELS ? pg.def_bytes <= 0 : pg.encoding != PQ_ENC_DICT) { run_counts[pi] = 0; return; }
     const u8* p = LEVELS ? pg.def_ptr : pg.values;
     const u8* end = p + (LEVELS ? pg.def_bytes : pg.values_bytes);
     int bw = 1;
@@ -584,7 +732,7 @@ template <int DW> __device__ __forceinline__ void store_dict(const void* dict, i
 // one warp per run; blockIdx.y = page
 template <int DW> __global__ void k_pq_rle_decode(const PqPage* pages, const PqRun* runs, const int* run_counts, const void* dict_all, void* out, int* err) {
     const PqPage pg = pages[blockIdx.y];
-    if (pg.encoding == 0) return;
+    if (pg.encoding != PQ_ENC_DICT) return;
     const void* dict = (const u8*)dict_all + (size_t)pg.dict_off * DW;
     const int dict_size = pg.dict_size;
     const int n_runs = run_counts[blockIdx.y];

@@ -1,4 +1,4 @@
-// parquet_kernels.h -- device-side Parquet page decode: Snappy decompression, PLAIN, RLE_DICTIONARY, definition
+// parquet_kernels.h -- device-side Parquet page decode: Snappy decompression, PLAIN, BYTE_STREAM_SPLIT, DELTA_BINARY_PACKED, RLE_DICTIONARY, definition
 // levels (validity + NULL scatter).
 #pragma once
 #include "parquet_pages.h"
@@ -16,8 +16,11 @@ void launch_pq_copy(void* dst, const void* src, size_t bytes, cudaStream_t st);
 void launch_pq_snappy_segmented(PqPage* pages_dev, int n_pages, unsigned* ckpt_dev, int n_segs_total, int* err, cudaStream_t st);
 // locate levels / values inside every page body; nonnull = num_values
 void launch_pq_resolve(PqPage* pages_dev, int n_pages, cudaStream_t st);
-// PLAIN fixed-width pages -> out[dst_row + k] for the page's k-th encoded value (element width given by the conversion)
+// PLAIN and BYTE_STREAM_SPLIT fixed-width pages -> out[dst_row + k] for the page's k-th encoded value (element width given by the conversion)
 void launch_pq_plain(const PqPage* pages_dev, int n_pages, int conv, int flba_len, void* out, int* err, cudaStream_t st);
+// DELTA_BINARY_PACKED INT32 / INT64 pages (conv PQ_COPY32 / PQ_COPY64 / PQ_I32_TO_I64) -> out[dst_row + k], like PLAIN.  `table` holds
+// every page's miniblock entries at [mb_base, mb_base + mb_cap); four launches (header walk, sums, carries, decode)
+void launch_pq_dbp(PqPage* pages_dev, int n_pages, PqMiniblock* table, int conv, void* out, int* err, cudaStream_t st);
 // RLE_DICTIONARY pages: (1) scan run headers, one thread per page
 void launch_pq_rle_scan(const PqPage* pages_dev, int n_pages, PqRun* runs, int* run_counts, int* err, cudaStream_t st);
 // (2) decode runs (warp per run) and gather through the dictionary: dict_width 4/8/16 bytes per entry

@@ -17,7 +17,13 @@ enum PqErr {
     PQ_ERR_DICT_INDEX = 4,        // dictionary index out of range
     PQ_ERR_SNAPPY = 8,            // malformed Snappy page
     PQ_ERR_TRUNCATED = 16,        // fewer encoded values than the page header declares
+    PQ_ERR_DELTA = 32,            // malformed DELTA_BINARY_PACKED page (sizes, bit width, value count, body past the page, table overflow)
+    PQ_ERR_BSS = 64,              // BYTE_STREAM_SPLIT page whose size is not (non-null values) x (value width)
 };
+
+// PqPage::encoding: the Parquet value encoding the device decodes the page by.  Pages the host re-encoded (strings, DELTA_BYTE_ARRAY
+// decimals) are PQ_ENC_PLAIN; PLAIN_DICTIONARY pages are PQ_ENC_DICT.
+enum { PQ_ENC_PLAIN = 0, PQ_ENC_DBP = 5, PQ_ENC_DICT = 8, PQ_ENC_BSS = 9 };
 
 // One page of a column chunk resident on the device.  The host fills what the page HEADER tells it; everything
 // that lives inside the (possibly compressed) page body is resolved on the device by k_pq_resolve.
@@ -34,7 +40,7 @@ struct PqPage {
     long long dst_row;            // first output row of this page
     int num_values;               // rows of the page (incl. NULLs)
     int nonnull;                  // resolved: encoded values present
-    int encoding;                 // 0 PLAIN, 8 RLE_DICTIONARY (2 PLAIN_DICTIONARY is the same on the wire)
+    int encoding;                 // PQ_ENC_*
     long long run_base;           // value runs: first entry of this page in the run table, capacity
     int max_runs;
     long long def_run_base;       // definition-level runs (NULL-aware path)
@@ -43,6 +49,21 @@ struct PqPage {
     int dict_size;
     int seg_base;                 // Snappy pages: first entry of this page in the column's checkpoint table (one entry per 64 KB of output)
     int n_segs;
+    long long mb_base;            // DELTA_BINARY_PACKED: first entry of this page in the column's miniblock table, capacity (num_values / 32 + 2),
+    int mb_cap;                   //   entries the header walk wrote
+    int mb_count;
+};
+
+// One DELTA_BINARY_PACKED miniblock, written by the header walk.  Entry 0 of a page is the first value, stored as a lone delta from
+// zero, so every value of the page is a prefix sum of deltas; `carry` is the sum of all deltas before the entry's first value.
+struct PqMiniblock {
+    const unsigned char* src;     // packed deltas
+    long long min_delta;
+    long long carry;
+    int out_idx;                  // index of the entry's first value within the page's non-null values
+    int count;                    // values
+    int bit_width;
+    int nbytes;                   // body bytes (the packed deltas are read inside them only)
 };
 
 struct PqRun {              // one run of the RLE / bit-packed hybrid

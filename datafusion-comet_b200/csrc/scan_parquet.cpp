@@ -2,7 +2,8 @@
 // native/core/src/parquet/parquet_exec.rs:60-200): the device pipeline over the host plans of scan_plan.cpp.
 //
 // Footers and page headers are parsed on the host (parquet.cpp, scan_plan.cpp); encoded pages cross PCIe as they sit in the file and
-// every value byte is decoded on the device (parquet_kernels.cu).  d(p<=18) / INT64 decimals stay 8 bytes wide in HBM (the Parquet
+// every value byte is decoded on the device (parquet_kernels.cu) -- but for strings (turned into dictionary codes on the host) and
+// DELTA_BYTE_ARRAY decimals (sequential by construction, re-encoded as PLAIN on the host).  d(p<=18) / INT64 decimals stay 8 bytes wide in HBM (the Parquet
 // physical width) and the fused kernels read them as such.
 //
 // Memory.  A scan owns two SLOTS that alternate between consecutive batches, so that batch k+1's encoded bytes cross PCIe
@@ -431,6 +432,8 @@ struct NativeScanSource : ExecNode {
         if (perr & PQ_ERR_NULL_ON_FAST_PATH) throw PlanError("parquet: a column chunk whose statistics say null_count = 0 contains NULLs (corrupt statistics)");
         if (perr & PQ_ERR_SNAPPY) throw PlanError("parquet: malformed Snappy page");
         if (perr & PQ_ERR_DICT_INDEX) throw ExecError(3, "", "parquet: dictionary index out of range (corrupt page)");
+        if (perr & PQ_ERR_DELTA) throw PlanError("parquet: malformed DELTA_BINARY_PACKED page (block sizes, bit width, value count or a body past the page)");
+        if (perr & PQ_ERR_BSS) throw PlanError("parquet: BYTE_STREAM_SPLIT page whose size is not (non-null values) x (value width)");
         if (perr & PQ_ERR_TRUNCATED) throw PlanError("parquet: truncated page (fewer encoded values than the page header declares)");
         if (perr & PQ_ERR_RLE) throw Unsupported("parquet: malformed RLE stream, or one with more than n/8 + 64 runs per page");
         out = std::move(cur->batch);
@@ -471,6 +474,10 @@ struct NativeScanSource : ExecNode {
             launch_pq_rle_scan(data_pages, n_data, (PqRun*)cp.runs, (int*)cp.counts, derr, ds);
             launch_pq_rle_decode(data_pages, n_data, (const PqRun*)cp.runs, (const int*)cp.counts, cp.ddict, cp.out_w, dense, derr, ds);
             ctx->kernel_launches += 2;
+        }
+        if (cp.mb_base > 0) { // DELTA_BINARY_PACKED pages: header walk, miniblock sums, carries, decode
+            launch_pq_dbp(data_pages, n_data, (PqMiniblock*)cp.dmb, cp.conv, dense, derr, ds);
+            ctx->kernel_launches += 4;
         }
         if (cp.null_aware) {
             launch_pq_scatter(cp.dvalid, (const unsigned*)cp.didx, dense, cp.out, (unsigned*)cp.validity, total, cp.out_w, ds);

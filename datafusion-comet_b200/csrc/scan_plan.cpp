@@ -1,10 +1,11 @@
 // scan_plan.cpp -- host planning of the native Parquet scan (scan_plan.h).
 //
 // Row groups come from the footers: a file split owns the row groups that start inside it, and the pushed-down filters drop those
-// whose min/max statistics rule them out (parquet_exec.rs:143-196).  Page tables come from the page headers; only string values and
-// pages of the host codecs are touched on the host, every other value byte is decoded on the device.
+// whose min/max statistics rule them out (parquet_exec.rs:143-196).  Page tables come from the page headers; only string values, DELTA_BYTE_ARRAY
+// decimals and pages of the host codecs are touched on the host, every other value byte is decoded on the device.
 #include "scan_plan.h"
 
+#include "device/cb_delta.h"
 #include "device/cb_snappy.h"
 #include "host_codecs.h"
 
@@ -196,17 +197,21 @@ BatchPlan plan_batches(const std::vector<Unit>& units, const std::vector<ScanFil
         for (size_t c = 0; c < fields.size(); c++) {
             const DType& t = fields[c].type;
             const size_t w = t.is_decimal() ? (t.precision <= 18 ? 8 : 16) : t.is_string() ? 4 : (size_t)std::max(t.arrow_width(), 1);
-            bool nulls = false, dict_encoded = false;
+            bool nulls = false, dict_encoded = false, delta = false;
             for (size_t i = b.first; i < b.second; i++) {
                 const ScanFile& f = files[units[i].file];
                 const pq::ColumnChunkMeta& cc = f.chunk(units[i].rg, c);
                 if (f.leaf(c).repetition == 1 && cc.null_count != 0) nulls = true;
-                for (int enc : cc.encodings) if (enc == pq::RLE_DICTIONARY || enc == pq::PLAIN_DICTIONARY) dict_encoded = true;
+                for (int enc : cc.encodings) {
+                    if (enc == pq::RLE_DICTIONARY || enc == pq::PLAIN_DICTIONARY) dict_encoded = true;
+                    if (enc == pq::DELTA_BINARY_PACKED) delta = true;
+                }
             }
             work += (size_t)rows * w + 4096;                                  // decoded column
             work += (b.second - b.first) * 96 * 1024;                         // page tables / dictionaries
             if (dict_encoded) work += (size_t)rows * 4 + (b.second - b.first) * 16 * 2048; // run table: (values / 8 + 64) runs of 32 bytes per page
             if (nulls) work += (size_t)rows * (w + 5 + 4) + 65536;            // dense values + validity bytes + indices + level runs
+            if (delta) work += ((size_t)rows / 16 + (b.second - b.first) * 256) * sizeof(PqMiniblock); // miniblock table: values / 32 + 2 entries per page
         }
         bp.chunk_need = std::max(bp.chunk_need, enc + 65536);
         bp.work_estimate = std::max(bp.work_estimate, work + work / 16);
@@ -344,6 +349,50 @@ struct ByteArrays {
     }
 };
 
+// a DELTA_BINARY_PACKED section of at most `cap` values (device/cb_delta.h) at p, as 32-bit lengths; advances p past it
+std::vector<int32_t> delta_lengths(const uint8_t*& p, const uint8_t* e, long long cap, const char* what) {
+    cb::DbpHeader h;
+    if (cb::dbp_header(p, e, h) != 0 || h.total > cap) throw PlanError(std::string("parquet: malformed DELTA_BINARY_PACKED ") + what);
+    std::vector<cb::i64> v((size_t)h.total + 1);
+    long long n = 0;
+    const uint8_t* q = cb::dbp_decode_serial(p, e, 32, v.data(), cap, &n);
+    if (!q) throw PlanError(std::string("parquet: malformed DELTA_BINARY_PACKED ") + what);
+    p = q;
+    std::vector<int32_t> out((size_t)n);
+    for (long long i = 0; i < n; i++) {
+        out[(size_t)i] = (int32_t)v[(size_t)i];
+        if (out[(size_t)i] < 0) throw PlanError(std::string("parquet: negative length in ") + what);
+    }
+    return out;
+}
+
+// The values of a BYTE_ARRAY / FIXED_LEN_BYTE_ARRAY section in order, in any byte-array value encoding: PLAIN ([u32 length][bytes]),
+// DELTA_LENGTH_BYTE_ARRAY (DELTA_BINARY_PACKED lengths, then the bytes back to back) or DELTA_BYTE_ARRAY (DELTA_BINARY_PACKED prefix
+// lengths, then the suffixes as DELTA_LENGTH_BYTE_ARRAY; a value is the previous value's first `prefix` bytes + its suffix).  At most
+// `cap` values (the page's row count).
+template <typename F> void for_each_byte_array(int encoding, const uint8_t* p, const uint8_t* e, long long cap, F f) {
+    if (encoding == pq::PLAIN) {
+        ByteArrays vals{p, e, "parquet: truncated PLAIN string page"};
+        while (vals.more()) f(vals.next());
+        return;
+    }
+    std::vector<int32_t> prefix;
+    if (encoding == pq::DELTA_BYTE_ARRAY) prefix = delta_lengths(p, e, cap, "prefix lengths");
+    const std::vector<int32_t> len = delta_lengths(p, e, cap, "lengths");
+    if (encoding == pq::DELTA_BYTE_ARRAY && prefix.size() != len.size()) throw PlanError("parquet: DELTA_BYTE_ARRAY prefix and suffix counts differ");
+    std::string v;
+    for (size_t i = 0; i < len.size(); i++) {
+        if ((size_t)len[i] > (size_t)(e - p)) throw PlanError("parquet: truncated DELTA_LENGTH_BYTE_ARRAY / DELTA_BYTE_ARRAY page");
+        if (encoding == pq::DELTA_BYTE_ARRAY) {
+            if ((size_t)prefix[i] > v.size()) throw PlanError("parquet: DELTA_BYTE_ARRAY prefix longer than the previous value");
+            v.resize((size_t)prefix[i]);
+            v.append((const char*)p, (size_t)len[i]);
+        } else v.assign((const char*)p, (size_t)len[i]);
+        p += len[i];
+        f(v);
+    }
+}
+
 // a body kept as an offset until resolve_bodies
 void set_body_offset(PqPage& d, size_t off) { d.body = (unsigned char*)(uintptr_t)off; }
 
@@ -435,10 +484,12 @@ class ColumnPlanner {
         }
     }
 
-    // PLAIN-encoded string page (a writer's dictionary fallback).  Strings live on the device as codes of the plan-wide dictionary
-    // only, so the host -- which already parses every string dictionary page -- turns the page's values into codes: the page
-    // the device sees is [levels as written][int32 codes], PLAIN.
-    void place_plain_strings(PqPage& d, const Section& s) {
+    // String pages that are not dictionary-encoded (PLAIN: a writer's dictionary fallback; DELTA_LENGTH_BYTE_ARRAY / DELTA_BYTE_ARRAY).
+    // Strings live on the device as codes of the plan-wide dictionary only, so the host -- which already parses every string
+    // dictionary page -- turns the page's values into codes: the page the device sees is [levels as written][int32 codes], PLAIN.
+    // DELTA_BYTE_ARRAY decimals (FIXED_LEN_BYTE_ARRAY) are sequential by construction -- every value starts with a prefix of the one
+    // before -- and come out the same way as [levels as written][type_length-byte big-endian values], a PLAIN page.
+    void place_host_values(PqPage& d, const Section& s, int encoding) {
         const auto b = host_section(s, "page");
         size_t pre = 0;
         if (d.flags & PQ_PAGE_V1_LEVELS) { // [u32 byte length][RLE definition levels] stay as they are
@@ -450,14 +501,20 @@ class ColumnPlanner {
         }
         const size_t off = cp.hostdec.size();
         cp.hostdec.insert(cp.hostdec.end(), b.first, b.first + pre);
-        ByteArrays vals{b.first + pre, b.first + b.second, "parquet: truncated PLAIN string page"};
-        while (vals.more()) {
-            const int32_t code = strings.code(vals.next());
-            const uint8_t* code_bytes = (const uint8_t*)&code;
-            cp.hostdec.insert(cp.hostdec.end(), code_bytes, code_bytes + 4);
+        if (se.type == pq::BYTE_ARRAY) {
+            for_each_byte_array(encoding, b.first + pre, b.first + b.second, d.num_values, [&](std::string v) {
+                const int32_t code = strings.code(std::move(v));
+                const uint8_t* code_bytes = (const uint8_t*)&code;
+                cp.hostdec.insert(cp.hostdec.end(), code_bytes, code_bytes + 4);
+            });
+            cp.conv = PQ_COPY32; // k_pq_plain copies the codes of PLAIN pages; dictionary pages of the same column go through k_pq_rle_decode
+        } else {
+            for_each_byte_array(encoding, b.first + pre, b.first + b.second, d.num_values, [&](const std::string& v) {
+                if (v.size() != (size_t)se.type_length) throw PlanError("parquet: DELTA_BYTE_ARRAY value of column '" + field.name + "' is not type_length bytes long");
+                cp.hostdec.insert(cp.hostdec.end(), (const uint8_t*)v.data(), (const uint8_t*)v.data() + v.size());
+            });
         }
         host_body(d, off);
-        cp.conv = PQ_COPY32; // k_pq_plain copies the codes of PLAIN pages; dictionary pages of the same column go through k_pq_rle_decode
     }
 
     void dictionary_page(const pq::PageInfo& pg, const Section& s) {
@@ -493,19 +550,33 @@ class ColumnPlanner {
             d.def_bytes = pg.def_levels_bytes;
             vals = {s.host + lv, s.dev + lv, s.comp - lv, s.unc - lv, pg.v2_compressed ? s.codec : (int)pq::UNCOMPRESSED};
         }
-        if (se.type == pq::BYTE_ARRAY && pg.encoding == pq::PLAIN) place_plain_strings(d, vals);
+        const int enc = pg.encoding;
+        const bool dict = enc == pq::RLE_DICTIONARY || enc == pq::PLAIN_DICTIONARY;
+        const bool fixed_int = se.type == pq::INT32 || se.type == pq::INT64;
+        const bool on_host = (se.type == pq::BYTE_ARRAY && (enc == pq::PLAIN || enc == pq::DELTA_LENGTH_BYTE_ARRAY || enc == pq::DELTA_BYTE_ARRAY)) ||
+                             (se.type == pq::FIXED_LEN_BYTE_ARRAY && enc == pq::DELTA_BYTE_ARRAY);
+        if (!(dict || on_host || enc == pq::PLAIN || (enc == pq::DELTA_BINARY_PACKED && fixed_int) || (enc == pq::BYTE_STREAM_SPLIT && se.type != pq::BYTE_ARRAY)))
+            throw Unsupported("parquet value encoding " + std::to_string(enc) + " on physical type " + std::to_string(se.type) + " (column '" + field.name + "')");
+        if (on_host) place_host_values(d, vals, enc);
         else place_body(d, vals);
-        if (pg.encoding == pq::PLAIN) {
-            d.encoding = 0;
-        } else if (pg.encoding == pq::RLE_DICTIONARY || pg.encoding == pq::PLAIN_DICTIONARY) {
+        if (enc == pq::PLAIN || on_host) {
+            d.encoding = PQ_ENC_PLAIN;
+        } else if (enc == pq::DELTA_BINARY_PACKED) {
+            d.encoding = PQ_ENC_DBP;
+            d.mb_base = cp.mb_base;
+            d.mb_cap = (int)(pg.num_values / 32 + 2); // entry 0 = the first value, then miniblocks of >= 32 values each
+            cp.mb_base += d.mb_cap;
+        } else if (enc == pq::BYTE_STREAM_SPLIT) {
+            d.encoding = PQ_ENC_BSS;
+        } else {
             if (dict_off < 0) throw PlanError("parquet: dictionary-encoded page without a dictionary page");
-            d.encoding = 8;
+            d.encoding = PQ_ENC_DICT;
             d.run_base = cp.run_base;
             d.max_runs = (int)(pg.num_values / 8 + 64);
             d.dict_off = dict_off;
             d.dict_size = dict_size;
             cp.run_base += d.max_runs;
-        } else throw Unsupported("parquet value encoding " + std::to_string(pg.encoding) + " (DELTA_* / BYTE_STREAM_SPLIT are next-row work)");
+        }
         if (optional) {
             d.def_run_base = cp.def_run_base;
             d.def_max_runs = (int)(pg.num_values / 8 + 64);
@@ -550,6 +621,7 @@ void buffer_requests(ColPlan& cp, int64_t total, std::vector<std::pair<uint8_t**
         cp.validity_bytes = (n + 31) / 32 * 4 + 16;
         reqs.push_back({&cp.validity, cp.validity_bytes});
     }
+    if (cp.mb_base > 0) reqs.push_back({&cp.dmb, (size_t)cp.mb_base * sizeof(PqMiniblock)});
     if (cp.run_base > 0) {
         reqs.push_back({&cp.runs, (size_t)cp.run_base * sizeof(PqRun)});
         reqs.push_back({&cp.counts, cp.n_data * 4 + 16});

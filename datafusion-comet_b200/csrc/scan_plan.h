@@ -88,13 +88,14 @@ struct ColPlan {
     size_t n_data = 0, n_dict_pages = 0;
     std::vector<int32_t> remap;   // string columns: combined code remap tables
     int64_t run_base = 0, def_run_base = 0, dict_elems = 0;
+    int64_t mb_base = 0;          // DELTA_BINARY_PACKED: miniblock table entries over all pages
     size_t unc_bytes = 0;
     int64_t n_segs_total = 0;     // Snappy: 64 KB output segments over all compressed pages (checkpoint table entries)
     std::vector<uint8_t> hostdec; // page bodies produced on the host, 16-byte aligned each; shipped with the page tables
     bool optional = false, null_aware = false, any_compressed = false;
     // device buffers, bound by the scan (buffer_requests)
     uint8_t *out = nullptr, *dunc = nullptr, *dpd = nullptr, *ddict = nullptr, *dense = nullptr, *dvalid = nullptr, *didx = nullptr, *druns = nullptr,
-            *dcounts = nullptr, *validity = nullptr, *runs = nullptr, *counts = nullptr, *dckpt = nullptr;
+            *dcounts = nullptr, *validity = nullptr, *runs = nullptr, *counts = nullptr, *dckpt = nullptr, *dmb = nullptr;
     size_t out_bytes = 0, validity_bytes = 0;
 };
 

@@ -28,7 +28,7 @@ static std::string hex(const std::string& s) {
 // one column of one batch: its page table (data pages first), and for host-encoded PLAIN string pages the codes they carry
 static void column_json(std::ostringstream& o, ColPlan& cp) {
     resolve_bodies(cp, cp.hostdec.data()); // host-produced bodies now point into cp.hostdec
-    o << "{\"conv\": " << cp.conv << ", \"n_data\": " << cp.n_data << ", \"dict_elems\": " << cp.dict_elems << ", \"remap\": [";
+    o << "{\"conv\": " << cp.conv << ", \"mb_entries\": " << cp.mb_base << ", \"n_data\": " << cp.n_data << ", \"dict_elems\": " << cp.dict_elems << ", \"remap\": [";
     for (size_t i = 0; i < cp.remap.size(); i++) o << (i ? ", " : "") << cp.remap[i];
     o << "], \"pages\": [";
     for (size_t i = 0; i < cp.pages.size(); i++) {
@@ -42,6 +42,12 @@ static void column_json(std::ostringstream& o, ColPlan& cp) {
             o << ", \"codes\": [";
             for (size_t k = pre; k + 4 <= (size_t)d.body_bytes; k += 4) { int32_t v; memcpy(&v, d.body + k, 4); o << (k > pre ? ", " : "") << v; }
             o << "]";
+        }
+        if (d.encoding == PQ_ENC_DBP) o << ", \"mb_base\": " << d.mb_base << ", \"mb_cap\": " << d.mb_cap;
+        if ((cp.conv == PQ_FLBA_TO_I64 || cp.conv == PQ_FLBA_TO_I128) && (d.flags & PQ_PAGE_HOSTDEC)) { // decimal page re-encoded (DELTA_BYTE_ARRAY) or decompressed on the host
+            o << ", \"body\": \"";
+            for (int k = 0; k < d.body_bytes; k++) { static const char* hx = "0123456789abcdef"; o << hx[d.body[k] >> 4] << hx[d.body[k] & 15]; }
+            o << "\"";
         }
         o << "}";
     }
