@@ -355,6 +355,8 @@ int cb200_plan_stats(cb200_plan* plan, cb200_stats* out) {
     out->scan_pruned_row_groups = c.scan_pruned_row_groups;
     out->scan_pruned_rows = c.scan_pruned_rows;
     out->agg_strategies = c.agg_strategies;
+    out->scan_pruned_pages = c.scan_pruned_pages;
+    out->scan_page_pruned_rows = c.scan_page_pruned_rows;
     return 0;
 }
 

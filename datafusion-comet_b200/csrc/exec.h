@@ -102,6 +102,7 @@ struct ExecContext {
     int64_t pipeline_rows = 0;    // rows those launches scanned
     int64_t h2d_bytes = 0, d2h_bytes = 0;
     int64_t scan_pruned_row_groups = 0, scan_pruned_rows = 0; // Parquet row groups skipped by statistics (parquet_exec.rs:143-196)
+    int64_t scan_pruned_pages = 0, scan_page_pruned_rows = 0;  // data pages / rows of kept row groups skipped by the page index
     int64_t agg_strategies = 0;   // CB200_AGG_* bits of the aggregate strategies that ran
     std::vector<int64_t> partition_starts; // last ShuffleWriter batch: partition p = rows [starts[p], starts[p+1])
     void check_device_errors();

@@ -2,6 +2,8 @@
 #include "parquet.h"
 #include "exec.h"
 
+#include <algorithm>
+#include <cstdint>
 #include <cstdio>
 #include <cstring>
 #include <sstream>
@@ -185,12 +187,67 @@ ColumnChunkMeta parse_column_meta(TReader& r) {
 
 ColumnChunkMeta parse_column_chunk(TReader& r) {
     ColumnChunkMeta m;
+    int64_t oi_off = -1, ci_off = -1;
+    int32_t oi_len = 0, ci_len = 0;
     FOR_FIELDS(r) {
-        if (fid == 3) m = parse_column_meta(r);
-        else r.skip(t);
+        switch (fid) {
+        case 3: m = parse_column_meta(r); break;
+        case 4: oi_off = r.zigzag(); break;
+        case 5: oi_len = (int32_t)r.zigzag(); break;
+        case 6: ci_off = r.zigzag(); break;
+        case 7: ci_len = (int32_t)r.zigzag(); break;
+        default: r.skip(t);
+        }
         last = fid;
     }
+    m.offset_index_offset = oi_off;
+    m.offset_index_length = oi_len;
+    m.column_index_offset = ci_off;
+    m.column_index_length = ci_len;
     return m;
+}
+
+// the index of one column chunk is used only if it tiles the chunk: pages inside [start, start + total_compressed) in file order,
+// first rows 0 = f0 < f1 < ... < num_rows, and a ColumnIndex entry per page
+bool offset_index_valid(const ColumnChunkMeta& cc, int64_t num_rows) {
+    const auto& loc = cc.offset_index;
+    if (loc.empty() || loc[0].first_row_index != 0) return false;
+    const int64_t lo = cc.start(), hi = lo + cc.total_compressed;
+    int64_t prev_end = lo;
+    for (size_t i = 0; i < loc.size(); i++) {
+        if (loc[i].compressed_page_size <= 0 || loc[i].offset < prev_end || loc[i].offset + loc[i].compressed_page_size > hi) return false;
+        if (loc[i].first_row_index >= num_rows || (i && loc[i].first_row_index <= loc[i - 1].first_row_index)) return false;
+        prev_end = loc[i].offset + loc[i].compressed_page_size;
+    }
+    return true;
+}
+
+void load_page_indexes(FileMeta& m, const uint8_t* span, int64_t span_lo, int64_t span_hi) {
+    for (auto& rg : m.row_groups)
+        for (auto& cc : rg.columns) {
+            auto in_span = [&](int64_t off, int32_t len) { return off >= span_lo && len > 0 && off + len <= span_hi; };
+            if (in_span(cc.offset_index_offset, cc.offset_index_length)) {
+                try { cc.offset_index = parse_offset_index(span + (cc.offset_index_offset - span_lo), (size_t)cc.offset_index_length); }
+                catch (const PlanError&) { cc.offset_index.clear(); }
+                if (!offset_index_valid(cc, rg.num_rows)) cc.offset_index.clear();
+            }
+            if (!cc.offset_index.empty() && in_span(cc.column_index_offset, cc.column_index_length)) {
+                try { cc.column_index = parse_column_index(span + (cc.column_index_offset - span_lo), (size_t)cc.column_index_length); }
+                catch (const PlanError&) { cc.column_index = ColumnIndex(); }
+                if (cc.column_index.null_pages.size() != cc.offset_index.size()) cc.column_index = ColumnIndex();
+            }
+        }
+}
+
+// [lo, hi): the bytes that hold every page index of the file (they sit together in front of the footer); false if there are none
+bool page_index_span(const FileMeta& m, int64_t file_size, int64_t* lo, int64_t* hi) {
+    *lo = INT64_MAX;
+    *hi = -1;
+    for (auto& rg : m.row_groups)
+        for (auto& cc : rg.columns)
+            for (auto [off, len] : {std::pair<int64_t, int64_t>{cc.offset_index_offset, cc.offset_index_length}, {cc.column_index_offset, cc.column_index_length}})
+                if (off >= 0 && len > 0 && off + len <= file_size) { *lo = std::min(*lo, off); *hi = std::max(*hi, off + len); }
+    return *hi > *lo && *hi - *lo <= ((int64_t)1 << 30);
 }
 
 RowGroupMeta parse_row_group(TReader& r) {
@@ -257,6 +314,73 @@ FileMeta read_footer(const std::string& path, int64_t* file_size) {
     }
     fclose(f);
     return parse_footer(tail.data(), tail.size());
+}
+
+// OffsetIndex: 1 page_locations list<PageLocation{1 offset, 2 compressed_page_size, 3 first_row_index}>
+std::vector<PageLocation> parse_offset_index(const uint8_t* p, size_t len) {
+    TReader r{p, p + len};
+    std::vector<PageLocation> out;
+    FOR_FIELDS(r) {
+        if (fid == 1 && t == 9) {
+            int et;
+            const uint32_t n = r.list_of(&et);
+            if (et != 12) throw PlanError("parquet: OffsetIndex page_locations is not a list of structs");
+            for (uint32_t i = 0; i < n; i++) {
+                PageLocation pl;
+                int16_t f2 = 0, l2 = 0; int t2;
+                while ((t2 = r.field(&f2, l2)) != 0) {
+                    if (f2 == 1) pl.offset = r.zigzag();
+                    else if (f2 == 2) pl.compressed_page_size = (int32_t)r.zigzag();
+                    else if (f2 == 3) pl.first_row_index = r.zigzag();
+                    else r.skip(t2);
+                    l2 = f2;
+                }
+                out.push_back(pl);
+            }
+        } else r.skip(t);
+        last = fid;
+    }
+    return out;
+}
+
+// ColumnIndex: 1 null_pages list<bool>, 2 min_values / 3 max_values list<binary>, 4 boundary_order, 5 null_counts (not used).  The lists
+// must be equally long, or the index is not used.
+ColumnIndex parse_column_index(const uint8_t* p, size_t len) {
+    TReader r{p, p + len};
+    ColumnIndex ci;
+    FOR_FIELDS(r) {
+        int et;
+        if (fid == 1 && t == 9) {
+            const uint32_t n = r.list_of(&et);
+            if (et != 1 && et != 2) throw PlanError("parquet: ColumnIndex null_pages is not a list of bools");
+            for (uint32_t i = 0; i < n; i++) ci.null_pages.push_back(*r.p++ == 1); // a bool in a list is one byte: 1 true, anything else false
+        } else if ((fid == 2 || fid == 3) && t == 9) {
+            const uint32_t n = r.list_of(&et);
+            if (et != 8) throw PlanError("parquet: ColumnIndex min / max values are not binary");
+            auto& v = fid == 2 ? ci.min_values : ci.max_values;
+            for (uint32_t i = 0; i < n; i++) v.push_back(r.binary());
+        } else r.skip(t);
+        last = fid;
+    }
+    if (ci.min_values.size() != ci.null_pages.size() || ci.max_values.size() != ci.null_pages.size()) throw PlanError("parquet: ColumnIndex lists differ in length");
+    return ci;
+}
+
+void read_page_indexes(FileMeta& m, const uint8_t* file, size_t file_len) {
+    int64_t lo, hi;
+    if (page_index_span(m, (int64_t)file_len, &lo, &hi)) load_page_indexes(m, file + lo, lo, hi);
+}
+
+void read_page_indexes(FileMeta& m, const std::string& path, int64_t file_size) {
+    int64_t lo, hi;
+    if (!page_index_span(m, file_size, &lo, &hi)) return;
+    std::vector<uint8_t> span((size_t)(hi - lo));
+    FILE* f = fopen(path.c_str(), "rb");
+    if (!f) throw ExecError(3, "", "parquet: cannot open " + path);
+    const bool ok = fseeko(f, (off_t)lo, SEEK_SET) == 0 && fread(span.data(), 1, span.size(), f) == span.size();
+    fclose(f);
+    if (!ok) throw ExecError(3, "", "parquet: short read on " + path);
+    load_page_indexes(m, span.data(), lo, hi);
 }
 
 std::vector<PageInfo> walk_pages(const uint8_t* chunk, size_t len, int64_t num_values) {

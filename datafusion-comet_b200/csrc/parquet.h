@@ -30,6 +30,18 @@ struct SchemaElement {
     bool logical_decimal = false;
     std::string name;
 };
+// OffsetIndex.page_locations (parquet.thrift): where one data page of a column chunk sits, header included, and its first row
+struct PageLocation {
+    int64_t offset = 0;
+    int32_t compressed_page_size = 0;
+    int64_t first_row_index = 0;
+};
+// ColumnIndex (parquet.thrift): per data page, whether it holds only NULLs and its min / max (PLAIN-encoded, like chunk statistics;
+// meaningless for an all-NULL page)
+struct ColumnIndex {
+    std::vector<uint8_t> null_pages;
+    std::vector<std::string> min_values, max_values;
+};
 struct ColumnChunkMeta {
     int type = 0, codec = 0;
     std::vector<int> encodings;
@@ -38,6 +50,12 @@ struct ColumnChunkMeta {
     int64_t null_count = -1; // statistics, -1 unknown
     bool has_min_max = false; // statistics min_value / max_value (fields 5, 6: the type's own sort order), PLAIN-encoded
     std::string min_value, max_value;
+    int64_t offset_index_offset = -1, column_index_offset = -1; // ColumnChunk fields 4-7: the page index, stored outside the footer
+    int32_t offset_index_length = 0, column_index_length = 0;
+    // the page index as read_page_indexes left it: empty unless present and valid (offset_index: pages inside the chunk, first rows
+    // 0 < ... < num_rows; column_index: as many pages as offset_index)
+    std::vector<PageLocation> offset_index;
+    ColumnIndex column_index;
     int64_t start() const { return dictionary_page_offset > 0 && dictionary_page_offset < data_page_offset ? dictionary_page_offset : data_page_offset; }
 };
 struct RowGroupMeta {
@@ -68,6 +86,12 @@ struct PageInfo {
 
 FileMeta parse_footer(const uint8_t* file, size_t file_len);               // whole file image or at least its tail
 FileMeta read_footer(const std::string& path, int64_t* file_size);
+// The page indexes of every column chunk that has them, from the whole file image / from the file.  An index that does not parse
+// or fails validation is left out: that chunk is read whole.
+void read_page_indexes(FileMeta& m, const uint8_t* file, size_t file_len);
+void read_page_indexes(FileMeta& m, const std::string& path, int64_t file_size);
+std::vector<PageLocation> parse_offset_index(const uint8_t* p, size_t len);
+ColumnIndex parse_column_index(const uint8_t* p, size_t len);
 // walk the page headers of one column chunk (bytes = the chunk, [0, total_compressed))
 std::vector<PageInfo> walk_pages(const uint8_t* chunk, size_t len, int64_t num_values);
 std::string describe(const FileMeta& m); // JSON, for tests

@@ -862,4 +862,56 @@ void launch_pq_scatter(const unsigned char* valid, const unsigned* idx, const vo
     else k_pq_scatter<16><<<blocks, 256, 0, st>>>(valid, idx, (const u8*)dense, (u8*)out, bitmap, total);
 }
 
+// ---- page-pruned columns ----------------------------------------------------------------------------------------------------
+// The pages of a page-pruned column were decoded into covered rows; out[row] takes covered row segs[s].cov_row + (row - segs[s].out_row)
+// for the segment s that holds `row`.  NULLABLE (the NULL-aware path): valid / idx are read at the covered row, NULL slots are zeroed
+// and the Arrow bitmap is built, as k_pq_scatter does for unpruned columns.  Every warp takes a contiguous tile of rows: one binary search
+// for the tile's first row, then each lane walks forward.
+template <int W, bool NULLABLE>
+__global__ void k_pq_select(const PqSeg* segs, int n_segs, long long total, const u8* valid, const u32* idx, const u8* src, u8* out, u32* bitmap) {
+    const int lane = threadIdx.x & 31;
+    const long long n32 = (total + 31) / 32 * 32;
+    const long long warps = (long long)gridDim.x * (blockDim.x >> 5), warp = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5;
+    const long long tile = (n32 / 32 + warps - 1) / warps * 32;
+    const long long r0 = warp * tile, r1 = r0 + tile < n32 ? r0 + tile : n32;
+    if (r0 >= r1) return;
+    int lo = 0, hi = n_segs - 1; // the last segment starting at or before r0
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (segs[mid].out_row <= r0) lo = mid;
+        else hi = mid - 1;
+    }
+    int s = lo;
+    for (long long row = r0 + lane; row - lane < r1; row += 32) {
+        bool ok = false;
+        if (row < total) {
+            while (s + 1 < n_segs && segs[s + 1].out_row <= row) s++;
+            const long long cov = segs[s].cov_row + (row - segs[s].out_row);
+            ok = NULLABLE ? valid[cov] != 0 : true;
+            const long long at = NULLABLE ? (long long)idx[cov] : cov;
+            if (W == 4) ((u32*)out)[row] = ok ? ((const u32*)src)[at] : 0u;
+            else if (W == 8) ((u64*)out)[row] = ok ? ((const u64*)src)[at] : 0ull;
+            else ((ulonglong2*)out)[row] = ok ? ((const ulonglong2*)src)[at] : make_ulonglong2(0ull, 0ull);
+        }
+        if (NULLABLE) {
+            const u32 word = __ballot_sync(0xffffffffu, ok);
+            if (lane == 0) bitmap[(row - lane) >> 5] = word;
+        }
+    }
+}
+template <bool NULLABLE>
+static void select_width(const PqSeg* segs, int n_segs, long long total, const u8* valid, const u32* idx, const u8* src, u8* out, u32* bitmap, int width,
+                         cudaStream_t st) {
+    const int blocks = (int)std::min<long long>((total + 255) / 256, 132 * 16); // 16 CTAs per H100 SM, each warp a tile of >= 32 rows
+    if (width == 4) k_pq_select<4, NULLABLE><<<blocks, 256, 0, st>>>(segs, n_segs, total, valid, idx, src, out, bitmap);
+    else if (width == 8) k_pq_select<8, NULLABLE><<<blocks, 256, 0, st>>>(segs, n_segs, total, valid, idx, src, out, bitmap);
+    else k_pq_select<16, NULLABLE><<<blocks, 256, 0, st>>>(segs, n_segs, total, valid, idx, src, out, bitmap);
+}
+void launch_pq_select(const PqSeg* segs, int n_segs, long long total, const unsigned char* valid, const unsigned* idx, const void* src, void* out, unsigned* bitmap,
+                      int width, cudaStream_t st) {
+    if (total <= 0 || n_segs <= 0) return;
+    if (valid) select_width<true>(segs, n_segs, total, valid, idx, (const u8*)src, (u8*)out, bitmap, width, st);
+    else select_width<false>(segs, n_segs, total, nullptr, nullptr, (const u8*)src, (u8*)out, nullptr, width, st);
+}
+
 } // namespace cb200

@@ -33,5 +33,9 @@ void launch_pq_check_def_levels(const PqPage* pages_dev, int n_pages, int* err, 
 void launch_pq_def_levels(PqPage* pages_dev, int n_pages, PqRun* runs, int* run_counts, unsigned char* valid, unsigned* idx, int* err, cudaStream_t st);
 //   out[row] = valid[row] ? dense[idx[row]] : 0 ; bitmap = Arrow validity (total rows, width 4/8/16 bytes)
 void launch_pq_scatter(const unsigned char* valid, const unsigned* idx, const void* dense, void* out, unsigned* bitmap, long long total, int width, cudaStream_t st);
+// page-pruned columns: out[row] = the covered row segs map `row` to, for total output rows (width 4/8/16 bytes).  valid == nullptr: `src`
+// holds the covered rows' values.  Otherwise the NULL-aware path in covered rows: out[row] = valid[c] ? src[idx[c]] : 0 and the Arrow bitmap
+void launch_pq_select(const PqSeg* segs, int n_segs, long long total, const unsigned char* valid, const unsigned* idx, const void* src, void* out, unsigned* bitmap,
+                      int width, cudaStream_t st);
 
 } // namespace cb200

@@ -75,6 +75,14 @@ struct PqRun {              // one run of the RLE / bit-packed hybrid
     int bit_width;
 };
 
+// One run of consecutive output rows of a page-pruned column: output rows [out_row, out_row + count) are its decoded ("covered") rows
+// [cov_row, cov_row + count).  A column's segments are sorted by out_row and tile its output rows.
+struct PqSeg {
+    long long out_row;
+    long long cov_row;
+    long long count;
+};
+
 enum PqConv { PQ_COPY32, PQ_COPY64, PQ_I32_TO_I64, PQ_FLBA_TO_I64, PQ_FLBA_TO_I128 };
 
 // segmented Snappy decoder: one checkpoint table entry per PQ_SNAPPY_SEG bytes of a page's output

@@ -213,12 +213,15 @@ struct NativeScanSource : ExecNode {
         }
         Selection sel = select_row_groups(open_files, file_start, file_length, fields.size(), terms);
         all_units = std::move(sel.units);
+        const PageSelection ps = select_pages(all_units, open_files, fields.size(), terms);
         strings.resize(fields.size());
         plan = plan_batches(all_units, open_files, fields, ctx->chunk_rows);
-        if (trace_on()) fprintf(stderr, "[cb200 trace]   parquet scan: %zu row groups in %zu batches (%lld pruned by statistics), chunk block %.1f MB, work block %.1f MB per slot\n",
-                                all_units.size(), plan.batches.size(), (long long)sel.pruned_row_groups, plan.chunk_need / 1e6, plan.work_estimate / 1e6);
+        if (trace_on()) fprintf(stderr, "[cb200 trace]   parquet scan: %zu row groups in %zu batches (%lld pruned by statistics, %lld data pages by the page index), chunk block %.1f MB, work block %.1f MB per slot\n",
+                                all_units.size(), plan.batches.size(), (long long)sel.pruned_row_groups, (long long)ps.pruned_pages, plan.chunk_need / 1e6, plan.work_estimate / 1e6);
         ctx->scan_pruned_row_groups += sel.pruned_row_groups;
         ctx->scan_pruned_rows += sel.pruned_rows;
+        ctx->scan_pruned_pages += ps.pruned_pages;
+        ctx->scan_page_pruned_rows += ps.pruned_rows;
         opened = true;
     }
 
@@ -328,18 +331,14 @@ struct NativeScanSource : ExecNode {
         }
         cuda_check(cudaEventRecord(res.uploaded[si], res.copy_stream), "event record");
         std::vector<std::vector<ChunkLoc>> loc(fields.size());
-        for (size_t c = 0; c < fields.size(); c++)
-            for (const ChunkAt& at : up.chunk_at[c]) {
-                const UploadRange& r = up.ranges[at.range];
-                loc[c].push_back({host_of(r) + at.off, sl.chunk->ptr + r.dev_off + at.off});
-            }
+        for (size_t c = 0; c < fields.size(); c++) loc[c] = locate_chunks(up, c, host_of, sl.chunk->ptr);
         return loc;
     }
 
     // one bump allocation in the work block per device buffer, sized now that every page is known; page tables into the pinned block
     void bind_buffers(std::vector<ColPlan>& plans, int64_t total, Slot& sl) {
         size_t need = 1024, meta_need = 4096;
-        for (auto& p : plans) meta_need += align_up(p.pages.size() * sizeof(PqPage), 64) + align_up(p.remap.size() * 4, 64) + align_up(p.hostdec.size(), 64) + 192;
+        for (auto& p : plans) meta_need += align_up(p.pages.size() * sizeof(PqPage), 64) + align_up(p.remap.size() * 4, 64) + align_up(p.hostdec.size(), 64) + align_up(p.segs.size() * sizeof(PqSeg), 64) + 256;
         std::vector<std::pair<uint8_t**, size_t>> reqs;
         uint8_t* derr = nullptr;
         reqs.push_back({&derr, 64});
@@ -379,6 +378,7 @@ struct NativeScanSource : ExecNode {
         resolve_bodies(cp, hostdec_dev);
         cp.dpd = stage(sl, cp.pages.data(), cp.pages.size() * sizeof(PqPage));
         if (!cp.remap.empty()) cp.ddict = stage(sl, cp.remap.data(), cp.remap.size() * 4);
+        if (!cp.segs.empty()) cp.dsegs = stage(sl, cp.segs.data(), cp.segs.size() * sizeof(PqSeg));
     }
 
     void launch(std::vector<ColPlan>& plans, int64_t total, Batch& out, int si) {
@@ -458,7 +458,7 @@ struct NativeScanSource : ExecNode {
         const int n_all = (int)cp.pages.size(), n_data = (int)cp.n_data;
         PqPage* data_pages = (PqPage*)cp.dpd;
         const PqPage* dict_pages = data_pages + n_data;
-        uint8_t* dense = cp.null_aware ? cp.dense : cp.out;
+        uint8_t* dense = cp.null_aware ? cp.dense : !cp.segs.empty() ? cp.dcov : cp.out; // page-pruned: decoded into covered rows first
         launch_pq_resolve(data_pages, n_all, ds);
         ctx->kernel_launches++;
         if (cp.n_dict_pages) { launch_pq_plain(dict_pages, (int)cp.n_dict_pages, cp.conv, cp.type_length, cp.ddict, derr, ds); ctx->kernel_launches++; }
@@ -479,7 +479,11 @@ struct NativeScanSource : ExecNode {
             launch_pq_dbp(data_pages, n_data, (PqMiniblock*)cp.dmb, cp.conv, dense, derr, ds);
             ctx->kernel_launches += 4;
         }
-        if (cp.null_aware) {
+        if (!cp.segs.empty()) {
+            launch_pq_select((const PqSeg*)cp.dsegs, (int)cp.segs.size(), total, cp.null_aware ? cp.dvalid : nullptr, (const unsigned*)cp.didx, dense, cp.out,
+                             (unsigned*)cp.validity, cp.out_w, ds);
+            ctx->kernel_launches++;
+        } else if (cp.null_aware) {
             launch_pq_scatter(cp.dvalid, (const unsigned*)cp.didx, dense, cp.out, (unsigned*)cp.validity, total, cp.out_w, ds);
             ctx->kernel_launches++;
         }

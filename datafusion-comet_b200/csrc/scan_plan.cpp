@@ -33,14 +33,18 @@ static pq::FileMeta open_parquet(const std::string& path, const uint8_t** mem, s
     const std::string pre = "memory://";
     if (path.compare(0, pre.size(), pre) != 0) {
         int64_t sz = 0;
-        return pq::read_footer(strip_file_scheme(path), &sz);
+        pq::FileMeta m = pq::read_footer(strip_file_scheme(path), &sz);
+        pq::read_page_indexes(m, strip_file_scheme(path), sz);
+        return m;
     }
     std::lock_guard<std::mutex> lk(g_memfile_mu);
     auto it = g_memfiles.find(path.substr(pre.size()));
     if (it == g_memfiles.end()) throw ExecError(3, "", "parquet: memory file '" + path + "' is not registered");
     *mem = it->second.first;
     *mem_len = it->second.second;
-    return pq::parse_footer(*mem, *mem_len);
+    pq::FileMeta m = pq::parse_footer(*mem, *mem_len);
+    pq::read_page_indexes(m, *mem, *mem_len);
+    return m;
 }
 
 std::string describe_parquet(const std::string& path) {
@@ -112,12 +116,20 @@ static bool stat_value(const pq::SchemaElement& se, const std::string& raw, bool
 }
 
 bool term_excludes(const PruneTerm& t, const pq::SchemaElement& se, const pq::ColumnChunkMeta& cc) {
-    if (t.op == ExprKind::IsNotNull) return cc.null_count >= 0 && cc.null_count == cc.num_values && cc.num_values > 0;
-    if (!cc.has_min_max) return false;
+    StatVals s;
+    if (cc.has_min_max) { s.min = &cc.min_value; s.max = &cc.max_value; }
+    // a chunk's null_count rules out IsNotNull only: comparison terms on a chunk are decided by its min / max alone
+    s.all_null = t.op == ExprKind::IsNotNull && cc.null_count >= 0 && cc.null_count == cc.num_values && cc.num_values > 0;
+    return stats_exclude(t, se, s);
+}
+
+bool stats_exclude(const PruneTerm& t, const pq::SchemaElement& se, const StatVals& s) {
+    if (s.all_null) return true; // a comparison with NULL is never true
+    if (t.op == ExprKind::IsNotNull || !s.min || !s.max) return false;
     bool fmin, fmax;
     __int128 imin = 0, imax = 0;
     double dmin = 0, dmax = 0;
-    if (!stat_value(se, cc.min_value, &fmin, &imin, &dmin) || !stat_value(se, cc.max_value, &fmax, &imax, &dmax)) return false;
+    if (!stat_value(se, *s.min, &fmin, &imin, &dmin) || !stat_value(se, *s.max, &fmax, &imax, &dmax)) return false;
     if (fmin != t.is_float) return false;
     if (t.is_float) {
         // float statistics may be written with -0.0 / +0.0 either way; comparisons below treat them as equal, which is safe
@@ -165,7 +177,90 @@ Selection select_row_groups(const std::vector<ScanFile>& files, const std::vecto
     return s;
 }
 
+// ---- pages ----------------------------------------------------------------------------------------------------------
+// [first row, end row) of page i of a chunk's offset index
+static std::pair<int64_t, int64_t> page_rows(const std::vector<pq::PageLocation>& loc, size_t i, int64_t rg_rows) {
+    return {loc[i].first_row_index, i + 1 < loc.size() ? loc[i + 1].first_row_index : rg_rows};
+}
+
+// the pages of one column that overlap `ranges`, their covered rows and the segments that map selected rows onto them
+static ColumnWindow column_window(const std::vector<pq::PageLocation>& loc, int64_t rg_rows, const std::vector<std::pair<int64_t, int64_t>>& ranges) {
+    ColumnWindow w;
+    std::vector<int64_t> cov_at(loc.size(), -1); // covered row of a selected page's first row
+    size_t r = 0;
+    for (size_t i = 0; i < loc.size(); i++) {
+        const auto [p0, p1] = page_rows(loc, i, rg_rows);
+        while (r < ranges.size() && ranges[r].second <= p0) r++;
+        if (r < ranges.size() && ranges[r].first < p1) {
+            cov_at[i] = w.covered;
+            w.pages.push_back((int)i);
+            w.covered += p1 - p0;
+        }
+    }
+    int64_t out = 0;
+    size_t i = 0;
+    for (const auto& [a, b] : ranges) { // every page a range touches is selected, and they are consecutive: one segment per range
+        while (page_rows(loc, i, rg_rows).second <= a) i++;
+        w.segs.push_back({out, cov_at[i] + (a - loc[i].first_row_index), b - a});
+        out += b - a;
+    }
+    return w;
+}
+
+PageSelection select_pages(std::vector<Unit>& units, const std::vector<ScanFile>& files, size_t n_cols, const std::vector<PruneTerm>& terms) {
+    PageSelection ps;
+    if (terms.empty()) return ps;
+    std::vector<Unit> kept;
+    for (Unit& u : units) {
+        const ScanFile& f = files[u.file];
+        const int64_t n = f.meta.row_groups[u.rg].num_rows;
+        bool usable = !u.sel;
+        for (size_t c = 0; c < n_cols && usable; c++) usable = !f.chunk(u.rg, c).offset_index.empty();
+        for (auto& t : terms)
+            if (usable && t.col >= 0 && t.col < (int)n_cols) usable = !f.chunk(u.rg, (size_t)t.col).column_index.null_pages.empty();
+        if (!usable) { kept.push_back(u); continue; }
+        // the rows some term's page statistics rule out, merged; the selection is what is left
+        std::vector<std::pair<int64_t, int64_t>> out;
+        for (auto& t : terms) {
+            if (t.col < 0 || t.col >= (int)n_cols) continue;
+            const pq::ColumnChunkMeta& cc = f.chunk(u.rg, (size_t)t.col);
+            const pq::ColumnIndex& ci = cc.column_index;
+            for (size_t i = 0; i < cc.offset_index.size(); i++) {
+                StatVals s;
+                if (ci.null_pages[i]) s.all_null = true;
+                else { s.min = &ci.min_values[i]; s.max = &ci.max_values[i]; }
+                if (stats_exclude(t, f.leaf((size_t)t.col), s)) out.push_back(page_rows(cc.offset_index, i, n));
+            }
+        }
+        std::sort(out.begin(), out.end());
+        auto sel = std::make_shared<RowSelection>();
+        int64_t at = 0, rows = 0;
+        for (const auto& [a, b] : out) {
+            if (a > at) { sel->ranges.push_back({at, a}); rows += a - at; }
+            at = std::max(at, b);
+        }
+        if (at < n) { sel->ranges.push_back({at, n}); rows += n - at; }
+        if (rows == n) { kept.push_back(u); continue; }
+        int64_t pages = 0;
+        for (size_t c = 0; c < n_cols; c++) pages += (int64_t)f.chunk(u.rg, c).offset_index.size();
+        ps.pruned_rows += n - rows;
+        if (rows == 0) { ps.pruned_pages += pages; ps.dropped_row_groups++; continue; }
+        for (size_t c = 0; c < n_cols; c++) {
+            sel->cols.push_back(column_window(f.chunk(u.rg, c).offset_index, n, sel->ranges));
+            pages -= (int64_t)sel->cols.back().pages.size();
+        }
+        ps.pruned_pages += pages;
+        u.rows = rows;
+        u.sel = std::move(sel);
+        kept.push_back(u);
+    }
+    units = std::move(kept);
+    return ps;
+}
+
 // ---- batches --------------------------------------------------------------------------------------------------------
+static void unit_ranges(const ScanFile& f, const Unit& unit, size_t u, size_t n_cols, UploadPlan& up);
+
 BatchPlan plan_batches(const std::vector<Unit>& units, const std::vector<ScanFile>& files, const std::vector<StructField>& fields, int64_t chunk_rows) {
     BatchPlan bp;
     // greedy fill up to chunk_rows; the FIRST batch is a sixteenth of that: nothing overlaps its upload, so it should be short
@@ -188,9 +283,15 @@ BatchPlan plan_batches(const std::vector<Unit>& units, const std::vector<ScanFil
         int64_t rows = 0;
         for (size_t i = b.first; i < b.second; i++) {
             rows += units[i].rows;
+            if (units[i].sel) { // page-pruned: its upload ranges exactly, and the uncompressed bytes of its share of the chunks
+                UploadPlan one;
+                one.chunk_at.assign(fields.size(), std::vector<ChunkAt>(1));
+                unit_ranges(files[units[i].file], units[i], 0, fields.size(), one);
+                for (auto& r : one.ranges) enc += align_up((size_t)(r.end - r.start), 256) + 256;
+            }
             for (size_t c = 0; c < fields.size(); c++) {
                 const pq::ColumnChunkMeta& cc = files[units[i].file].chunk(units[i].rg, c);
-                enc += align_up((size_t)std::max<int64_t>(cc.total_compressed, 0), 256) + 256;
+                if (!units[i].sel) enc += align_up((size_t)std::max<int64_t>(cc.total_compressed, 0), 256) + 256;
                 if (cc.codec != pq::UNCOMPRESSED) work += (size_t)std::max<int64_t>(cc.total_uncompressed, 0) + 64 * 1024;
             }
         }
@@ -198,9 +299,11 @@ BatchPlan plan_batches(const std::vector<Unit>& units, const std::vector<ScanFil
             const DType& t = fields[c].type;
             const size_t w = t.is_decimal() ? (t.precision <= 18 ? 8 : 16) : t.is_string() ? 4 : (size_t)std::max(t.arrow_width(), 1);
             bool nulls = false, dict_encoded = false, delta = false;
+            int64_t cov = 0; // rows the column's pages decode into
             for (size_t i = b.first; i < b.second; i++) {
                 const ScanFile& f = files[units[i].file];
                 const pq::ColumnChunkMeta& cc = f.chunk(units[i].rg, c);
+                cov += units[i].sel ? units[i].sel->cols[c].covered : units[i].rows;
                 if (f.leaf(c).repetition == 1 && cc.null_count != 0) nulls = true;
                 for (int enc : cc.encodings) {
                     if (enc == pq::RLE_DICTIONARY || enc == pq::PLAIN_DICTIONARY) dict_encoded = true;
@@ -208,10 +311,11 @@ BatchPlan plan_batches(const std::vector<Unit>& units, const std::vector<ScanFil
                 }
             }
             work += (size_t)rows * w + 4096;                                  // decoded column
+            if (cov != rows) work += (size_t)cov * w + 4096;                  // page-pruned: the covered rows it is selected from
             work += (b.second - b.first) * 96 * 1024;                         // page tables / dictionaries
-            if (dict_encoded) work += (size_t)rows * 4 + (b.second - b.first) * 16 * 2048; // run table: (values / 8 + 64) runs of 32 bytes per page
-            if (nulls) work += (size_t)rows * (w + 5 + 4) + 65536;            // dense values + validity bytes + indices + level runs
-            if (delta) work += ((size_t)rows / 16 + (b.second - b.first) * 256) * sizeof(PqMiniblock); // miniblock table: values / 32 + 2 entries per page
+            if (dict_encoded) work += (size_t)cov * 4 + (b.second - b.first) * 16 * 2048; // run table: (values / 8 + 64) runs of 32 bytes per page
+            if (nulls) work += (size_t)cov * (w + 5 + 4) + 65536;             // dense values + validity bytes + indices + level runs
+            if (delta) work += ((size_t)cov / 16 + (b.second - b.first) * 256) * sizeof(PqMiniblock); // miniblock table: values / 32 + 2 entries per page
         }
         bp.chunk_need = std::max(bp.chunk_need, enc + 65536);
         bp.work_estimate = std::max(bp.work_estimate, work + work / 16);
@@ -230,28 +334,52 @@ std::vector<Unit> batch_units(const std::vector<Unit>& units, std::pair<size_t, 
 // Per row group, the selected column chunks sorted by file offset and merged into byte ranges (gaps of unselected columns up to
 // 64 KB ride along) -- PCIe moves few large copies faster than many chunk-sized ones (measured: 49 GB/s at 1.8 MB per copy,
 // 54 GB/s at 12 MB).
+// The file bytes a page-pruned unit reads of column c: what precedes the first data page (the dictionary page), then every run of
+// selected data pages.
+static std::vector<std::pair<int64_t, int64_t>> chunk_pieces(const pq::ColumnChunkMeta& cc, const ColumnWindow& w) {
+    std::vector<std::pair<int64_t, int64_t>> out;
+    const auto& loc = cc.offset_index;
+    if (loc[0].offset > cc.start()) out.push_back({cc.start(), loc[0].offset});
+    for (size_t k = 0; k < w.pages.size(); k++) {
+        const pq::PageLocation& p = loc[(size_t)w.pages[k]];
+        const bool next_to_last = k > 0 && w.pages[k] == w.pages[k - 1] + 1 && out.back().second == p.offset;
+        if (next_to_last) out.back().second = p.offset + p.compressed_page_size;
+        else out.push_back({p.offset, p.offset + p.compressed_page_size});
+    }
+    return out;
+}
+
+// the upload ranges of unit u, appended to `up`
+static void unit_ranges(const ScanFile& f, const Unit& unit, size_t u, size_t n_cols, UploadPlan& up) {
+    struct Item { int64_t start, end; size_t col; long piece; }; // piece -1: the whole chunk
+    std::vector<Item> items;
+    for (size_t c = 0; c < n_cols; c++) {
+        const pq::ColumnChunkMeta& cc = f.chunk(unit.rg, c);
+        if (cc.total_compressed < 0 || cc.start() < 0) throw PlanError("parquet: negative column chunk offset / size");
+        if (f.mem && (size_t)cc.start() + (size_t)cc.total_compressed > f.mem_len) throw PlanError("parquet: column chunk beyond the end of the file image");
+        if (!unit.sel) { items.push_back({cc.start(), cc.start() + cc.total_compressed, c, -1}); continue; }
+        const auto pieces = chunk_pieces(cc, unit.sel->cols[c]);
+        for (size_t k = 0; k < pieces.size(); k++) items.push_back({pieces[k].first, pieces[k].second, c, (long)k});
+    }
+    std::sort(items.begin(), items.end(), [](const Item& a, const Item& b) { return a.start != b.start ? a.start < b.start : a.col != b.col ? a.col < b.col : a.piece < b.piece; });
+    bool open_range = false;
+    for (auto& it : items) {
+        // a gap of up to 64 KB rides along; chunks may also overlap (the same column projected twice)
+        if (open_range && it.start - up.ranges.back().end <= 65536) up.ranges.back().end = std::max(up.ranges.back().end, it.end);
+        else { up.ranges.push_back({unit.file, it.start, it.end, 0}); open_range = true; }
+        const size_t r = up.ranges.size() - 1;
+        const int64_t off = it.start - up.ranges.back().start;
+        ChunkAt& at = up.chunk_at[it.col][u];
+        if (it.piece < 0) { at.range = r; at.off = off; continue; }
+        if (it.piece == 0) { at.range = r; at.off = off; }
+        at.pieces.push_back({it.start, it.end, r, off});
+    }
+}
+
 UploadPlan plan_uploads(const std::vector<Unit>& units, const std::vector<ScanFile>& files, size_t n_cols) {
     UploadPlan up;
     up.chunk_at.assign(n_cols, std::vector<ChunkAt>(units.size()));
-    for (size_t u = 0; u < units.size(); u++) {
-        const ScanFile& f = files[units[u].file];
-        std::vector<std::pair<int64_t, size_t>> items; // (file offset, column)
-        for (size_t c = 0; c < n_cols; c++) {
-            const pq::ColumnChunkMeta& cc = f.chunk(units[u].rg, c);
-            if (cc.total_compressed < 0 || cc.start() < 0) throw PlanError("parquet: negative column chunk offset / size");
-            if (f.mem && (size_t)cc.start() + (size_t)cc.total_compressed > f.mem_len) throw PlanError("parquet: column chunk beyond the end of the file image");
-            items.push_back({cc.start(), c});
-        }
-        std::sort(items.begin(), items.end());
-        bool open_range = false;
-        for (auto& it : items) {
-            const int64_t st0 = it.first, en0 = st0 + f.chunk(units[u].rg, it.second).total_compressed;
-            // a gap of up to 64 KB rides along; chunks may also overlap (the same column projected twice)
-            if (open_range && st0 - up.ranges.back().end <= 65536) up.ranges.back().end = std::max(up.ranges.back().end, en0);
-            else { up.ranges.push_back({units[u].file, st0, en0, 0}); open_range = true; }
-            up.chunk_at[it.second][u] = {up.ranges.size() - 1, st0 - up.ranges.back().start};
-        }
-    }
+    for (size_t u = 0; u < units.size(); u++) unit_ranges(files[units[u].file], units[u], u, n_cols, up);
     for (auto& r : up.ranges) { r.dev_off = up.dev_total; up.dev_total += align_up((size_t)(r.end - r.start), 256); }
     return up;
 }
@@ -412,16 +540,45 @@ class ColumnPlanner {
         if (optional && cc.null_count != 0) nulls_possible = true; // unknown (-1) counts as possible
         if (cc.codec != pq::UNCOMPRESSED && cc.codec != pq::SNAPPY && !host_codec_supported(cc.codec))
             throw Unsupported("parquet codec " + std::to_string(cc.codec) + " (UNCOMPRESSED and SNAPPY are decompressed on the device, ZSTD / LZ4 / LZ4_RAW / GZIP on the host; BROTLI / LZO are not read)");
-        if (cc.num_values != unit.rows) throw Unsupported("parquet: repeated column (num_values != num_rows)");
-        row = unit.row0;
+        const int64_t rg_rows = f.meta.row_groups[unit.rg].num_rows;
+        if (cc.num_values != rg_rows) throw Unsupported("parquet: repeated column (num_values != num_rows)");
+        const int64_t cov0 = row; // pages decode into covered rows: the batch's rows unless a unit before this one is page-pruned
         dict_off = -1;
         dict_size = 0;
-        for (auto& pg : pq::walk_pages(at.host, (size_t)cc.total_compressed, cc.num_values)) {
-            const Section s{at.host + pg.data_offset, at.dev + pg.data_offset, pg.compressed_size, pg.uncompressed_size, cc.codec};
-            if (pg.type == pq::DICTIONARY_PAGE) dictionary_page(pg, s);
-            else if (pg.type == pq::DATA_PAGE || pg.type == pq::DATA_PAGE_V2) data_page(pg, s, optional);
+        if (!unit.sel) {
+            for (auto& pg : pq::walk_pages(at.host, (size_t)cc.total_compressed, cc.num_values)) {
+                const Section s{at.host + pg.data_offset, at.dev + pg.data_offset, pg.compressed_size, pg.uncompressed_size, cc.codec};
+                if (pg.type == pq::DICTIONARY_PAGE) dictionary_page(pg, s);
+                else if (pg.type == pq::DATA_PAGE || pg.type == pq::DATA_PAGE_V2) data_page(pg, s, optional);
+            }
+            if (row != cov0 + rg_rows) throw PlanError("parquet: data pages of column '" + field.name + "' do not add up to the row group's row count");
+            add_seg({unit.row0, cov0, unit.rows});
+            return;
         }
-        if (row != unit.row0 + unit.rows) throw PlanError("parquet: data pages of column '" + field.name + "' do not add up to the row group's row count");
+        // page-pruned: the dictionary page in front of the first data page, then the selected data pages where the offset index puts them
+        const ColumnWindow& w = unit.sel->cols[c];
+        const auto& loc = cc.offset_index;
+        if (loc[0].offset > cc.start()) {
+            const auto [h, d] = piece(at, cc.start(), loc[0].offset - cc.start());
+            for (auto& pg : pq::walk_pages(h, (size_t)(loc[0].offset - cc.start()), 1)) {
+                const Section s{h + pg.data_offset, d + pg.data_offset, pg.compressed_size, pg.uncompressed_size, cc.codec};
+                if (pg.type == pq::DICTIONARY_PAGE) dictionary_page(pg, s);
+                else if (pg.type == pq::DATA_PAGE || pg.type == pq::DATA_PAGE_V2) throw PlanError("parquet: column '" + field.name + "' has a data page in front of the first page its offset index lists");
+            }
+        }
+        for (int i : w.pages) {
+            const pq::PageLocation& pl = loc[(size_t)i];
+            const int64_t span = ((size_t)i + 1 < loc.size() ? loc[(size_t)i + 1].first_row_index : rg_rows) - pl.first_row_index;
+            const auto [h, d] = piece(at, pl.offset, pl.compressed_page_size);
+            const std::vector<pq::PageInfo> one = pq::walk_pages(h, (size_t)pl.compressed_page_size, 1);
+            if (one.size() != 1 || (one[0].type != pq::DATA_PAGE && one[0].type != pq::DATA_PAGE_V2) || one[0].num_values != span ||
+                one[0].data_offset + one[0].compressed_size != pl.compressed_page_size)
+                throw PlanError("parquet: a page header of column '" + field.name + "' contradicts its offset index");
+            const pq::PageInfo& pg = one[0];
+            data_page(pg, Section{h + pg.data_offset, d + pg.data_offset, pg.compressed_size, pg.uncompressed_size, cc.codec}, optional);
+        }
+        if (row != cov0 + w.covered) throw PlanError("parquet: selected data pages of column '" + field.name + "' do not add up to their rows");
+        for (const PqSeg& s : w.segs) add_seg({unit.row0 + s.out_row, cov0 + s.cov_row, s.count});
     }
 
     void finish(int64_t total) {
@@ -429,10 +586,13 @@ class ColumnPlanner {
         cp.n_dict_pages = dict_pages.size();
         cp.pages.insert(cp.pages.end(), dict_pages.begin(), dict_pages.end()); // one upload for every descriptor of this column
         for (auto& d : cp.pages) { d.seg_base = (int)cp.n_segs_total; cp.n_segs_total += d.n_segs; } // n_segs = 0 unless Snappy
+        // the covered rows are the batch's rows exactly when no unit is page-pruned in this column: no selection step then
+        cp.covered = row;
+        if (row == total) cp.segs.clear();
         // definition levels: the statistics' null_count == 0 selects the verify-only fast path; otherwise values are decoded
         // densely and scattered to their rows
         cp.null_aware = cp.optional && nulls_possible;
-        if (cp.null_aware && total >= (int64_t)1 << 32) throw Unsupported("parquet: NULL-aware decode of more than 2^32 rows per batch (lower spark.comet.b200.chunkRows)");
+        if (cp.null_aware && row >= (int64_t)1 << 32) throw Unsupported("parquet: NULL-aware decode of more than 2^32 rows per batch (lower spark.comet.b200.chunkRows)");
     }
 
   private:
@@ -446,6 +606,23 @@ class ColumnPlanner {
     bool nulls_possible = false;
     int64_t row = 0, dict_off = -1; // next output row / the current chunk's dictionary in the combined one
     int dict_size = 0;
+
+    // host / device address of the file bytes [off, off + len) of a page-pruned chunk
+    std::pair<const uint8_t*, unsigned char*> piece(const ChunkLoc& at, int64_t off, int64_t len) const {
+        for (const PieceLoc& p : at.pieces)
+            if (p.start <= off && off + len <= p.end) return {p.host + (off - p.start), p.dev + (off - p.start)};
+        throw PlanError("parquet: a selected page of column '" + field.name + "' was not uploaded");
+    }
+
+    // appends a segment, extending the last one when they are contiguous in both row spaces
+    void add_seg(const PqSeg& s) {
+        if (s.count <= 0) return;
+        if (!cp.segs.empty()) {
+            PqSeg& b = cp.segs.back();
+            if (b.out_row + b.count == s.out_row && b.cov_row + b.count == s.cov_row) { b.count += s.count; return; }
+        }
+        cp.segs.push_back(s);
+    }
 
     // uncompressed bytes of a section on the host, valid until the next call
     std::pair<const uint8_t*, size_t> host_section(const Section& s, const char* what) {
@@ -604,6 +781,7 @@ ColPlan plan_column(const std::vector<ScanFile>& files, const StructField& field
 
 void buffer_requests(ColPlan& cp, int64_t total, std::vector<std::pair<uint8_t**, size_t>>& reqs) {
     const size_t n = (size_t)std::max<int64_t>(total, 1);
+    const size_t nc = cp.segs.empty() ? n : (size_t)std::max<int64_t>(cp.covered, 1); // rows the pages decode into
     cp.out_bytes = n * (size_t)cp.out_w;
     reqs.push_back({&cp.out, cp.out_bytes});
     if (cp.pages.empty()) return;
@@ -612,10 +790,11 @@ void buffer_requests(ColPlan& cp, int64_t total, std::vector<std::pair<uint8_t**
         reqs.push_back({&cp.dckpt, (size_t)(cp.n_segs_total + 1) * 4});
     }
     if (cp.dict_elems > 0 && cp.remap.empty()) reqs.push_back({&cp.ddict, (size_t)cp.dict_elems * (size_t)cp.out_w + 16}); // string dictionaries: the remap table in the mirror IS the dictionary
+    if (!cp.segs.empty() && !cp.null_aware) reqs.push_back({&cp.dcov, nc * (size_t)cp.out_w});
     if (cp.null_aware) {
-        reqs.push_back({&cp.dense, n * (size_t)cp.out_w});
-        reqs.push_back({&cp.dvalid, n + 64});
-        reqs.push_back({&cp.didx, n * 4 + 64});
+        reqs.push_back({&cp.dense, nc * (size_t)cp.out_w});
+        reqs.push_back({&cp.dvalid, nc + 64});
+        reqs.push_back({&cp.didx, nc * 4 + 64});
         reqs.push_back({&cp.druns, (size_t)std::max<int64_t>(cp.def_run_base, 1) * sizeof(PqRun)});
         reqs.push_back({&cp.dcounts, cp.n_data * 4 + 16});
         cp.validity_bytes = (n + 31) / 32 * 4 + 16;

@@ -6,6 +6,7 @@
 #include "parquet.h"
 #include "parquet_pages.h"
 
+#include <memory>
 #include <unordered_map>
 #include <utility>
 
@@ -36,10 +37,34 @@ struct PruneTerm {
     double fval = 0;
 };
 void collect_prune_terms(const ExprP& e, std::vector<PruneTerm>& out);
-// true = the statistics prove that no row of the chunk satisfies the term
+// the statistics of a column chunk or of one page: min / max (PLAIN-encoded values; nullptr = not known) and whether every value is NULL
+struct StatVals {
+    const std::string* min = nullptr;
+    const std::string* max = nullptr;
+    bool all_null = false;
+};
+// true = the statistics prove that no row they describe satisfies the term (all NULL: no term holds; else min / max decide)
+bool stats_exclude(const PruneTerm& t, const pq::SchemaElement& se, const StatVals& s);
+// the same for a whole column chunk
 bool term_excludes(const PruneTerm& t, const pq::SchemaElement& se, const pq::ColumnChunkMeta& cc);
 
-struct Unit { size_t file, rg; int64_t rows, row0; }; // one row group; row0: its first row within its batch
+// The rows of one row group that the page index cannot rule out, and per read column the data pages that hold them.  A column decodes
+// those pages into "covered" rows (the rows of its selected pages back to back); `segs` maps selected rows to covered rows.
+struct ColumnWindow {
+    std::vector<int> pages;    // into the chunk's offset_index, ascending
+    int64_t covered = 0;       // rows of those pages
+    std::vector<PqSeg> segs;   // out_row: among the unit's selected rows; cov_row: among its covered rows
+};
+struct RowSelection {
+    std::vector<std::pair<int64_t, int64_t>> ranges; // [begin, end) rows of the row group, sorted and disjoint
+    std::vector<ColumnWindow> cols;                  // per read column
+};
+// one row group; rows: the rows it emits (all of them, or the selected ones); row0: its first row within its batch
+struct Unit {
+    size_t file, rg;
+    int64_t rows, row0;
+    std::shared_ptr<const RowSelection> sel = nullptr; // nullptr: the whole row group
+};
 struct Selection {
     std::vector<Unit> units;
     int64_t pruned_row_groups = 0, pruned_rows = 0;
@@ -47,6 +72,17 @@ struct Selection {
 // the row groups a scan reads: those a file split owns, minus those the statistics rule out
 Selection select_row_groups(const std::vector<ScanFile>& files, const std::vector<int64_t>& file_start, const std::vector<int64_t>& file_length,
                             size_t n_cols, const std::vector<PruneTerm>& terms);
+
+// ---- pages ---------------------------------------------------------------------------------------------------------------------
+struct PageSelection {
+    int64_t pruned_pages = 0;       // data pages of read columns that are not uploaded
+    int64_t pruned_rows = 0;        // rows of the given units that are not emitted
+    int64_t dropped_row_groups = 0; // units none of whose pages survive
+};
+// Attaches a row selection to every unit whose page index rules rows out, and drops the units it rules out entirely.  A row leaves
+// only when the ColumnIndex of its page, in some term's column, proves that term false.  Applies to a unit whose term columns all have
+// a ColumnIndex and whose read columns all have an OffsetIndex; every other unit stays whole.
+PageSelection select_pages(std::vector<Unit>& units, const std::vector<ScanFile>& files, size_t n_cols, const std::vector<PruneTerm>& terms);
 
 // ---- batches -------------------------------------------------------------------------------------------------------------------
 struct BatchPlan {
@@ -60,12 +96,18 @@ std::vector<Unit> batch_units(const std::vector<Unit>& units, std::pair<size_t, 
 
 // ---- upload ranges -------------------------------------------------------------------------------------------------------------
 struct UploadRange { size_t file; int64_t start, end; size_t dev_off; };
-struct ChunkAt { size_t range; int64_t off; }; // a column chunk inside an upload range
+struct PieceAt { int64_t start, end; size_t range; int64_t off; }; // file bytes [start, end) of a page-pruned chunk inside an upload range
+struct ChunkAt {   // a column chunk inside an upload range
+    size_t range;
+    int64_t off;
+    std::vector<PieceAt> pieces = {}; // page-pruned unit: its dictionary page, then its runs of selected data pages (range / off unused)
+};
 struct UploadPlan {
     std::vector<UploadRange> ranges;
     std::vector<std::vector<ChunkAt>> chunk_at; // [column][unit]
     size_t dev_total = 0;                       // device bytes of all ranges, each 256-byte aligned
 };
+// Whole row groups upload whole column chunks; a page-pruned one uploads its dictionary pages and its runs of selected data pages.
 UploadPlan plan_uploads(const std::vector<Unit>& units, const std::vector<ScanFile>& files, size_t n_cols);
 
 // ---- columns -------------------------------------------------------------------------------------------------------------------
@@ -77,7 +119,27 @@ struct StringInterner {
     int32_t code(std::string v);
 };
 
-struct ChunkLoc { const uint8_t* host; unsigned char* dev; }; // one column chunk of a batch: its bytes on the host and where they land on the device
+// one column chunk of a batch: its bytes on the host and where they land on the device; for a page-pruned unit, those of each piece
+struct PieceLoc { int64_t start, end; const uint8_t* host; unsigned char* dev; };
+struct ChunkLoc {
+    const uint8_t* host;
+    unsigned char* dev;
+    std::vector<PieceLoc> pieces = {};
+};
+// the ChunkLocs of column c: `host_of(range)` is the host address of an upload range's first byte, `dev_base` the device block
+template <typename HostOf> std::vector<ChunkLoc> locate_chunks(const UploadPlan& up, size_t c, HostOf host_of, unsigned char* dev_base) {
+    std::vector<ChunkLoc> loc;
+    for (const ChunkAt& at : up.chunk_at[c]) {
+        const UploadRange& r = up.ranges[at.range];
+        ChunkLoc l{host_of(r) + at.off, dev_base + r.dev_off + at.off};
+        for (const PieceAt& p : at.pieces) {
+            const UploadRange& pr = up.ranges[p.range];
+            l.pieces.push_back({p.start, p.end, host_of(pr) + p.off, dev_base + pr.dev_off + p.off});
+        }
+        loc.push_back(std::move(l));
+    }
+    return loc;
+}
 
 // one column of one batch: page tables on the host, then the device buffers they refer to
 struct ColPlan {
@@ -93,9 +155,13 @@ struct ColPlan {
     int64_t n_segs_total = 0;     // Snappy: 64 KB output segments over all compressed pages (checkpoint table entries)
     std::vector<uint8_t> hostdec; // page bodies produced on the host, 16-byte aligned each; shipped with the page tables
     bool optional = false, null_aware = false, any_compressed = false;
+    // page-pruned units: the pages decode into `covered` rows (PqPage::dst_row counts them), `segs` picks the batch's rows out of them.
+    // Empty when the covered rows are the batch's rows: the pages decode straight into `out`.
+    int64_t covered = 0;
+    std::vector<PqSeg> segs;
     // device buffers, bound by the scan (buffer_requests)
     uint8_t *out = nullptr, *dunc = nullptr, *dpd = nullptr, *ddict = nullptr, *dense = nullptr, *dvalid = nullptr, *didx = nullptr, *druns = nullptr,
-            *dcounts = nullptr, *validity = nullptr, *runs = nullptr, *counts = nullptr, *dckpt = nullptr, *dmb = nullptr;
+            *dcounts = nullptr, *validity = nullptr, *runs = nullptr, *counts = nullptr, *dckpt = nullptr, *dmb = nullptr, *dcov = nullptr, *dsegs = nullptr;
     size_t out_bytes = 0, validity_bytes = 0;
 };
 

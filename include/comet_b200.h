@@ -184,6 +184,8 @@ typedef struct cb200_stats {
     int64_t scan_pruned_row_groups; /* Parquet row groups skipped because their statistics rule the pushed filters out */
     int64_t scan_pruned_rows;
     int64_t agg_strategies;    /* OR of CB200_AGG_* over the plan's aggregates: which accumulation strategies ran */
+    int64_t scan_pruned_pages; /* Parquet data pages of read columns not uploaded because the page index rules the pushed filters out */
+    int64_t scan_page_pruned_rows; /* rows of row groups the statistics kept that the page index ruled out */
 } cb200_stats;
 #define CB200_AGG_DENSE 1      /* thread-private accumulators over dictionary / bool key codes (and ungrouped aggregates) */
 #define CB200_AGG_TABLE 2      /* global key table */
