@@ -63,8 +63,8 @@ def f_float(field, v):
 DATA_TYPE_ID = dict(BOOL=0, INT8=1, INT16=2, INT32=3, INT64=4, FLOAT=5, DOUBLE=6, STRING=7, BYTES=8, TIMESTAMP=9,
                     DECIMAL=10, TIMESTAMP_NTZ=11, DATE=12, NULL=13)  # types.proto:43-66
 EXPR_FIELD = dict(literal=2, bound=3, add=4, subtract=5, multiply=6, divide=7, cast=8, eq=9, neq=10, gt=11, gt_eq=12,
-                  lt=13, lt_eq=14, is_null=15, is_not_null=16, **{"and": 17, "or": 18}, check_overflow=25,
-                  caseWhen=38, **{"in": 39, "not": 40}, unary_minus=41, **{"if": 44}, unbound=51)  # expr.proto:30-109
+                  lt=13, lt_eq=14, is_null=15, is_not_null=16, **{"and": 17, "or": 18}, check_overflow=25, like=26,
+                  scalarFunc=31, caseWhen=38, **{"in": 39, "not": 40}, unary_minus=41, **{"if": 44}, unbound=51)  # expr.proto:30-109
 AGG_FIELD = dict(count=2, sum=3, min=4, max=5, avg=6)  # expr.proto:143-176
 OP_FIELD = dict(scan=100, projection=101, filter=102, sort=103, hash_agg=104, limit=105, shuffle_writer=106,
                 native_scan=111, shuffle_scan=116)  # operator.proto:32-86
@@ -235,6 +235,14 @@ def case_when(whens, thens, else_expr=None):  # CaseWhen expr.proto:473
 
 def in_(value, lst, negated=False):
     return _expr("in", f_len(1, value) + b"".join(f_len(2, x) for x in lst) + f_bool(3, negated))
+
+
+def like(value, pattern):  # BinaryExpr (left, right): `value LIKE pattern`, escape character `\`
+    return _binary("like", value, pattern)
+
+
+def scalar_func(name, args, return_type=BOOL):  # ScalarFunc expr.proto:466 (Comet's starts_with / ends_with / contains bridge)
+    return _expr("scalarFunc", f_str(1, name) + b"".join(f_len(2, a) for a in args) + f_len(3, return_type.encode()))
 
 
 # ---- AggExpr (expr.proto:143-215) ----------------------------------------------------------------

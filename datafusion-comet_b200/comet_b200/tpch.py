@@ -22,6 +22,8 @@ DATE_1995_01_01 = 9131
 DATE_1995_06_17 = 9298
 RETURNFLAGS = ["A", "N", "R"]
 LINESTATUS = ["F", "O"]
+SHIPMODES = ["REG AIR", "AIR", "RAIL", "SHIP", "TRUCK", "MAIL", "FOB"]                  # TPC-H 4.2.2.13 Modes
+SHIPINSTRUCTS = ["DELIVER IN PERSON", "COLLECT COD", "NONE", "TAKE BACK RETURN"]       # TPC-H 4.2.2.13 Instructions
 
 
 # ---- data -----------------------------------------------------------------------------------------
@@ -42,8 +44,12 @@ def gen_lineitem(n, seed=42):
     ar = rng.integers(0, 2, size=n).astype(np.uint8) * 2  # A (0) or R (2)
     rf = np.where(receipt <= DATE_1995_06_17, ar, np.uint8(1)).astype(np.uint8)  # else N (1)
     ls = (ship > DATE_1995_06_17).astype(np.uint8)  # F (0) / O (1)
+    # ship mode / instruction codes (into SHIPMODES / SHIPINSTRUCTS) from a stream of their own: the columns above do not change
+    rng2 = np.random.Generator(np.random.PCG64([seed, 1]))
+    mode = rng2.integers(0, len(SHIPMODES), size=n).astype(np.uint8)
+    instruct = rng2.integers(0, len(SHIPINSTRUCTS), size=n).astype(np.uint8)
     return dict(l_orderkey=orderkey, l_quantity=qty_units * 100, l_extendedprice=price, l_discount=disc, l_tax=tax,
-                l_shipdate=ship, l_returnflag=rf, l_linestatus=ls)
+                l_shipdate=ship, l_returnflag=rf, l_linestatus=ls, l_shipmode=mode, l_shipinstruct=instruct)
 
 
 def _dec_array(cents, precision=12, scale=2, valid=None):
@@ -74,6 +80,8 @@ def lineitem_table(cols, variant="dec", dictionary=True, columns=None):
         "l_tax": lambda: money(cols["l_tax"]),
         "l_returnflag": lambda: flags(cols["l_returnflag"], RETURNFLAGS),
         "l_linestatus": lambda: flags(cols["l_linestatus"], LINESTATUS),
+        "l_shipmode": lambda: flags(cols["l_shipmode"], SHIPMODES),
+        "l_shipinstruct": lambda: flags(cols["l_shipinstruct"], SHIPINSTRUCTS),
         "l_shipdate": lambda: pa.array(cols["l_shipdate"], type=pa.date32()),
     }
     names = columns or ["l_quantity", "l_extendedprice", "l_discount", "l_tax", "l_returnflag", "l_linestatus", "l_shipdate"]

@@ -682,6 +682,7 @@ struct AggNode : FusedBase {
         clear_vmask();
         cb::PipeParams p;
         fill_inputs(p, b, k.g.tile, r0, r1);
+        bind_str_masks(p, k.spec, b);
         int grid = grid_for(ctx, p.n_tiles);
         size_t part_bytes = (size_t)grid * tot_bytes;
         if (!dense.partials || dense.partials->bytes < part_bytes) dense.partials = std::make_shared<DeviceBuf>(part_bytes);
@@ -730,6 +731,7 @@ struct AggNode : FusedBase {
         clear_vmask();
         cb::PipeParams p;
         fill_inputs(p, b, k.g.tile, r0, r1);
+        bind_str_masks(p, k.spec, b);
         p.hkeys = with_table ? (cb::u64*)table.hkeys->ptr : nullptr;
         p.hkey_of_gid = (cb::u64*)rows.hkey_of_gid->ptr;
         p.htotals = (cb::u64*)rows.htotals->ptr;

@@ -4,6 +4,7 @@
 // codes.  (Plan-dependent kernels are JIT-specialised: device/cb_kernels.cuh.)
 #include "aot_kernels.h"
 #include "device/cb_math.h"
+#include "device/cb_strpred.h"
 
 namespace cb200 {
 using namespace cb;
@@ -63,6 +64,26 @@ void launch_remap_codes(const void* in, int in_width, i64 n, const i32* table, i
     if (in_width == 1) k_remap_codes<signed char><<<blocks, 256, 0, st>>>((const signed char*)in, n, table, table_len, out);
     else if (in_width == 2) k_remap_codes<short><<<blocks, 256, 0, st>>>((const short*)in, n, table, table_len, out);
     else k_remap_codes<i32><<<blocks, 256, 0, st>>>((const i32*)in, n, table, table_len, out);
+}
+
+// ---- string predicate over dictionary entries -> one bit per code ---------------------------------------------------------------------
+// One thread per entry; a warp's 32 entries are one mask word (first is a multiple of 32), written whole by the ballot: no atomics and no
+// read-modify-write of a word another launch owns.  Bits past n are 0 in the last word; the next launch over a grown dictionary starts
+// at that word again.
+__global__ void k_str_pred(StrPredDev d, const i32* off, const u8* chars, i64 first, i64 n, u32* mask) {
+    const i64 i = first + (i64)blockIdx.x * blockDim.x + threadIdx.x;
+    bool bit = false;
+    if (i < n) {
+        const i64 k = i - first;
+        bit = sp_eval(d, chars + off[k], off[k + 1] - off[k]);
+    }
+    const u32 w = __ballot_sync(0xffffffffu, bit);
+    if ((threadIdx.x & 31) == 0 && i < n) mask[i >> 5] = w;
+}
+void launch_str_pred(const StrPredDev& d, const int* offsets, const unsigned char* chars, i64 first, i64 n, unsigned* mask, cudaStream_t st) {
+    if (n <= first) return;
+    const int threads = 256;
+    k_str_pred<<<(unsigned)((n - first + threads - 1) / threads), threads, 0, st>>>(d, offsets, chars, first, n, mask);
 }
 
 // ---- device string dictionary -----------------------------------------------------------------------

@@ -3,10 +3,15 @@
 #include <cuda_runtime.h>
 #include <cstdint>
 
+#include "device/cb_strpred.h"
+
 namespace cb200 {
 
 void launch_bitmap_append(uint32_t* dst, long long dst_off, const uint8_t* src, long long src_off, long long n, cudaStream_t st);
 void launch_bytes_to_bitmap(const uint8_t* bytes, long long n, uint32_t* out, cudaStream_t st);
+// string predicate d over dictionary entries [first, n) -> mask bits [first, n) (bit i & 31 of word i >> 5).  Entry i is
+// chars[offsets[i - first], offsets[i - first + 1]).  first must be a multiple of 32: each warp writes whole words of its own.
+void launch_str_pred(const cb::StrPredDev& d, const int* offsets, const unsigned char* chars, long long first, long long n, unsigned* mask, cudaStream_t st);
 void launch_remap_codes(const void* in, int in_width, long long n, const int* table, int table_len, int* out, cudaStream_t st);
 
 enum { CB_DICT_FULL = 1, CB_DICT_COLLISION = 2 };

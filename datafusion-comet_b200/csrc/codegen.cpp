@@ -4,11 +4,13 @@
 // hand-written device library device/cb_math.h (host-tested against the oracle).
 #include "codegen.h"
 #include <mutex>
+#include "device/cb_params.h"
 #include "ranges.h"
 
 #include <climits>
 #include <cstring>
 #include <functional>
+#include <set>
 #include <sstream>
 
 namespace cb200 {
@@ -98,7 +100,11 @@ struct Emitter {
     std::vector<u128r> col_bounds; // assumed (kernel-validated) magnitude bound per staged column
     std::vector<bool> col_masked;  // columns whose value mask is accumulated (decimal inputs of aggregate pipelines)
 
+    std::map<std::string, int> str_slot; // StrPred key -> PipeParams::smask index
+
     explicit Emitter(const PipelineSpec& s) : spec(s) {
+        const std::vector<ExprP> sp = str_preds_of(s);
+        for (size_t i = 0; i < sp.size(); i++) str_slot[std::to_string(sp[i]->children[0]->index) + "@" + str_pred_key(*sp[i])] = (int)i;
         for (auto& c : s.cols) {
             u128r b = RSAT;
             if (c.type.is_decimal()) {
@@ -128,6 +134,7 @@ struct Emitter {
         memcpy(&fb, &e.lit_f64, 8);
         o << fb << "|" << (uint64_t)e.lit_dec << "," << (uint64_t)(e.lit_dec >> 64) << "|" << (int)e.eval_mode << "|"
           << e.fail_on_error << "|" << e.negated << "|" << e.wide_decimal << "|" << e.integral_div << e.check_divide_overflow << "|" << e.return_type.str() << "(";
+        if (e.kind == ExprKind::StrPred) o << str_pred_key(e) << "|" << e.in_has_null << "|";
         for (auto& c : e.children) o << key_of(*c) << ",";
         o << ")";
         return o.str();
@@ -251,6 +258,7 @@ struct Emitter {
             return r;
         }
         case ExprKind::In: return emit_in(e);
+        case ExprKind::StrPred: return emit_str_pred(e);
         }
         throw PlanError("unhandled expression kind");
     }
@@ -592,6 +600,31 @@ struct Emitter {
         return r;
     }
 
+    // String predicate: one bit per dictionary code, computed on the host side of the launch (k_str_pred); here only the lookup by the
+    // code the kernel already staged.  The literal never enters the source, so plans that differ only in literals share one kernel.
+    // A NULL row is NULL and its code (which Arrow leaves unspecified) is never used; a valid code outside the mask raises error bit 5.
+    Val emit_str_pred(const Expr& e) {
+        Val c = emit(*e.children[0]);
+        auto it = str_slot.find(std::to_string(e.children[0]->index) + "@" + str_pred_key(e));
+        if (it == str_slot.end()) throw PlanError("internal: string predicate without a mask slot");
+        const std::string m = "p.smask[" + std::to_string(it->second) + "]";
+        const std::string valid = c.n.empty() ? "true" : "!" + c.n;
+        std::string ok = declb(valid + " && (cb::u32)" + c.v + " < (cb::u32)" + m + ".n_entries");
+        uses_err = true;
+        body << "    if (" << (base_guard.empty() ? "" : base_guard + " && ") << valid << " && !" << ok << ") cb::set_err(p, 5);\n";
+        std::string hit = declb(ok + " && ((" + m + ".bits[(cb::u32)" + c.v + " >> 5] >> ((cb::u32)" + c.v + " & 31u)) & 1u) != 0u");
+        Val r;
+        r.type = e.type;
+        if (e.str_op == StrOp::In) { // Spark In: NULL value -> NULL; match -> TRUE; else NULL if the list has a NULL, else FALSE
+            r.v = e.negated ? declb("!" + hit) : hit;
+            r.n = e.in_has_null ? or_null(c.n, "!" + hit) : c.n;
+        } else {
+            r.v = hit;
+            r.n = c.n;
+        }
+        return r;
+    }
+
     Val emit_in(const Expr& e) { // Spark In: NULL value -> NULL; match -> TRUE; else NULL if list has NULL, else FALSE
         Val v = emit(*e.children[0]);
         bool list_has_null = false;
@@ -722,6 +755,7 @@ void sig_expr(std::ostringstream& o, const Expr& e) {
     o << (int)e.kind << '|' << e.type.str() << '|' << e.index << '|' << e.lit_null << '|' << e.lit_i64 << '|' << fb << '|' << (uint64_t)e.lit_dec << ','
       << (uint64_t)(e.lit_dec >> 64) << '|' << e.lit_str << '|' << (int)e.eval_mode << '|' << e.fail_on_error << '|' << e.negated << '|' << e.wide_decimal << '|' << e.integral_div << e.check_divide_overflow << '|'
       << e.return_type.str() << '(';
+    if (e.kind == ExprKind::StrPred) o << str_pred_key(e) << '|' << e.in_has_null << '|';
     for (auto& c : e.children) { sig_expr(o, *c); o << ','; }
     o << ')';
 }
@@ -753,6 +787,37 @@ GeneratedKernel generate_pipeline_uncached(const PipelineSpec& spec);
 } // namespace
 
 std::string pipeline_signature(const PipelineSpec& spec) { return spec_signature(spec); }
+
+std::string str_pred_key(const Expr& e) {
+    std::ostringstream o;
+    o << (int)e.str_op << ':' << e.str_lits.size();
+    for (auto& l : e.str_lits) o << ':' << l.size() << '=' << l; // length-prefixed: any bytes
+    return o.str();
+}
+
+std::vector<ExprP> str_preds_of(const PipelineSpec& spec) {
+    std::vector<ExprP> out;
+    std::set<std::string> seen;
+    std::function<void(const ExprP&)> walk = [&](const ExprP& e) {
+        if (!e) return;
+        if (e->kind == ExprKind::StrPred) {
+            if (seen.insert(std::to_string(e->children[0]->index) + "@" + str_pred_key(*e)).second) out.push_back(e);
+            return;
+        }
+        for (auto& c : e->children) walk(c);
+    };
+    for (auto& e : spec.predicates) walk(e);
+    for (auto& e : spec.outputs) walk(e);
+    for (auto& e : spec.keys) walk(e);
+    if (spec.mode == AggMode::Partial)
+        for (auto& a : spec.aggs) {
+            for (auto& c : a.children) walk(c);
+            walk(a.filter);
+        }
+    if (out.size() > CB_MAX_STR_PREDS)
+        throw Unsupported("more than " + std::to_string(CB_MAX_STR_PREDS) + " distinct string predicates in one fused pipeline");
+    return out;
+}
 
 GeneratedKernel generate_pipeline(const PipelineSpec& spec) {
     const std::string sig = spec_signature(spec);

@@ -75,6 +75,13 @@ struct GeneratedKernel {
 };
 
 GeneratedKernel generate_pipeline(const PipelineSpec& spec);
+
+// The distinct string predicates (ExprKind::StrPred) of a pipeline in mask-slot order: PipeParams::smask[i] holds the mask of entry i.
+// Order: predicates, outputs, group keys, then the arguments and FILTER clauses of Partial aggregates, each depth first.  Throws
+// Unsupported above CB_MAX_STR_PREDS.
+std::vector<ExprP> str_preds_of(const PipelineSpec& spec);
+// what one StrPred computes per dictionary entry: operation and literals.  Two nodes with equal keys over the same column share a mask.
+std::string str_pred_key(const Expr& e);
 // canonical text of a pipeline (expressions, column encodings, sink): equal specs give equal strings
 std::string pipeline_signature(const PipelineSpec& spec);
 

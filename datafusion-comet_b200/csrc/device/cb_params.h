@@ -11,6 +11,13 @@ namespace cb {
 #define CB_MAX_KEYS 4
 
 #define CB_SCAN_CHUNK 4096
+#define CB_MAX_STR_PREDS 8  // distinct string predicates one pipeline evaluates
+
+// a string predicate's value per dictionary code: bit c & 31 of word c >> 5, for codes [0, n_entries) (see exec_internal.h StrMasks)
+struct StrMask {
+    const u32* bits;
+    i32 n_entries;
+};
 
 struct PipeParams {
     const u8* col[CB_MAX_COLS];      // input column value buffers (16-byte aligned, padded)
@@ -45,6 +52,7 @@ struct PipeParams {
     i32* hflags;                     // [0] bit 0: sentinel key seen, bit 1: out of group ids / table full, bit 2: key does not fit
                                      //     the 64-bit packing, bit 3: NULL-key group used;
                                      // [CB_HFLAG_CTR + r], r < CB_GID_RANGES: group ids handed out in id range r (see below)
+    StrMask smask[CB_MAX_STR_PREDS]; // string predicates, in the order codegen.h str_preds_of lists them
 };
 // Group ids come from CB_GID_RANGES independent counters, not one: range r owns the ids [r * R, (r + 1) * R), R = max_groups /
 // CB_GID_RANGES, and every warp draws from its home range (spilling to the next one when it is full).  One counter for the whole

@@ -12,7 +12,7 @@
 namespace cb200 {
 
 // error bits raised by kernels (device/cb_kernels.cuh set_err)
-enum { ERR_I128_OVERFLOW = 0, ERR_ANSI_OVERFLOW = 1, ERR_ORDER_DEPENDENT = 2, ERR_DIVIDE_BY_ZERO = 3, ERR_ARROW_DIVIDE_BY_ZERO = 4 };
+enum { ERR_I128_OVERFLOW = 0, ERR_ANSI_OVERFLOW = 1, ERR_ORDER_DEPENDENT = 2, ERR_DIVIDE_BY_ZERO = 3, ERR_ARROW_DIVIDE_BY_ZERO = 4, ERR_DICT_CODE = 5 };
 
 bool trace_on() {
     static int on = -1;
@@ -149,10 +149,80 @@ void ExecContext::check_device_errors() {
     if (e & (1 << ERR_ARROW_DIVIDE_BY_ZERO)) throw ExecError(11, "", "Arrow error: Divide by zero error"); // arrow-arith checked division in Legacy mode
     if (e & (1 << ERR_I128_OVERFLOW))
         throw ExecError(11, "", "Arrow error: Arithmetic overflow: Overflow happened on decimal arithmetic"); // arrow-arith checked ops
+    if (e & (1 << ERR_DICT_CODE)) // a valid row's dictionary code outside its dictionary: the input batch is malformed
+        throw ExecError(3, "", "dictionary code out of range: a non-NULL row of a dictionary-encoded string column has a code outside its dictionary");
     if (e & (1 << ERR_ORDER_DEPENDENT))
         throw ExecError(12, "", "SUM/AVG overflow here depends on the row order (some orderings of these rows overflow, others do not); "
                                 "the reference adds in row order -- the row-ordered fallback is not built yet, so the plan is refused rather than guessed");
     throw ExecError(13, "", "device error flags " + std::to_string(e));
+}
+
+// =================================================================================================
+// string predicate masks (exec_internal.h)
+// =================================================================================================
+void StrMasks::bind(cb::PipeParams& p, const PipelineSpec& spec, const Batch& b, ExecContext* ctx) {
+    const std::vector<ExprP> preds = str_preds_of(spec);
+    cudaStream_t st = ctx->stream;
+    for (size_t j = 0; j < preds.size(); j++) {
+        const Expr& e = *preds[j];
+        const int src = spec.cols.at((size_t)e.children[0]->index).src_index;
+        const Column& c = b.cols.at((size_t)src);
+        if (!c.is_dict || !c.dict) throw Unsupported("string predicate over a plain (non-dictionary) Utf8 column");
+        StrMask& m = by_key[std::to_string(src) + "@" + str_pred_key(e)];
+        if (!m.payload) { // [lit_off: n_lits + 1 x i32][LIKE items: u16][literal bytes]
+            std::vector<uint8_t> blob;
+            std::vector<int32_t> off{0};
+            std::string bytes;
+            for (auto& l : e.str_lits) { bytes += l; off.push_back((int32_t)bytes.size()); }
+            auto put = [&](const void* q, size_t n) { size_t at = (blob.size() + 15) / 16 * 16; blob.resize(at + n); if (n) memcpy(blob.data() + at, q, n); return at; };
+            const size_t o_off = put(off.data(), off.size() * 4), o_pat = put(e.like_items.data(), e.like_items.size() * 2), o_lit = put(bytes.data(), bytes.size());
+            m.payload = std::make_shared<DeviceBuf>(blob.size() + 16);
+            cuda_check(cudaMemcpyAsync(m.payload->ptr, blob.data(), blob.size(), cudaMemcpyHostToDevice, st), "H2D string predicate");
+            ctx->h2d_bytes += (int64_t)blob.size();
+            const uint8_t* base = (const uint8_t*)m.payload->ptr;
+            m.dev.op = (int)e.str_op;
+            m.dev.n_lits = (int)e.str_lits.size();
+            m.dev.lit_off = (const int*)(base + o_off);
+            m.dev.pat = (const uint16_t*)(base + o_pat);
+            m.dev.pat_len = (int)e.like_items.size();
+            m.dev.lit = base + o_lit;
+        }
+        if (m.dict != c.dict) { m.dict = c.dict; m.done = 0; }
+        const std::vector<std::string>& vals = c.dict->values;
+        const int64_t n = (int64_t)vals.size();
+        if (n > INT32_MAX) throw Unsupported("string predicate over a dictionary of more than 2^31 entries");
+        const size_t words = (size_t)(n + 31) / 32;
+        if (!m.bits || m.bits->bytes < words * 4) {
+            const size_t cap = std::max<size_t>({words, m.bits ? m.bits->bytes / 2 : 0, 64}); // bytes / 2 = twice the words
+            auto nb = std::make_shared<DeviceBuf>(cap * 4);
+            if (m.bits && m.done > 0) cuda_check(cudaMemcpyAsync(nb->ptr, m.bits->ptr, (size_t)(m.done + 31) / 32 * 4, cudaMemcpyDeviceToDevice, st), "grow mask");
+            m.bits = nb;
+        }
+        if (m.done < n) {
+            // the tail [first, n), first on a word boundary: the partial last word of the previous update is evaluated again
+            const int64_t first = m.done & ~(int64_t)31;
+            std::vector<int32_t>& off = m.h_off;
+            std::string& chars = m.h_chars;
+            off.assign((size_t)(n - first) + 1, 0);
+            size_t total = 0;
+            for (int64_t i = first; i < n; i++) total += vals[(size_t)i].size();
+            if (total > INT32_MAX) throw Unsupported("string predicate over more than 2 GiB of new dictionary bytes");
+            chars.clear();
+            chars.reserve(total);
+            for (int64_t i = first; i < n; i++) { chars += vals[(size_t)i]; off[(size_t)(i - first + 1)] = (int32_t)chars.size(); }
+            if (!m.off || m.off->bytes < off.size() * 4) m.off = std::make_shared<DeviceBuf>(off.size() * 4 * 2);
+            if (!m.chars || m.chars->bytes < chars.size() + 16) m.chars = std::make_shared<DeviceBuf>(chars.size() * 2 + 16);
+            cuda_check(cudaMemcpyAsync(m.off->ptr, off.data(), off.size() * 4, cudaMemcpyHostToDevice, st), "H2D dictionary offsets");
+            if (!chars.empty()) cuda_check(cudaMemcpyAsync(m.chars->ptr, chars.data(), chars.size(), cudaMemcpyHostToDevice, st), "H2D dictionary chars");
+            ctx->h2d_bytes += (int64_t)(off.size() * 4 + chars.size());
+            launch_str_pred(m.dev, (const int*)m.off->ptr, (const unsigned char*)m.chars->ptr, first, n, (unsigned*)m.bits->ptr, st);
+            cuda_check(cudaGetLastError(), "k_str_pred launch");
+            ctx->kernel_launches++;
+            m.done = n;
+        }
+        p.smask[j].bits = (const cb::u32*)m.bits->ptr;
+        p.smask[j].n_entries = (cb::i32)n;
+    }
 }
 
 // =================================================================================================
@@ -584,6 +654,7 @@ struct SelectNode : FusedBase {
         cb::PipeParams p;
         if (masked()) fill_inputs_of(p, in, out_cols_used, g.tile);
         else fill_inputs(p, in, g.tile);
+        bind_str_masks(p, spec, in);
         out.cols.clear();
         out.cols.resize(g.out_cols.size());
         cudaStream_t st = ctx->stream;
@@ -612,10 +683,12 @@ struct SelectNode : FusedBase {
         int64_t* h_kept = nullptr;
         if (!predicates.empty()) {
             // pass 1: kept rows per (tile, warp), then their exclusive prefix sum = where pass 2 writes
-            GeneratedKernel cg = generate_pipeline(make_count_spec(&in));
+            const PipelineSpec cspec = make_count_spec(&in);
+            GeneratedKernel cg = generate_pipeline(cspec);
             auto cmod = jit_get(cg, true);
             cb::PipeParams cp;
             fill_inputs_of(cp, in, pred_cols, cg.tile);
+            bind_str_masks(cp, cspec, in);
             const size_t m = (size_t)p.n_tiles * (size_t)(g.threads / 32);
             const size_t n_chunks = (m + CB_SCAN_CHUNK - 1) / CB_SCAN_CHUNK;
             if (!sel_off || sel_off->bytes < m * 4) sel_off = std::make_shared<DeviceBuf>(m * 4 + m / 2);

@@ -3,6 +3,7 @@
 #pragma once
 #include "exec.h"
 
+#include "aot_kernels.h"
 #include "device/cb_params.h"
 
 #include <cstring>
@@ -54,6 +55,28 @@ inline void rewrite_bound(const ExprP& e, const std::map<int, int>& slot_of) {
     if (e->kind == ExprKind::Bound) { e->index = slot_of.at(e->index); return; }
     for (auto& c : e->children) rewrite_bound(c, slot_of);
 }
+
+// ---- string predicate masks ----------------------------------------------------------------------------------------
+// A string predicate is decided once per dictionary entry: a device bitmask over the codes of its column, read by the pipeline kernel
+// (codegen.cpp emit_str_pred).  Dictionaries only grow and codes never change (Dictionary::values: a batch's dictionary is unified into
+// the plan-wide one, the Parquet scan interns into one dictionary per column), so a mask is brought up to date before every launch
+// that reads it by evaluating only the entries added since the previous one.  A column that carries another Dictionary object starts
+// again from entry 0.
+struct StrMask {
+    DictionaryP dict;                // the dictionary `done` refers to
+    int64_t done = 0;                // entries evaluated
+    DeviceBufP bits;                 // mask words (capacity grows geometrically)
+    DeviceBufP payload;              // the predicate's literals / LIKE items on the device
+    cb::StrPredDev dev{};
+    DeviceBufP off, chars;           // the tail of the dictionary being evaluated ...
+    std::vector<int32_t> h_off;      // ... and its host staging (kept: the copies are asynchronous)
+    std::string h_chars;
+};
+struct StrMasks {
+    std::map<std::string, StrMask> by_key; // "<source column>@<str_pred_key>"
+    // update the masks of every string predicate of `spec` for batch b and bind them to p.smask
+    void bind(cb::PipeParams& p, const PipelineSpec& spec, const Batch& b, ExecContext* ctx);
+};
 
 // ---- fused pipeline nodes ------------------------------------------------------------------------------------------
 struct FusedBase : ExecNode {
@@ -117,6 +140,9 @@ struct FusedBase : ExecNode {
         p.n_tiles = (int)((p.n_rows + tile - 1) / tile);
         p.err = ctx->d_err;
     }
+    // the string predicate masks a launch of `spec` over b reads (after fill_inputs*, which clears p)
+    StrMasks str_masks;
+    void bind_str_masks(cb::PipeParams& p, const PipelineSpec& spec, const Batch& b) { str_masks.bind(p, spec, b, ctx); }
     void launch(cudaKernel_t k, dim3 grid, dim3 block, size_t smem, void* params) {
         cuda_check(cudaFuncSetAttribute((const void*)k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "cudaFuncSetAttribute(smem)");
         void* args[] = {params};

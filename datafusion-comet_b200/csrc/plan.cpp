@@ -3,6 +3,7 @@
 // partitioning}.proto (cited inline).  Type rules: native/core/src/execution/planner.rs.
 #include "plan.h"
 #include "proto_wire.h"
+#include "device/cb_strpred.h"
 
 #include <algorithm>
 #include <sstream>
@@ -253,6 +254,29 @@ static ExprP decode_expr(PbReader r) {
             out = tail;
             break;
         }
+        case 26: { // Like: BinaryExpr (left, pattern); lowered in resolve
+            out = decode_binary(ExprKind::StrPred, r.sub(), false);
+            out->str_op = StrOp::Like;
+            break;
+        }
+        case 31: { // ScalarFunc expr.proto:466 {func = 1, args = 2, return_type = 3, fail_on_error = 4}
+            PbReader c = r.sub();
+            std::string func;
+            std::vector<ExprP> args;
+            while (c.next()) {
+                if (c.field == 1) func = c.bytes();
+                else if (c.field == 2) args.push_back(decode_expr(c.sub()));
+                else c.skip();
+            }
+            // Comet sends Spark's StartsWith / EndsWith / Contains under these names (serde/strings.scala CometScalarFunction)
+            if (func != "starts_with" && func != "ends_with" && func != "contains")
+                throw Unsupported("scalar function '" + func + "' is outside the GPU hot path");
+            if (args.size() != 2) throw PlanError("scalar function " + func + " expects two arguments");
+            out = mk(ExprKind::StrPred);
+            out->str_op = func == "starts_with" ? StrOp::StartsWith : func == "ends_with" ? StrOp::EndsWith : StrOp::Contains;
+            out->children = args;
+            break;
+        }
         case 90: r.skip(); break; // query_context
         default:
             throw Unsupported("expression field " + std::to_string(r.field) + " is outside the GPU hot path");
@@ -283,10 +307,68 @@ static bool cast_supported(const DType& from, const DType& to) {
     return false;
 }
 
+// ---- string predicates ----------------------------------------------------------------------------------------------------
+static bool is_str_col(const Expr& e) { return e.kind == ExprKind::Bound && e.type.id == TypeId::String; }
+static bool is_str_lit(const Expr& e) { return e.kind == ExprKind::Literal && e.type.id == TypeId::String; }
+static void to_null_bool(Expr& e) { // a NULL literal operand: the predicate is NULL on every row
+    e.kind = ExprKind::Literal;
+    e.children.clear();
+    e.lit_null = true;
+    e.type = mk_type(TypeId::Bool);
+}
+
+// Lowers a comparison, IN, LIKE or starts_with / ends_with / contains whose operand is a string to StrPred over the Bound column,
+// or throws Unsupported.  Only column-vs-literal shapes are evaluated: the predicate is decided once per dictionary entry.
+static void lower_string_predicate(Expr& e) {
+    const char* what = e.kind == ExprKind::In ? "IN" : e.kind == ExprKind::StrPred ? "string function" : "comparison";
+    if (e.kind == ExprKind::In) {
+        if (!is_str_col(*e.children[0])) throw Unsupported(std::string("IN over a string that is not a column reference (") + e.children[0]->type.str() + ")");
+        std::vector<std::string> lits;
+        bool has_null = false;
+        for (size_t i = 1; i < e.children.size(); i++) {
+            const Expr& m = *e.children[i];
+            if (!is_str_lit(m)) throw Unsupported("IN over utf8 with a member that is not a utf8 literal");
+            if (m.lit_null) has_null = true;
+            else lits.push_back(m.lit_str);
+        }
+        if (lits.empty() && has_null) { to_null_bool(e); return; } // NULL value -> NULL, anything else -> no match, list has NULL -> NULL
+        e.str_op = StrOp::In;
+        e.str_lits = lits;
+        e.in_has_null = has_null;
+    } else {
+        ExprP col = e.children[0], lit = e.children[1];
+        StrOp op = e.str_op;
+        if (e.kind != ExprKind::StrPred) {
+            static const StrOp ops[] = {StrOp::Eq, StrOp::Neq, StrOp::Gt, StrOp::GtEq, StrOp::Lt, StrOp::LtEq};
+            op = ops[(int)e.kind - (int)ExprKind::Eq];
+            if (is_str_lit(*col) && is_str_col(*lit)) { // literal <op> column: mirror
+                std::swap(col, lit);
+                op = op == StrOp::Lt ? StrOp::Gt : op == StrOp::LtEq ? StrOp::GtEq : op == StrOp::Gt ? StrOp::Lt : op == StrOp::GtEq ? StrOp::LtEq : op;
+            }
+        }
+        if (!is_str_col(*col)) throw Unsupported(std::string(what) + " over " + col->type.str() + " that is not a string column reference");
+        if (!is_str_lit(*lit)) throw Unsupported(std::string(what) + " between " + col->type.str() + " and " + lit->type.str() + " (only a string column against a string literal)");
+        if (lit->lit_null) { to_null_bool(e); return; }
+        e.str_op = op;
+        e.str_lits = {lit->lit_str};
+        if (op == StrOp::Like) {
+            std::vector<uint16_t> items(lit->lit_str.size());
+            const int k = cb::sp_like_compile((const uint8_t*)lit->lit_str.data(), (int)lit->lit_str.size(), items.data());
+            if (k < 0) throw Unsupported("LIKE pattern with a '\\' that escapes something other than '%', '_' or '\\', or ends the pattern");
+            items.resize((size_t)k);
+            e.like_items = items;
+        }
+        e.children = {col};
+    }
+    e.kind = ExprKind::StrPred;
+    e.type = mk_type(TypeId::Bool);
+}
+
 static void resolve(Expr& e, const std::vector<DType>& in) {
     for (auto& c : e.children) resolve(*c, in);
     auto ct = [&](int i) -> const DType& { return e.children[i]->type; };
     switch (e.kind) {
+    case ExprKind::StrPred: lower_string_predicate(e); break;
     case ExprKind::Literal: case ExprKind::Unbound: break;
     case ExprKind::Bound:
         if (e.index >= (int)in.size()) throw PlanError("bound reference index " + std::to_string(e.index) + " out of range");
@@ -331,6 +413,7 @@ static void resolve(Expr& e, const std::vector<DType>& in) {
     }
     case ExprKind::Eq: case ExprKind::Neq: case ExprKind::Gt: case ExprKind::GtEq: case ExprKind::Lt: case ExprKind::LtEq: {
         const DType &l = ct(0), &r = ct(1);
+        if (l.id == TypeId::String && r.id == TypeId::String) { lower_string_predicate(e); break; }
         bool ok = l == r || (l.is_decimal() && r.is_decimal() && l.scale == r.scale);
         if (!ok || l.is_string() || l.id == TypeId::Null)
             throw Unsupported("comparison between " + l.str() + " and " + r.str());
@@ -371,6 +454,7 @@ static void resolve(Expr& e, const std::vector<DType>& in) {
         e.type = ct(1);
         break;
     case ExprKind::In:
+        if (ct(0).id == TypeId::String) { lower_string_predicate(e); break; }
         for (size_t i = 1; i < e.children.size(); i++) {
             if (e.children[i]->kind != ExprKind::Literal) throw Unsupported("IN list with non-literal members");
             const DType &l = ct(0), &r = ct((int)i);
@@ -667,7 +751,7 @@ OperatorP decode_plan(const uint8_t* data, size_t len) {
 std::string expr_str(const Expr& e) {
     std::ostringstream o;
     static const char* names[] = {"lit", "col", "unbound", "+", "-", "*", "/", "=", "!=", ">", ">=", "<", "<=", "isnull",
-                                  "isnotnull", "and", "or", "not", "cast", "checkoverflow", "neg", "if", "in"};
+                                  "isnotnull", "and", "or", "not", "cast", "checkoverflow", "neg", "if", "in", "strpred"};
     o << names[(int)e.kind];
     if (e.kind == ExprKind::Bound) o << e.index;
     o << ":" << e.type.str();

@@ -49,8 +49,12 @@ enum class ExprKind {
     Add, Sub, Mul, Div,
     Eq, Neq, Gt, GtEq, Lt, LtEq,
     IsNull, IsNotNull, And, Or, Not,
-    Cast, CheckOverflow, UnaryMinus, If, In
+    Cast, CheckOverflow, UnaryMinus, If, In,
+    StrPred // a predicate on a dictionary-coded string column against literals (children[0]: the Bound column)
 };
+
+// StrPred operations (the values of cb::StrOp, device/cb_strpred.h)
+enum class StrOp : int { Eq, Neq, Lt, LtEq, Gt, GtEq, In, Like, StartsWith, EndsWith, Contains };
 
 struct Expr;
 using ExprP = std::shared_ptr<Expr>;
@@ -77,6 +81,12 @@ struct Expr {
     bool check_divide_overflow = false; // MathExpr.check_divide_overflow (expr.proto:335-340)
     // decimal arithmetic lowering chosen by the reference's rule (planner.rs:998-1027)
     bool wide_decimal = false;
+    // StrPred: the literals (In: the non-NULL members; Like: the pattern text), whether an In list holds a NULL, and the compiled LIKE
+    // pattern (cb_strpred.h items).  The generated kernel sees none of these: they only decide the per-code mask.
+    StrOp str_op = StrOp::Eq;
+    std::vector<std::string> str_lits;
+    bool in_has_null = false;
+    std::vector<uint16_t> like_items;
 };
 
 enum class AggKind { Count, Sum, Min, Max, Avg };
