@@ -419,9 +419,11 @@ class Plan:
         return out
 
     def partition_starts(self):
-        buf = (C.c_int64 * 4096)()
-        self._lib.cb200_plan_partition_starts.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.c_int32]
-        n = self._lib.cb200_plan_partition_starts(self.handle, buf, 4096)
+        f = self._lib.cb200_plan_partition_starts
+        f.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.c_int32]
+        n = f(self.handle, None, 0)  # the count first: N + 1 entries for N partitions
+        buf = (C.c_int64 * max(n, 1))()
+        n = f(self.handle, buf, n)
         return [buf[i] for i in range(n)]
 
     def stats(self):

@@ -191,6 +191,7 @@ int64_t cb200_execute_device(cb200_plan* plan, cb200_device_column* cols, int32_
         return cb200_guarded(err, [&]() -> int64_t { throw PlanError("cb200_execute_device: the current batch is still being handed out by cb200_execute"); }, (int64_t)-2);
     return execute_common(plan, err, [&](Batch& b) {
         if ((int)b.cols.size() != n_cols) throw PlanError("execute_device: plan produces " + std::to_string(b.cols.size()) + " columns");
+        if (to_arrow_layout(b, &plan->ctx)) cuda_check(cudaStreamSynchronize(plan->ctx.stream), "to_arrow_layout"); // the caller reads the columns on its own stream
         for (int i = 0; i < n_cols; i++) {
             Column& c = b.cols[(size_t)i];
             cb200_device_column& o = cols[i];

@@ -258,6 +258,7 @@ __global__ void k_partition_ids(HashKeyCols kc, i64 n, u32 n_parts, u32* hashes,
         const u8* d = (const u8*)k.data;
         switch (k.kind) {
         case HK_BOOL: h = mm3_i32(bit_at(d, i) ? 1 : 0, h); break;
+        case HK_BOOL8: h = mm3_i32(d[i] ? 1 : 0, h); break;
         case HK_I8: h = mm3_i32((i32)((const signed char*)d)[i], h); break;
         case HK_I16: h = mm3_i32((i32)((const short*)d)[i], h); break;
         case HK_I32: h = mm3_i32(((const i32*)d)[i], h); break;
@@ -267,6 +268,7 @@ __global__ void k_partition_ids(HashKeyCols kc, i64 n, u32 n_parts, u32* hashes,
         case HK_DEC_SMALL_128: h = mm3_i64((i64)((const i128*)d)[i].lo, h); break; // d(p<=18): hashed as i64 (utils.rs:159-196)
         case HK_DEC_LARGE_128: h = mm3_i128(((const i128*)d)[i], h); break;        // d(p>18): 16 LE bytes (utils.rs:199-226)
         case HK_DEC_LARGE_64: h = mm3_i128(i128_from_i64(((const i64*)d)[i]), h); break;
+        case HK_DEC_SMALL_32: h = mm3_i64((i64)((const i32*)d)[i], h); break;
         case HK_DICT8: case HK_DICT16: case HK_DICT32: {
             i32 code = k.kind == HK_DICT8 ? (i32)((const signed char*)d)[i] : k.kind == HK_DICT16 ? (i32)((const short*)d)[i] : ((const i32*)d)[i];
             i32 o0 = k.dict_offsets[code], o1 = k.dict_offsets[code + 1];
@@ -378,17 +380,26 @@ __global__ void k_gather_bits(const u8* in_bits, const i64* row_idx, i64 n, u8* 
 }
 
 i64 partition_chunks(i64 n) { const i64 nb = (n + 1023) / 1024; return (nb + PID_CHUNK - 1) / PID_CHUNK; }
-void launch_partition(const HashKeyCols& kc, i64 n, u32 n_parts, u32* hashes, u32* pids, i32* block_hist, i64* block_base, i64* chunk_tmp, i64* starts,
-                      i64* row_idx, cudaStream_t st) {
-    if (n <= 0) return;
+cudaError_t launch_partition(const HashKeyCols& kc, i64 n, u32 n_parts, u32* hashes, u32* pids, i32* block_hist, i64* block_base, i64* chunk_tmp,
+                             i64* starts, i64* row_idx, cudaStream_t st) {
+    if (n <= 0) return cudaSuccess;
+    if (n_parts == 0 || n_parts > (u32)CB_MAX_HASH_PARTITIONS) return cudaErrorInvalidValue;
+    // one counter per partition in shared memory: above the default 48 KB a kernel has to opt in
+    const int smem32 = (int)(n_parts * sizeof(i32)), smem64 = (int)(n_parts * sizeof(i64));
+    cudaError_t e = cudaSuccess;
+    if (smem32 > 48 * 1024) e = cudaFuncSetAttribute((const void*)k_pid_block_hist, cudaFuncAttributeMaxDynamicSharedMemorySize, smem32);
+    if (smem64 > 48 * 1024 && e == cudaSuccess) e = cudaFuncSetAttribute((const void*)k_pid_chunk_scan, cudaFuncAttributeMaxDynamicSharedMemorySize, smem64);
+    if (smem64 > 48 * 1024 && e == cudaSuccess) e = cudaFuncSetAttribute((const void*)k_pid_place, cudaFuncAttributeMaxDynamicSharedMemorySize, smem64);
+    if (e != cudaSuccess) return e;
     i64 nb = (n + 1023) / 1024;
     const i64 nc = partition_chunks(n);
     k_partition_ids<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(kc, n, n_parts, hashes, pids);
-    k_pid_block_hist<<<(unsigned)nb, 256, n_parts * sizeof(i32), st>>>(pids, n, n_parts, block_hist);
+    k_pid_block_hist<<<(unsigned)nb, 256, smem32, st>>>(pids, n, n_parts, block_hist);
     k_pid_chunk_totals<<<(unsigned)nc, 256, 0, st>>>(block_hist, nb, n_parts, chunk_tmp);
-    k_pid_chunk_scan<<<1, 256, n_parts * sizeof(i64), st>>>(chunk_tmp, nc, n_parts, starts);
+    k_pid_chunk_scan<<<1, 256, smem64, st>>>(chunk_tmp, nc, n_parts, starts);
     k_pid_block_bases<<<(unsigned)nc, 256, 0, st>>>(block_hist, nb, n_parts, chunk_tmp, block_base);
-    k_pid_place<<<(unsigned)nb, 64, n_parts * sizeof(i64), st>>>(pids, n, n_parts, block_base, row_idx);
+    k_pid_place<<<(unsigned)nb, 64, smem64, st>>>(pids, n, n_parts, block_base, row_idx);
+    return cudaGetLastError();
 }
 void launch_gather(const void* in, int width, const i64* row_idx, i64 n, void* out, cudaStream_t st) {
     if (n <= 0) return;
@@ -401,6 +412,25 @@ void launch_gather(const void* in, int width, const i64* row_idx, i64 n, void* o
 }
 void launch_gather_bits(const void* in_bits, const i64* row_idx, i64 n, void* out_bytes, cudaStream_t st) {
     if (n > 0) k_gather_bits<<<(unsigned)((n + 255) / 256), 256, 0, st>>>((const u8*)in_bits, row_idx, n, (u8*)out_bytes);
+}
+
+// ---- device values -> Arrow layout (hand-off) ----------------------------------------------------------------------------------------
+// The scan and the device tables keep some columns narrower or wider than Arrow does: INT32-backed int8 / int16 / decimal(p <= 9) 4 bytes
+// per row, decimal(p <= 18) 8 bytes, booleans as bitmaps.  Decimals are sign-extended to Decimal128, ints narrowed (the scan wrote them
+// from values of the narrow type), booleans spelled out one byte per row.
+__global__ void k_to_arrow_layout(int conv, const u8* in, i64 n, u8* out) {
+    const i64 i = (i64)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    switch (conv) {
+    case CB_SEXT32_TO_128: { const i64 v = ((const i32*)in)[i]; ((i64*)out)[2 * i] = v; ((i64*)out)[2 * i + 1] = v >> 63; break; }
+    case CB_SEXT64_TO_128: { const i64 v = ((const i64*)in)[i]; ((i64*)out)[2 * i] = v; ((i64*)out)[2 * i + 1] = v >> 63; break; }
+    case CB_NARROW32_TO_8: ((signed char*)out)[i] = (signed char)((const i32*)in)[i]; break;
+    case CB_NARROW32_TO_16: ((short*)out)[i] = (short)((const i32*)in)[i]; break;
+    case CB_BITS_TO_BYTES: out[i] = bit_at(in, i) ? 1 : 0; break;
+    }
+}
+void launch_to_arrow_layout(int conv, const void* in, i64 n, void* out, cudaStream_t st) {
+    if (n > 0) k_to_arrow_layout<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(conv, (const u8*)in, n, (u8*)out);
 }
 
 // ---- chunked exclusive scan (select pipelines: per-(tile, warp) kept-row counts -> output offsets) ------------------------

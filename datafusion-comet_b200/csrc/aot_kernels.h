@@ -32,8 +32,9 @@ void launch_dict_encode(const StringDictDev& d, const int* offsets, const unsign
                         int* row_slot, int* codes, cudaStream_t st);
 
 // hash partitioning (ShuffleWriter with HashPartition): murmur3 seed 42 chained over the key columns, pmod, stable counting sort
+// HK_BOOL reads an Arrow bitmap, HK_BOOL8 one byte per row; HK_DEC_SMALL_32 is a decimal(p <= 9) stored as INT32 (hashed as its i64)
 enum { HK_BOOL, HK_I8, HK_I16, HK_I32, HK_I64, HK_F32, HK_F64, HK_DEC_SMALL_128, HK_DEC_LARGE_128, HK_DEC_SMALL_64 = HK_I64, HK_DEC_LARGE_64 = 9,
-       HK_DICT8 = 10, HK_DICT16, HK_DICT32, HK_UTF8 };
+       HK_DICT8 = 10, HK_DICT16, HK_DICT32, HK_UTF8, HK_DEC_SMALL_32, HK_BOOL8 };
 struct HashKeyCol {
     int kind;
     const void* data;
@@ -46,10 +47,17 @@ struct HashKeyCols {
     HashKeyCol col[8];
 };
 long long partition_chunks(long long n); // entries per partition of launch_partition's chunk_tmp scratch
-void launch_partition(const HashKeyCols& kc, long long n, unsigned n_parts, unsigned* hashes, unsigned* pids, int* block_hist, long long* block_base,
+// n_parts <= CB_MAX_HASH_PARTITIONS: three of the kernels keep one counter per partition in shared memory (8 bytes each at most)
+enum { CB_MAX_HASH_PARTITIONS = 16384 };
+// returns the first error of the launches (a launch the device refuses is reported here, not by a later synchronisation)
+cudaError_t launch_partition(const HashKeyCols& kc, long long n, unsigned n_parts, unsigned* hashes, unsigned* pids, int* block_hist, long long* block_base,
                       long long* chunk_tmp, long long* starts, long long* row_idx, cudaStream_t st);
 void launch_gather(const void* in, int width, const long long* row_idx, long long n, void* out, cudaStream_t st);
 void launch_gather_bits(const void* in_bits, const long long* row_idx, long long n, void* out_bytes, cudaStream_t st);
+
+// device values -> the Arrow layout of their logical type, rows [0, n): what the hand-off (Arrow export, cb200_execute_device) gives out
+enum { CB_SEXT32_TO_128, CB_SEXT64_TO_128, CB_NARROW32_TO_8, CB_NARROW32_TO_16, CB_BITS_TO_BYTES };
+void launch_to_arrow_layout(int conv, const void* in, long long n, void* out, cudaStream_t st);
 
 // stream compaction (hash-aggregate results): per-1024-row-block counts + exclusive scan, then one scatter per column
 void launch_key_presence(const unsigned long long* keys, long long n, unsigned char* present, cudaStream_t st);

@@ -722,6 +722,31 @@ struct SelectNode : FusedBase {
 // =================================================================================================
 // hash repartitioning (ShuffleWriterExec with HashPartition, native/shuffle/src/partitioners/multi_partition.rs)
 // =================================================================================================
+// The murmur3 kind of a key column.  The logical type decides how Spark hashes a value (utils.rs: i8 / i16 / i32 / date as i32,
+// decimal(p <= 18) as i64, wider decimals as 16 bytes); the physical layout decides how it is read.  The Parquet scan keeps INT32-backed
+// int8 / int16 / decimal(p <= 9) columns 4 bytes wide, decimals with p <= 18 8 bytes wide (device tables too), and aggregate outputs keep
+// booleans one byte per row.
+static int hash_key_kind(const Column& c) {
+    const Phys ph = c.phys;
+    switch (c.type.id) {
+    case TypeId::Bool: return ph == Phys::Bitmap ? HK_BOOL : HK_BOOL8;
+    case TypeId::Int8: return ph == Phys::I32 ? HK_I32 : HK_I8; // sign-extended to i32 either way
+    case TypeId::Int16: return ph == Phys::I32 ? HK_I32 : HK_I16;
+    case TypeId::Int32: case TypeId::Date: return HK_I32;
+    case TypeId::Int64: case TypeId::Timestamp: case TypeId::TimestampNtz: return HK_I64;
+    case TypeId::Float32: return HK_F32;
+    case TypeId::Float64: return HK_F64;
+    case TypeId::Decimal:
+        if (ph == Phys::I32) return HK_DEC_SMALL_32;
+        if (ph == Phys::I64) return c.type.precision <= 18 ? HK_DEC_SMALL_64 : HK_DEC_LARGE_64;
+        return c.type.precision <= 18 ? HK_DEC_SMALL_128 : HK_DEC_LARGE_128;
+    case TypeId::String: case TypeId::Binary:
+        if (!c.is_dict) return HK_UTF8;
+        return ph == Phys::I8 ? HK_DICT8 : ph == Phys::I16 ? HK_DICT16 : HK_DICT32;
+    default: throw Unsupported("hash partitioning on " + c.type.str());
+    }
+}
+
 // Output: the child's rows reordered so that partition p occupies rows [starts[p], starts[p+1]) -- what the
 // reference writes as per-partition IPC blocks, kept on the device for the NVLink exchange.
 struct PartitionNode : ExecNode {
@@ -739,46 +764,33 @@ struct PartitionNode : ExecNode {
         cudaStream_t st = ctx->stream;
         HashKeyCols kc;
         memset(&kc, 0, sizeof(kc));
-        if (key_cols.size() > 8) throw Unsupported("more than 8 hash-partition keys");
         std::vector<DeviceBufP> keep;
         for (int ci : key_cols) {
             const Column& c = in.cols[(size_t)ci];
             HashKeyCol& k = kc.col[kc.n++];
             k.data = c.data ? c.data->ptr : nullptr;
             k.validity = c.validity ? (const unsigned char*)c.validity->ptr : nullptr;
-            switch (c.type.id) {
-            case TypeId::Bool: k.kind = HK_BOOL; break;
-            case TypeId::Int8: k.kind = HK_I8; break;
-            case TypeId::Int16: k.kind = HK_I16; break;
-            case TypeId::Int32: case TypeId::Date: k.kind = HK_I32; break;
-            case TypeId::Int64: case TypeId::Timestamp: case TypeId::TimestampNtz: k.kind = HK_I64; break;
-            case TypeId::Float32: k.kind = HK_F32; break;
-            case TypeId::Float64: k.kind = HK_F64; break;
-            case TypeId::Decimal:
-                if (c.phys == Phys::I64) k.kind = c.type.precision <= 18 ? HK_DEC_SMALL_64 : HK_DEC_LARGE_64;
-                else k.kind = c.type.precision <= 18 ? HK_DEC_SMALL_128 : HK_DEC_LARGE_128;
+            k.kind = hash_key_kind(c);
+            switch (k.kind) {
+            case HK_DICT8: case HK_DICT16: case HK_DICT32: {
+                std::vector<int32_t> off{0};
+                std::string chars;
+                for (auto& v : c.dict->values) { chars += v; off.push_back((int32_t)chars.size()); }
+                auto doff = std::make_shared<DeviceBuf>(off.size() * 4), dch = std::make_shared<DeviceBuf>(chars.size() + 16);
+                cuda_check(cudaMemcpyAsync(doff->ptr, off.data(), off.size() * 4, cudaMemcpyHostToDevice, st), "dict offsets");
+                if (!chars.empty()) cuda_check(cudaMemcpyAsync(dch->ptr, chars.data(), chars.size(), cudaMemcpyHostToDevice, st), "dict chars");
+                cuda_check(cudaStreamSynchronize(st), "dict upload");
+                keep.push_back(doff); keep.push_back(dch);
+                k.dict_offsets = (const int*)doff->ptr;
+                k.dict_chars = (const unsigned char*)dch->ptr;
                 break;
-            case TypeId::String: case TypeId::Binary:
-                if (c.is_dict) {
-                    k.kind = c.phys == Phys::I8 ? HK_DICT8 : c.phys == Phys::I16 ? HK_DICT16 : HK_DICT32;
-                    std::vector<int32_t> off{0};
-                    std::string chars;
-                    for (auto& v : c.dict->values) { chars += v; off.push_back((int32_t)chars.size()); }
-                    auto doff = std::make_shared<DeviceBuf>(off.size() * 4), dch = std::make_shared<DeviceBuf>(chars.size() + 16);
-                    cuda_check(cudaMemcpyAsync(doff->ptr, off.data(), off.size() * 4, cudaMemcpyHostToDevice, st), "dict offsets");
-                    if (!chars.empty()) cuda_check(cudaMemcpyAsync(dch->ptr, chars.data(), chars.size(), cudaMemcpyHostToDevice, st), "dict chars");
-                    cuda_check(cudaStreamSynchronize(st), "dict upload");
-                    keep.push_back(doff); keep.push_back(dch);
-                    k.dict_offsets = (const int*)doff->ptr;
-                    k.dict_chars = (const unsigned char*)dch->ptr;
-                } else {
-                    if (!c.offsets || !c.chars) throw Unsupported("string partition key without offsets/chars");
-                    k.kind = HK_UTF8;
-                    k.dict_offsets = (const int*)c.offsets->ptr;
-                    k.dict_chars = (const unsigned char*)c.chars->ptr;
-                }
+            }
+            case HK_UTF8:
+                if (!c.offsets || !c.chars) throw Unsupported("string partition key without offsets/chars");
+                k.dict_offsets = (const int*)c.offsets->ptr;
+                k.dict_chars = (const unsigned char*)c.chars->ptr;
                 break;
-            default: throw Unsupported("hash partitioning on " + c.type.str());
+            default: break;
             }
         }
         size_t nb = (size_t)(n + 1023) / 1024 + 1;
@@ -789,8 +801,8 @@ struct PartitionNode : ExecNode {
         auto row_idx = std::make_shared<DeviceBuf>((size_t)n * 8 + 16);
         cuda_check(cudaMemsetAsync(starts->ptr, 0, (size_t)(n_parts + 1) * 8, st), "memset starts");
         auto chunk_tmp = std::make_shared<DeviceBuf>((size_t)(partition_chunks(n) + 1) * n_parts * 8);
-        launch_partition(kc, n, (unsigned)n_parts, nullptr, (unsigned*)pids->ptr, (int*)hist->ptr, (long long*)base->ptr, (long long*)chunk_tmp->ptr,
-                         (long long*)starts->ptr, (long long*)row_idx->ptr, st);
+        cuda_check(launch_partition(kc, n, (unsigned)n_parts, nullptr, (unsigned*)pids->ptr, (int*)hist->ptr, (long long*)base->ptr, (long long*)chunk_tmp->ptr,
+                                    (long long*)starts->ptr, (long long*)row_idx->ptr, st), "partition launches");
         ctx->kernel_launches += 6;
         out.n_rows = n;
         out.cols.clear();
@@ -821,6 +833,7 @@ struct PartitionNode : ExecNode {
             }
             out.cols.push_back(o);
         }
+        cuda_check(cudaGetLastError(), "partition gathers");
         ctx->partition_starts.assign((size_t)n_parts + 1, 0);
         cuda_check(cudaMemcpyAsync(ctx->partition_starts.data(), starts->ptr, (size_t)(n_parts + 1) * 8, cudaMemcpyDeviceToHost, st), "starts D2H"); ctx->d2h_bytes += (int64_t)((size_t)(n_parts + 1) * 8);
         ctx->check_device_errors();
@@ -917,6 +930,15 @@ static ExecNodeP build_node(const OperatorP& op, ExecContext* ctx, PlanInputs* i
         for (auto& e : cur->hash_exprs) {
             if (e->kind != ExprKind::Bound) throw Unsupported("computed hash-partition keys (only plain column keys)");
             n->key_cols.push_back(e->index);
+        }
+        if (n->key_cols.size() > 8) throw Unsupported("more than 8 hash-partition keys");
+        if (n->n_parts > CB_MAX_HASH_PARTITIONS)
+            throw Unsupported("hash partitioning into " + std::to_string(n->n_parts) + " partitions (at most " + std::to_string((int)CB_MAX_HASH_PARTITIONS) + ")");
+        for (int ci : n->key_cols) { // refuses key types murmur3 has no rule for
+            if (ci < 0 || ci >= (int)cur->schema.size()) throw PlanError("hash-partition key out of range");
+            Column c;
+            c.type = cur->schema[(size_t)ci];
+            hash_key_kind(c);
         }
         return n;
     }
@@ -1032,11 +1054,41 @@ static std::vector<uint8_t> fetch_bits(ExecContext* ctx, const void* dev_bitmap,
     return out;
 }
 
+// Device columns whose values are not stored in the Arrow layout of their type get a converted copy (aot_kernels.h
+// launch_to_arrow_layout): INT32-backed int8 / int16 are narrowed, decimals stored in 4 or 8 bytes are sign-extended to Decimal128, and
+// bit-packed booleans are given one byte per row.  Idempotent: a converted column has the layout it reports.  Returns whether it launched.
+bool to_arrow_layout(Batch& b, ExecContext* ctx) {
+    const size_t n = (size_t)b.n_rows;
+    bool launched = false;
+    for (Column& c : b.cols) {
+        if (c.on_host || c.is_dict || !c.data) continue;
+        int conv = -1, w = 0;
+        if (c.type.id == TypeId::Bool && c.phys == Phys::Bitmap) {
+            if (c.bool_bytes) { c.data = c.bool_bytes; c.phys = Phys::I8; continue; }
+            conv = CB_BITS_TO_BYTES; w = 1;
+        } else if (c.type.is_decimal() && c.phys == Phys::I32) { conv = CB_SEXT32_TO_128; w = 16; }
+        else if (c.type.is_decimal() && c.phys == Phys::I64) { conv = CB_SEXT64_TO_128; w = 16; }
+        else if (c.type.id == TypeId::Int8 && c.phys == Phys::I32) { conv = CB_NARROW32_TO_8; w = 1; }
+        else if (c.type.id == TypeId::Int16 && c.phys == Phys::I32) { conv = CB_NARROW32_TO_16; w = 2; }
+        if (conv < 0) continue;
+        auto out = std::make_shared<DeviceBuf>(std::max<size_t>(n, 1) * (size_t)w);
+        launch_to_arrow_layout(conv, c.data->ptr, (long long)n, out->ptr, ctx->stream);
+        cuda_check(cudaGetLastError(), "to_arrow_layout launch");
+        ctx->kernel_launches++;
+        launched = true;
+        c.data = out;
+        c.phys = w == 16 ? Phys::I128 : w == 2 ? Phys::I16 : Phys::I8;
+        if (c.type.id == TypeId::Bool) c.bool_bytes = out;
+    }
+    return launched;
+}
+
 // rows [row0, row0 + n_rows) of batch b as Arrow C Data arrays (the caller's spark.comet.batchSize slices a large batch, CometConf.scala:539-544)
 void export_batch(Batch& b, ExecContext* ctx, ArrowArray* out_arrays, ArrowSchema* out_schemas, int n_cols, int64_t row0, int64_t n_rows) {
     TraceSpan ts("export_batch");
     if ((int)b.cols.size() != n_cols) throw PlanError("executePlan: caller passed " + std::to_string(n_cols) + " output slots, plan produces " + std::to_string(b.cols.size()) + " columns");
     if (row0 < 0 || n_rows < 0 || row0 + n_rows > b.n_rows) throw PlanError("export_batch: slice out of range");
+    to_arrow_layout(b, ctx);
     const size_t n = (size_t)n_rows, r0 = (size_t)row0;
     for (int i = 0; i < n_cols; i++) {
         Column& c = b.cols[(size_t)i];
@@ -1062,11 +1114,15 @@ void export_batch(Batch& b, ExecContext* ctx, ArrowArray* out_arrays, ArrowSchem
                 data.resize(data.size() + 8);
             }
         } else if (c.is_dict) {
-            // dictionary-coded string keys of a hash aggregate: fetch the codes, spell the strings out on the host
-            std::vector<int32_t> codes(n + 1);
-            if (n) cuda_check(cudaMemcpyAsync(codes.data(), (const uint8_t*)c.data->ptr + r0 * 4, n * 4, cudaMemcpyDeviceToHost, ctx->stream), "D2H key codes");
+            // dictionary-coded strings: fetch the codes (1, 2 or 4 bytes each, as the source delivered them), spell the strings out on the host
+            const size_t cw = c.phys == Phys::I8 ? 1 : c.phys == Phys::I16 ? 2 : 4;
+            std::vector<uint8_t> raw_codes(n * cw + 8);
+            if (n) cuda_check(cudaMemcpyAsync(raw_codes.data(), (const uint8_t*)c.data->ptr + r0 * cw, n * cw, cudaMemcpyDeviceToHost, ctx->stream), "D2H key codes");
             cuda_check(cudaStreamSynchronize(ctx->stream), "D2H sync");
-            ctx->d2h_bytes += (int64_t)n * 4;
+            ctx->d2h_bytes += (int64_t)(n * cw);
+            std::vector<int32_t> codes(n + 1);
+            for (size_t r = 0; r < n; r++)
+                codes[r] = cw == 1 ? (int32_t)(int8_t)raw_codes[r] : cw == 2 ? (int32_t)((const int16_t*)raw_codes.data())[r] : ((const int32_t*)raw_codes.data())[r];
             std::vector<uint8_t> vb = c.validity && n ? fetch_bits(ctx, c.validity->ptr, row0, n) : std::vector<uint8_t>((n + 7) / 8 + 8, 0xff);
             offs.resize((n + 1) * 4);
             int32_t* o = (int32_t*)offs.data();

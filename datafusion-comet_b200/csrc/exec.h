@@ -137,7 +137,8 @@ ExecNodeP build_exec(const OperatorP& op, ExecContext* ctx, PlanInputs* inputs);
 // native Parquet scan (scan_parquet.cpp)
 ExecNodeP make_native_scan(const OperatorP& op, ExecContext* ctx);
 
-// Export helpers (host-visible Arrow C Data)
+// Export helpers (host-visible Arrow C Data); to_arrow_layout gives every device column of b the Arrow layout of its type
+bool to_arrow_layout(Batch& b, ExecContext* ctx); // true if it launched conversions (on ctx->stream)
 void export_batch(Batch& b, ExecContext* ctx, ArrowArray* out_arrays, ArrowSchema* out_schemas, int n_cols, int64_t row0, int64_t n_rows);
 
 // Debug / build-time: generate (and NVRTC-compile, no device needed) the kernels a plan would use,

@@ -97,6 +97,8 @@ int cb200_plan_bind_table(cb200_plan* plan, int32_t input_index, cb200_table* t,
 void cb200_table_release(cb200_table* t);
 
 typedef struct cb200_device_column {
+    /* value_width: bytes per value of `values` -- the Arrow width of the type (BOOL: one byte per row, DECIMAL: 16), or the width of
+     * the codes (1, 2 or 4) of a dictionary-coded STRING column */
     int32_t type_id, precision, scale, value_width;
     const void* values;    /* device pointer (NULL when the column lives on the host: small aggregate results) */
     const void* validity;  /* device Arrow bitmap or NULL */
@@ -104,7 +106,7 @@ typedef struct cb200_device_column {
     const uint8_t* host_validity_bytes; /* one byte per row, or NULL */
     const void* validity_bytes;  /* device, one byte per row (ShuffleWriter plans: segments slice at any row) or NULL */
     const void* bool_bytes;      /* device, BOOL values one byte per row (ShuffleWriter plans) or NULL */
-    int32_t n_dict;              /* dictionary-coded STRING column: number of dictionary entries (values = int32 codes) */
+    int32_t n_dict;              /* dictionary-coded STRING column: number of dictionary entries (values = codes of value_width bytes) */
     int32_t pad;
 } cb200_device_column;
 /* i-th dictionary string of output column `col` of the last batch (valid until the next call on the plan) */
@@ -113,7 +115,8 @@ const char* cb200_plan_dict_value(cb200_plan* plan, int32_t col, int32_t i, int3
  * plan).  Returns rows, -1 at end, -2 on error. */
 int64_t cb200_execute_device(cb200_plan* plan, cb200_device_column* cols, int32_t n_cols, cb200_error* err);
 
-/* Plans rooted at a ShuffleWriter with HashPartition (operator.proto:688, partitioning.proto:38) return their
+/* Plans rooted at a ShuffleWriter with HashPartition (at most 8 key columns and 16 384 partitions; cb200_supports refuses more)
+ * (operator.proto:688, partitioning.proto:38) return their
  * child's rows reordered by partition id = pmod(murmur3(keys, seed 42), num_partitions) -- the reference's
  * multi_partition.rs:265-330 -- stable within a partition.  After each cb200_execute / cb200_execute_device
  * this returns the num_partitions+1 row offsets of that batch (the map-side of the exchange; the reference writes
