@@ -63,7 +63,7 @@ def f_float(field, v):
 DATA_TYPE_ID = dict(BOOL=0, INT8=1, INT16=2, INT32=3, INT64=4, FLOAT=5, DOUBLE=6, STRING=7, BYTES=8, TIMESTAMP=9,
                     DECIMAL=10, TIMESTAMP_NTZ=11, DATE=12, NULL=13)  # types.proto:43-66
 EXPR_FIELD = dict(literal=2, bound=3, add=4, subtract=5, multiply=6, divide=7, cast=8, eq=9, neq=10, gt=11, gt_eq=12,
-                  lt=13, lt_eq=14, is_null=15, is_not_null=16, **{"and": 17, "or": 18}, check_overflow=25, like=26,
+                  lt=13, lt_eq=14, is_null=15, is_not_null=16, **{"and": 17, "or": 18}, sort_order=19, check_overflow=25, like=26,
                   scalarFunc=31, caseWhen=38, **{"in": 39, "not": 40}, unary_minus=41, **{"if": 44}, unbound=51)  # expr.proto:30-109
 AGG_FIELD = dict(count=2, sum=3, min=4, max=5, avg=6)  # expr.proto:143-176
 OP_FIELD = dict(scan=100, projection=101, filter=102, sort=103, hash_agg=104, limit=105, shuffle_writer=106,
@@ -309,6 +309,19 @@ def hash_partitioning(exprs, num_partitions):  # partitioning.proto:38
 
 def shuffle_writer(child, partitioning, plan_id=0):  # operator.proto:688
     return _op("shuffle_writer", f_len(1, partitioning), (child,), plan_id)
+
+
+def sort_order(expr, descending=False, nulls_first=True):  # SortOrder expr.proto:385-389 (direction 1 = DESC, null_ordering 0 = NULLS FIRST)
+    return _expr("sort_order", f_len(1, expr) + f_varint(2, 1 if descending else 0) + f_varint(3, 0 if nulls_first else 1))
+
+
+def sort(child, orders, fetch=None, skip=None, plan_id=0):  # Sort operator.proto:641-645; TopK = the same message with fetch / skip
+    body = b"".join(f_len(1, o) for o in orders)
+    if fetch is not None:
+        body += f_varint(3, fetch)
+    if skip is not None:
+        body += f_varint(4, skip)
+    return _op("sort", body, (child,), plan_id)
 
 
 def struct_field(name, dt, nullable=True):  # SparkStructField operator.proto:97

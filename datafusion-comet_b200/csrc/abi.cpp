@@ -358,6 +358,10 @@ int cb200_plan_stats(cb200_plan* plan, cb200_stats* out) {
     out->agg_strategies = c.agg_strategies;
     out->scan_pruned_pages = c.scan_pruned_pages;
     out->scan_page_pruned_rows = c.scan_page_pruned_rows;
+    out->sort_rows = c.sort_rows;
+    out->sort_passes = c.sort_passes;
+    out->sort_pass_rows = c.sort_pass_rows;
+    out->sort_select_rows = c.sort_select_rows;
     return 0;
 }
 

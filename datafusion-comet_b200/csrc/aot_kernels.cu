@@ -6,6 +6,8 @@
 #include "device/cb_math.h"
 #include "device/cb_strpred.h"
 
+#include <algorithm>
+
 namespace cb200 {
 using namespace cb;
 
@@ -370,13 +372,13 @@ __global__ void k_pid_place(const u32* pids, i64 n, u32 n_parts, const i64* bloc
         __syncwarp();
     }
 }
-template <typename T> __global__ void k_gather_rows(const T* in, const i64* row_idx, i64 n, T* out) {
+template <typename T, typename I> __global__ void k_gather_rows(const T* in, const I* row_idx, i64 n, T* out) {
     i64 i = (i64)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) out[i] = in[row_idx[i]];
 }
-__global__ void k_gather_bits(const u8* in_bits, const i64* row_idx, i64 n, u8* out_bytes) {
+template <typename I> __global__ void k_gather_bits(const u8* in_bits, const I* row_idx, i64 n, u8* out_bytes) {
     i64 i = (i64)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) out_bytes[i] = bit_at(in_bits, row_idx[i]) ? 1 : 0;
+    if (i < n) out_bytes[i] = bit_at(in_bits, (i64)row_idx[i]) ? 1 : 0;
 }
 
 i64 partition_chunks(i64 n) { const i64 nb = (n + 1023) / 1024; return (nb + PID_CHUNK - 1) / PID_CHUNK; }
@@ -401,17 +403,296 @@ cudaError_t launch_partition(const HashKeyCols& kc, i64 n, u32 n_parts, u32* has
     k_pid_place<<<(unsigned)nb, 64, smem64, st>>>(pids, n, n_parts, block_base, row_idx);
     return cudaGetLastError();
 }
-void launch_gather(const void* in, int width, const i64* row_idx, i64 n, void* out, cudaStream_t st) {
+template <typename I> static void gather_rows(const void* in, int width, const I* row_idx, i64 n, void* out, cudaStream_t st) {
     if (n <= 0) return;
     unsigned blocks = (unsigned)((n + 255) / 256);
-    if (width == 16) k_gather_rows<ulonglong2><<<blocks, 256, 0, st>>>((const ulonglong2*)in, row_idx, n, (ulonglong2*)out);
-    else if (width == 8) k_gather_rows<u64><<<blocks, 256, 0, st>>>((const u64*)in, row_idx, n, (u64*)out);
-    else if (width == 4) k_gather_rows<u32><<<blocks, 256, 0, st>>>((const u32*)in, row_idx, n, (u32*)out);
-    else if (width == 2) k_gather_rows<u16><<<blocks, 256, 0, st>>>((const u16*)in, row_idx, n, (u16*)out);
-    else k_gather_rows<u8><<<blocks, 256, 0, st>>>((const u8*)in, row_idx, n, (u8*)out);
+    if (width == 16) k_gather_rows<ulonglong2, I><<<blocks, 256, 0, st>>>((const ulonglong2*)in, row_idx, n, (ulonglong2*)out);
+    else if (width == 8) k_gather_rows<u64, I><<<blocks, 256, 0, st>>>((const u64*)in, row_idx, n, (u64*)out);
+    else if (width == 4) k_gather_rows<u32, I><<<blocks, 256, 0, st>>>((const u32*)in, row_idx, n, (u32*)out);
+    else if (width == 2) k_gather_rows<u16, I><<<blocks, 256, 0, st>>>((const u16*)in, row_idx, n, (u16*)out);
+    else k_gather_rows<u8, I><<<blocks, 256, 0, st>>>((const u8*)in, row_idx, n, (u8*)out);
 }
+void launch_gather(const void* in, int width, const i64* row_idx, i64 n, void* out, cudaStream_t st) { gather_rows(in, width, row_idx, n, out, st); }
+void launch_gather(const void* in, int width, const u32* row_idx, i64 n, void* out, cudaStream_t st) { gather_rows(in, width, row_idx, n, out, st); }
 void launch_gather_bits(const void* in_bits, const i64* row_idx, i64 n, void* out_bytes, cudaStream_t st) {
-    if (n > 0) k_gather_bits<<<(unsigned)((n + 255) / 256), 256, 0, st>>>((const u8*)in_bits, row_idx, n, (u8*)out_bytes);
+    if (n > 0) k_gather_bits<i64><<<(unsigned)((n + 255) / 256), 256, 0, st>>>((const u8*)in_bits, row_idx, n, (u8*)out_bytes);
+}
+void launch_gather_bits(const void* in_bits, const u32* row_idx, i64 n, void* out_bytes, cudaStream_t st) {
+    if (n > 0) k_gather_bits<u32><<<(unsigned)((n + 255) / 256), 256, 0, st>>>((const u8*)in_bits, row_idx, n, (u8*)out_bytes);
+}
+
+// ---- sort: packed row keys, stable LSD radix sort -----------------------------------------------------------------------------------------
+// Keys are `W` 64-bit words per row (device/cb_sortkey.h), word 0 the most significant.  A pass sorts by one 8-bit digit, stably, over
+// tiles of SORT_TILE rows:
+//   k_sort_hist     : digit histogram of each tile, digit-major: hist[digit * n_tiles + tile]
+//   launch_scan_u32 : the select pipelines' chunked exclusive scan over that array, which in this order is the first output position of
+//                     (digit, tile) -- flat and coalesced (the partitioner's per-partition scan reads [tile][digit] with a 1 KB stride)
+//   k_sort_scatter  : moves keys and row indices; each of the 8 warps of a tile owns 512 consecutive rows, counts its digits, takes its
+//                     base from the warps before it, then walks its rows in order (a __match_any_sync rank per 32 rows): stable.
+//                     The tile is put in digit order in shared memory first and written out from there in runs.
+#define SORT_TILE 4096
+__global__ void __launch_bounds__(256) k_sort_keys(SortKeyCols kc, i64 n, u64* keys, u64* and_or) {
+    __shared__ u64 s_and[8][SK_MAX_WORDS], s_or[8][SK_MAX_WORDS];
+    u64 a[SK_MAX_WORDS] = {~0ull, ~0ull, ~0ull, ~0ull}, o[SK_MAX_WORDS] = {0, 0, 0, 0};
+    const int W = kc.words;
+    for (i64 i = (i64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (i64)gridDim.x * blockDim.x) {
+        u64 w[SK_MAX_WORDS] = {0, 0, 0, 0};
+        if (!sk_row(kc, i, w)) atomicOr(kc.err, 1 << 5);
+#pragma unroll
+        for (int j = 0; j < SK_MAX_WORDS; j++) {
+            if (j < W) keys[i * W + j] = w[j];
+            a[j] &= w[j];
+            o[j] |= w[j];
+        }
+    }
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int j = 0; j < SK_MAX_WORDS; j++) {
+#pragma unroll
+        for (int m = 16; m; m >>= 1) { a[j] &= __shfl_xor_sync(0xffffffffu, a[j], m); o[j] |= __shfl_xor_sync(0xffffffffu, o[j], m); }
+        if (lane == 0) { s_and[warp][j] = a[j]; s_or[warp][j] = o[j]; }
+    }
+    __syncthreads();
+    if (threadIdx.x < W) {
+        u64 ba = ~0ull, bo = 0;
+        for (int k = 0; k < 8; k++) { ba &= s_and[k][threadIdx.x]; bo |= s_or[k][threadIdx.x]; }
+        atomicAnd(&and_or[threadIdx.x], ba);
+        atomicOr(&and_or[W + threadIdx.x], bo);
+    }
+}
+void launch_sort_keys(const SortKeyCols& kc, i64 n, u64* keys, u64* and_or, cudaStream_t st) {
+    if (n <= 0) return;
+    const i64 blocks = std::min<i64>((n + 255) / 256, 132 * 16); // grid-stride: one and / or per block
+    k_sort_keys<<<(unsigned)blocks, 256, 0, st>>>(kc, n, keys, and_or);
+}
+
+template <int W> __global__ void __launch_bounds__(256) k_sort_hist(const u64* keys, i64 n, int digit, i64 n_tiles, u32* hist) {
+    __shared__ u32 h[256];
+    h[threadIdx.x] = 0;
+    __syncthreads();
+    const int word = W - 1 - (digit >> 3), sh = (digit & 7) * 8;
+    const i64 i0 = (i64)blockIdx.x * SORT_TILE;
+#pragma unroll 4
+    for (int k = threadIdx.x; k < SORT_TILE; k += 256) {
+        const i64 i = i0 + k;
+        if (i < n) atomicAdd(&h[(keys[i * W + word] >> sh) & 255u], 1u);
+    }
+    __syncthreads();
+    hist[(i64)threadIdx.x * n_tiles + blockIdx.x] = h[threadIdx.x];
+}
+
+// rows of a warp: r0 + k * 32 + lane, k < SORT_ITEMS; keys are staged in registers GROUP rows at a time.  Each row goes first to its
+// place in the tile ordered by digit (shared memory), and from there to the output: consecutive threads write consecutive positions of
+// a digit's run, instead of one scattered 8-byte key and 4-byte index per row.
+#define SORT_ITEMS (SORT_TILE / 8 / 32)
+template <int W> constexpr size_t sort_scatter_smem() { return (size_t)SORT_TILE * (8 * W + 4); }
+template <int W>
+__global__ void __launch_bounds__(256, 2) k_sort_scatter(const u64* kin, const u32* iin, i64 n, int digit, i64 n_tiles, const u32* hist,
+                                                      const u32* chunk_off, u64* kout, u32* iout) {
+    constexpr int GROUP = W <= 2 ? SORT_ITEMS : SORT_ITEMS / 2;
+    extern __shared__ u64 sm[];     // [W][SORT_TILE] key words, then [SORT_TILE] row indices: the tile in digit order
+    u64* skey = sm;
+    u32* sidx = (u32*)(sm + (size_t)W * SORT_TILE);
+    __shared__ u32 cur[8][256];     // per warp: digit count, then the warp's next tile position of each digit
+    __shared__ u32 dstart[256];     // tile position of each digit's first row
+    __shared__ u32 gbase[256];      // output position of each digit's first row
+    __shared__ u32 wsum[8];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int w = 0; w < 8; w++) cur[w][threadIdx.x] = 0;
+    __syncthreads();
+    const int word = W - 1 - (digit >> 3), sh = (digit & 7) * 8;
+    const i64 t0 = (i64)blockIdx.x * SORT_TILE, r0 = t0 + warp * (SORT_TILE / 8);
+    u32 dg[SORT_ITEMS];
+#pragma unroll
+    for (int k = 0; k < SORT_ITEMS; k++) {
+        const i64 i = r0 + k * 32 + lane;
+        dg[k] = i < n ? (u32)(kin[i * W + word] >> sh) & 255u : 256u + lane; // rows past the end match nobody
+    }
+#pragma unroll
+    for (int k = 0; k < SORT_ITEMS; k++)
+        if (dg[k] < 256u) atomicAdd(&cur[warp][dg[k]], 1u);
+    __syncthreads();
+    { // thread t: digit t.  Tile start of the digit = exclusive scan over digits; each warp's start after the warps before it
+        const u32 t = threadIdx.x;
+        u32 c[8], tot = 0;
+#pragma unroll
+        for (int w = 0; w < 8; w++) { c[w] = cur[w][t]; tot += c[w]; }
+        u32 incl = tot;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) { const u32 up = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += up; }
+        if (lane == 31) wsum[warp] = incl;
+        __syncthreads();
+        u32 run = incl - tot;
+        for (int w = 0; w < warp; w++) run += wsum[w];
+        dstart[t] = run;
+        const i64 at = (i64)t * n_tiles + blockIdx.x;
+        gbase[t] = hist[at] + chunk_off[at >> 12];
+#pragma unroll
+        for (int w = 0; w < 8; w++) { cur[w][t] = run; run += c[w]; }
+    }
+    __syncthreads();
+#pragma unroll
+    for (int g = 0; g < SORT_ITEMS; g += GROUP) {
+        u64 key[GROUP][W];
+        u32 id[GROUP];
+#pragma unroll
+        for (int k = 0; k < GROUP; k++) {
+            const i64 i = r0 + (g + k) * 32 + lane;
+            if (i < n) {
+#pragma unroll
+                for (int j = 0; j < W; j++) key[k][j] = kin[i * W + j];
+                id[k] = iin ? iin[i] : (u32)i;
+            }
+        }
+#pragma unroll
+        for (int k = 0; k < GROUP; k++) {
+            const u32 d = dg[g + k];
+            const u32 peers = __match_any_sync(0xffffffffu, d);
+            const int leader = __ffs(peers) - 1;
+            u32 base = 0;
+            if (d < 256u && lane == leader) { base = cur[warp][d]; cur[warp][d] = base + __popc(peers); }
+            base = __shfl_sync(0xffffffffu, base, leader);
+            if (d < 256u) {
+                const u32 l = base + __popc(peers & ((1u << lane) - 1u));
+#pragma unroll
+                for (int j = 0; j < W; j++) skey[j * SORT_TILE + l] = key[k][j];
+                sidx[l] = id[k];
+            }
+            __syncwarp();
+        }
+    }
+    __syncthreads();
+    const int rows = (int)min((i64)SORT_TILE, n - t0);
+    for (int l = threadIdx.x; l < rows; l += 256) {
+        u64 kw[W], dw = 0;
+#pragma unroll
+        for (int j = 0; j < W; j++) { kw[j] = skey[j * SORT_TILE + l]; if (j == word) dw = kw[j]; }
+        const u32 d = (u32)(dw >> sh) & 255u;
+        const i64 o = (i64)gbase[d] + (l - (int)dstart[d]);
+#pragma unroll
+        for (int j = 0; j < W; j++) kout[o * W + j] = kw[j];
+        iout[o] = sidx[l];
+    }
+}
+// ---- TopK selection: the key of the k-th row by an MSD radix select, then the rows before it in the stable order ------------------------
+// k_sort_select_hist: histogram of one digit over the rows whose key equals `want` under `mask` (the digits decided so far); one read of
+// the digit's word per row, shared-memory bins, one global add per bin and block.
+template <int W> __global__ void __launch_bounds__(256) k_sort_select_hist(const u64* keys, i64 n, SortSelectKey p, int digit, u32* hist) {
+    __shared__ u32 h[256];
+    h[threadIdx.x] = 0;
+    __syncthreads();
+    const int word = W - 1 - (digit >> 3), sh = (digit & 7) * 8;
+    for (i64 i = (i64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (i64)gridDim.x * blockDim.x) {
+        bool match = true;
+#pragma unroll
+        for (int j = 0; j < W; j++) match &= (keys[i * W + j] & p.mask[j]) == p.want[j];
+        if (match) atomicAdd(&h[(keys[i * W + word] >> sh) & 255u], 1u);
+    }
+    __syncthreads();
+    if (h[threadIdx.x]) atomicAdd(&hist[threadIdx.x], h[threadIdx.x]);
+}
+template <int W> __device__ __forceinline__ int sort_key_cmp(const u64* k, const SortSelectKey& p) { // -1 / 0 / 1: k against p.want
+#pragma unroll
+    for (int j = 0; j < W; j++)
+        if (k[j] != p.want[j]) return k[j] < p.want[j] ? -1 : 1;
+    return 0;
+}
+// eq[i] = row i's key equals the selected key
+template <int W> __global__ void k_sort_select_eq(const u64* keys, i64 n, SortSelectKey p, u8* eq) {
+    const i64 i = (i64)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) eq[i] = sort_key_cmp<W>(keys + i * W, p) == 0;
+}
+// keep[i] = key < selected, or key == selected and fewer than `r` equal rows come before it (eq_before: per 1024-row block, from
+// launch_compact_plan over eq).  Rows of a block in the (k, warp, lane) order k_compact_scatter uses: row order.
+template <int W> __global__ void k_sort_select_keep(const u64* keys, i64 n, SortSelectKey p, const i64* eq_before, i64 r, u8* keep) {
+    __shared__ i32 wcount[8];
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    i64 before = eq_before[blockIdx.x];
+    for (int k = 0; k < 4; k++) {
+        const i64 i = (i64)blockIdx.x * 1024 + k * 256 + threadIdx.x;
+        const int c = i < n ? sort_key_cmp<W>(keys + i * W, p) : 1;
+        const u32 bal = __ballot_sync(0xffffffffu, c == 0);
+        if (lane == 0) wcount[w] = __popc(bal);
+        __syncthreads();
+        i64 off = before;
+        int tot = 0;
+        for (int j = 0; j < 8; j++) { if (j < w) off += wcount[j]; tot += wcount[j]; }
+        if (i < n) keep[i] = c < 0 || (c == 0 && off + __popc(bal & ((1u << lane) - 1u)) < r);
+        before += tot;
+        __syncthreads();
+    }
+}
+template <int W> static void select_hist(const u64* keys, i64 n, const SortSelectKey& p, int digit, u32* hist, cudaStream_t st) {
+    const i64 blocks = std::min<i64>((n + 255) / 256, 132 * 8);
+    k_sort_select_hist<W><<<(unsigned)blocks, 256, 0, st>>>(keys, n, p, digit, hist);
+}
+template <int W> static void select_keep(const u64* keys, i64 n, const SortSelectKey& p, i64 r, u8* eq, i32* counts, i64* offsets, i64* total, u8* keep,
+                                         cudaStream_t st) {
+    k_sort_select_eq<W><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(keys, n, p, eq);
+    launch_compact_plan(eq, n, counts, offsets, total, st);
+    k_sort_select_keep<W><<<(unsigned)((n + 1023) / 1024), 256, 0, st>>>(keys, n, p, offsets, r, keep);
+}
+cudaError_t launch_sort_select_hist(const u64* keys, int words, i64 n, const SortSelectKey& p, int digit, u32* hist, cudaStream_t st) {
+    if (n <= 0) return cudaSuccess;
+    switch (words) {
+    case 1: select_hist<1>(keys, n, p, digit, hist, st); break;
+    case 2: select_hist<2>(keys, n, p, digit, hist, st); break;
+    case 3: select_hist<3>(keys, n, p, digit, hist, st); break;
+    default: select_hist<4>(keys, n, p, digit, hist, st); break;
+    }
+    return cudaGetLastError();
+}
+cudaError_t launch_sort_select_keep(const u64* keys, int words, i64 n, const SortSelectKey& p, i64 r, u8* eq, i32* counts, i64* offsets, i64* total,
+                                    u8* keep, cudaStream_t st) {
+    if (n <= 0) return cudaSuccess;
+    switch (words) {
+    case 1: select_keep<1>(keys, n, p, r, eq, counts, offsets, total, keep, st); break;
+    case 2: select_keep<2>(keys, n, p, r, eq, counts, offsets, total, keep, st); break;
+    case 3: select_keep<3>(keys, n, p, r, eq, counts, offsets, total, keep, st); break;
+    default: select_keep<4>(keys, n, p, r, eq, counts, offsets, total, keep, st); break;
+    }
+    return cudaGetLastError();
+}
+__global__ void k_sort_iota(u32* idx, i64 n) {
+    const i64 i = (i64)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) idx[i] = (u32)i;
+}
+void launch_sort_iota(unsigned* idx, i64 n, cudaStream_t st) {
+    if (n > 0) k_sort_iota<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(idx, n);
+}
+
+i64 sort_tiles(i64 n) { return (n + SORT_TILE - 1) / SORT_TILE; }
+
+template <int W> static cudaError_t sort_pass(const RadixScratch& s, i64 n, int digit, int from, bool first, cudaStream_t st) {
+    const i64 nt = sort_tiles(n);
+    k_sort_hist<W><<<(unsigned)nt, 256, 0, st>>>(s.keys[from], n, digit, nt, s.hist);
+    launch_scan_u32(s.hist, 256 * nt, 4096, s.chunk_off, s.total, st);
+    constexpr size_t smem = sort_scatter_smem<W>();
+    const cudaError_t e = cudaFuncSetAttribute((const void*)k_sort_scatter<W>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); // > 48 KB
+    if (e != cudaSuccess) return e;
+    k_sort_scatter<W><<<(unsigned)nt, 256, smem, st>>>(s.keys[from], first ? nullptr : s.idx[from], n, digit, nt, s.hist, s.chunk_off,
+                                                       s.keys[from ^ 1], s.idx[from ^ 1]);
+    return cudaGetLastError();
+}
+cudaError_t launch_sort_passes(const RadixScratch& s, int words, i64 n, const int* digits, int n_digits, int* result, cudaStream_t st) {
+    *result = 0;
+    if (n <= 0) return cudaSuccess;
+    if (n >= (i64)1 << 32 || words < 1 || words > SK_MAX_WORDS) return cudaErrorInvalidValue;
+    if (n_digits == 0) k_sort_iota<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(s.idx[0], n);
+    int from = 0;
+    for (int p = 0; p < n_digits; p++, from ^= 1) {
+        cudaError_t e;
+        switch (words) {
+        case 1: e = sort_pass<1>(s, n, digits[p], from, p == 0, st); break;
+        case 2: e = sort_pass<2>(s, n, digits[p], from, p == 0, st); break;
+        case 3: e = sort_pass<3>(s, n, digits[p], from, p == 0, st); break;
+        default: e = sort_pass<4>(s, n, digits[p], from, p == 0, st); break;
+        }
+        if (e != cudaSuccess) return e;
+    }
+    *result = from;
+    return cudaGetLastError();
 }
 
 // ---- device values -> Arrow layout (hand-off) ----------------------------------------------------------------------------------------

@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <cstdint>
 
+#include "device/cb_sortkey.h"
 #include "device/cb_strpred.h"
 
 namespace cb200 {
@@ -31,10 +32,8 @@ struct StringDictDev {
 void launch_dict_encode(const StringDictDev& d, const int* offsets, const unsigned char* chars, const unsigned char* validity, long long n,
                         int* row_slot, int* codes, cudaStream_t st);
 
-// hash partitioning (ShuffleWriter with HashPartition): murmur3 seed 42 chained over the key columns, pmod, stable counting sort
-// HK_BOOL reads an Arrow bitmap, HK_BOOL8 one byte per row; HK_DEC_SMALL_32 is a decimal(p <= 9) stored as INT32 (hashed as its i64)
-enum { HK_BOOL, HK_I8, HK_I16, HK_I32, HK_I64, HK_F32, HK_F64, HK_DEC_SMALL_128, HK_DEC_LARGE_128, HK_DEC_SMALL_64 = HK_I64, HK_DEC_LARGE_64 = 9,
-       HK_DICT8 = 10, HK_DICT16, HK_DICT32, HK_UTF8, HK_DEC_SMALL_32, HK_BOOL8 };
+// hash partitioning (ShuffleWriter with HashPartition): murmur3 seed 42 chained over the key columns, pmod, stable counting sort.
+// Key columns are read by their HK_* layout (device/cb_sortkey.h); HK_DEC_SMALL_32 is hashed as its i64.
 struct HashKeyCol {
     int kind;
     const void* data;
@@ -52,8 +51,41 @@ enum { CB_MAX_HASH_PARTITIONS = 16384 };
 // returns the first error of the launches (a launch the device refuses is reported here, not by a later synchronisation)
 cudaError_t launch_partition(const HashKeyCols& kc, long long n, unsigned n_parts, unsigned* hashes, unsigned* pids, int* block_hist, long long* block_base,
                       long long* chunk_tmp, long long* starts, long long* row_idx, cudaStream_t st);
+// out[i] = in[row_idx[i]] (width bytes per row), i < n; 64-bit (partitioning) or 32-bit (sort) row indices
 void launch_gather(const void* in, int width, const long long* row_idx, long long n, void* out, cudaStream_t st);
+void launch_gather(const void* in, int width, const unsigned* row_idx, long long n, void* out, cudaStream_t st);
 void launch_gather_bits(const void* in_bits, const long long* row_idx, long long n, void* out_bytes, cudaStream_t st);
+void launch_gather_bits(const void* in_bits, const unsigned* row_idx, long long n, void* out_bytes, cudaStream_t st);
+
+// ---- sort (SortExec / TopK): packed row keys (device/cb_sortkey.h), stable LSD radix sort of (key, row index) ----------------------------
+// k_sort_keys: kc.words 64-bit words per row into keys[n * words]; and_or[0, words) ANDs and and_or[words, 2 * words) ORs them over
+// all rows (the caller sets them to ~0 and 0 first): a digit equal in every row needs no pass.
+void launch_sort_keys(const cb::SortKeyCols& kc, long long n, unsigned long long* keys, unsigned long long* and_or, cudaStream_t st);
+// scratch of launch_sort_passes for n rows of `words` words: the key / index buffers come in pairs (keys[0] holds the input keys);
+// hist holds 256 x sort_tiles(n) entries, chunk_off 256 x sort_tiles(n) / 4096 + 1, total one
+struct RadixScratch {
+    unsigned long long* keys[2];
+    unsigned* idx[2];
+    unsigned* hist;
+    unsigned* chunk_off;
+    long long* total;
+};
+long long sort_tiles(long long n);
+// one stable counting-sort pass per digit in digits[0, n_digits) (8-bit digit d = bits [8d, 8d + 8) of the row key), least significant
+// first; n < 2^32.  The first pass reads row i's index as i; no digits: idx[0] = 0, 1, ... .  *result: which buffer pair holds the
+// sorted keys and indices.  Returns the first launch error.
+cudaError_t launch_sort_passes(const RadixScratch& s, int words, long long n, const int* digits, int n_digits, int* result, cudaStream_t st);
+// TopK selection.  A row key k "matches" when (k[j] & mask[j]) == want[j] for every word j.
+struct SortSelectKey {
+    unsigned long long mask[cb::SK_MAX_WORDS], want[cb::SK_MAX_WORDS];
+};
+// hist[256] += the histogram of digit `digit` over the matching rows (an MSD radix select step)
+cudaError_t launch_sort_select_hist(const unsigned long long* keys, int words, long long n, const SortSelectKey& p, int digit, unsigned* hist, cudaStream_t st);
+// keep[i] = row i is among the first rows of the stable order up to the selected key p.want: its key is smaller, or equal and fewer
+// than r equal rows precede it.  eq (n + 16 bytes), counts / offsets (n / 1024 + 1 entries) and total are scratch (launch_compact_plan).
+cudaError_t launch_sort_select_keep(const unsigned long long* keys, int words, long long n, const SortSelectKey& p, long long r, unsigned char* eq,
+                                    int* counts, long long* offsets, long long* total, unsigned char* keep, cudaStream_t st);
+void launch_sort_iota(unsigned* idx, long long n, cudaStream_t st); // idx[i] = i
 
 // device values -> the Arrow layout of their logical type, rows [0, n): what the hand-off (Arrow export, cb200_execute_device) gives out
 enum { CB_SEXT32_TO_128, CB_SEXT64_TO_128, CB_NARROW32_TO_8, CB_NARROW32_TO_16, CB_BITS_TO_BYTES };

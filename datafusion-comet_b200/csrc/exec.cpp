@@ -8,6 +8,7 @@
 #include <cstdlib>
 #include <ctime>
 #include <mutex>
+#include <unordered_map>
 
 namespace cb200 {
 
@@ -722,11 +723,11 @@ struct SelectNode : FusedBase {
 // =================================================================================================
 // hash repartitioning (ShuffleWriterExec with HashPartition, native/shuffle/src/partitioners/multi_partition.rs)
 // =================================================================================================
-// The murmur3 kind of a key column.  The logical type decides how Spark hashes a value (utils.rs: i8 / i16 / i32 / date as i32,
-// decimal(p <= 18) as i64, wider decimals as 16 bytes); the physical layout decides how it is read.  The Parquet scan keeps INT32-backed
-// int8 / int16 / decimal(p <= 9) columns 4 bytes wide, decimals with p <= 18 8 bytes wide (device tables too), and aggregate outputs keep
-// booleans one byte per row.
-static int hash_key_kind(const Column& c) {
+// The HK_* kind of a key column (device/cb_sortkey.h), for hash partitioning and the sort.  The logical type decides how Spark hashes
+// a value (utils.rs: i8 / i16 / i32 / date as i32, decimal(p <= 18) as i64, wider decimals as 16 bytes) and how many bits its sort key
+// takes; the physical layout decides how it is read.  The Parquet scan keeps INT32-backed int8 / int16 / decimal(p <= 9) columns 4 bytes
+// wide, decimals with p <= 18 8 bytes wide (device tables too), and aggregate outputs keep booleans one byte per row.
+static int key_kind(const Column& c) {
     const Phys ph = c.phys;
     switch (c.type.id) {
     case TypeId::Bool: return ph == Phys::Bitmap ? HK_BOOL : HK_BOOL8;
@@ -747,6 +748,84 @@ static int hash_key_kind(const Column& c) {
     }
 }
 
+// small host-resident aggregate results -> device columns
+static void columns_to_device(Batch& b, ExecContext* ctx) {
+    for (auto& c : b.cols) {
+        if (!c.on_host) continue;
+        size_t n = (size_t)b.n_rows;
+        if (c.type.is_string()) { // dictionary-encode on the host: these are group keys of a dense aggregate (a handful of rows)
+            auto d = std::make_shared<Dictionary>();
+            std::vector<int32_t> codes(n);
+            for (size_t r = 0; r < n; r++) {
+                std::string v((const char*)c.h_data.data() + c.h_offsets[r], (size_t)(c.h_offsets[r + 1] - c.h_offsets[r]));
+                auto it = std::find(d->values.begin(), d->values.end(), v);
+                if (it == d->values.end()) { codes[r] = (int32_t)d->values.size(); d->values.push_back(v); }
+                else codes[r] = (int32_t)(it - d->values.begin());
+            }
+            c.data = std::make_shared<DeviceBuf>(n * 4 + 16);
+            if (n) cuda_check(cudaMemcpyAsync(c.data->ptr, codes.data(), n * 4, cudaMemcpyHostToDevice, ctx->stream), "keys H2D");
+            cuda_check(cudaStreamSynchronize(ctx->stream), "keys H2D sync");
+            c.is_dict = true; c.dict = d; c.phys = Phys::I32;
+        } else if (c.type.id == TypeId::Bool) {
+            std::vector<uint8_t> bits((n + 7) / 8 + 8, 0);
+            for (size_t r = 0; r < n; r++) if (c.h_data[r]) bits[r >> 3] |= (uint8_t)(1u << (r & 7));
+            c.data = std::make_shared<DeviceBuf>(bits.size());
+            cuda_check(cudaMemcpyAsync(c.data->ptr, bits.data(), bits.size(), cudaMemcpyHostToDevice, ctx->stream), "bool H2D");
+            cuda_check(cudaStreamSynchronize(ctx->stream), "bool H2D sync");
+            c.phys = Phys::Bitmap;
+        } else {
+            c.data = std::make_shared<DeviceBuf>(c.h_data.size() + 16);
+            if (!c.h_data.empty()) cuda_check(cudaMemcpyAsync(c.data->ptr, c.h_data.data(), c.h_data.size(), cudaMemcpyHostToDevice, ctx->stream), "col H2D");
+            cuda_check(cudaStreamSynchronize(ctx->stream), "col H2D sync");
+            c.phys = phys_of(c.type);
+        }
+        if (!c.h_valid.empty()) {
+            std::vector<uint8_t> bits((n + 7) / 8 + 8, 0);
+            for (size_t r = 0; r < n; r++) if (c.h_valid[r]) bits[r >> 3] |= (uint8_t)(1u << (r & 7));
+            c.validity = std::make_shared<DeviceBuf>(bits.size());
+            cuda_check(cudaMemcpyAsync(c.validity->ptr, bits.data(), bits.size(), cudaMemcpyHostToDevice, ctx->stream), "validity H2D");
+            cuda_check(cudaStreamSynchronize(ctx->stream), "validity H2D sync");
+        }
+        c.on_host = false;
+    }
+}
+
+// out's columns = in's rows row_idx[0, n), in that order.  Bit-packed booleans and validity are gathered one byte per row and repacked
+// (the byte forms are kept: the exchange sends them).  `op` names the operator in the refusal of plain Utf8 columns.
+template <typename I> static void gather_columns(const Batch& in, const I* row_idx, int64_t n, Batch& out, ExecContext* ctx, const char* op) {
+    cudaStream_t st = ctx->stream;
+    out.n_rows = n;
+    out.cols.clear();
+    for (auto& c : in.cols) {
+        Column o = c;
+        if (c.offsets) throw Unsupported(std::string(op) + " plain string columns (dictionary-encode them first)");
+        int w = phys_bytes(c.is_dict && c.phys == Phys::I32 ? Phys::Dict32 : c.phys);
+        if (w == 0) { // bit-packed booleans: gather to bytes, repack
+            auto bytes = std::make_shared<DeviceBuf>((size_t)n + 16);
+            launch_gather_bits(c.data->ptr, row_idx, n, bytes->ptr, st);
+            o.data = std::make_shared<DeviceBuf>((size_t)(n + 31) / 32 * 4 + 8);
+            launch_bytes_to_bitmap((const unsigned char*)bytes->ptr, n, (uint32_t*)o.data->ptr, st);
+            o.bool_bytes = bytes;
+            ctx->kernel_launches += 2;
+        } else {
+            o.data = std::make_shared<DeviceBuf>((size_t)std::max<int64_t>(n, 1) * w);
+            launch_gather(c.data->ptr, w, row_idx, n, o.data->ptr, st);
+            ctx->kernel_launches++;
+            if (c.type.id == TypeId::Bool) o.bool_bytes = o.data; // aggregate outputs keep booleans one byte per row
+        }
+        if (c.validity) {
+            auto bytes = std::make_shared<DeviceBuf>((size_t)n + 16);
+            launch_gather_bits(c.validity->ptr, row_idx, n, bytes->ptr, st);
+            o.validity = std::make_shared<DeviceBuf>((size_t)(n + 31) / 32 * 4 + 8);
+            launch_bytes_to_bitmap((const unsigned char*)bytes->ptr, n, (uint32_t*)o.validity->ptr, st);
+            o.valid_bytes = bytes;
+            ctx->kernel_launches += 2;
+        }
+        out.cols.push_back(o);
+    }
+    cuda_check(cudaGetLastError(), "gathers");
+}
+
 // Output: the child's rows reordered so that partition p occupies rows [starts[p], starts[p+1]) -- what the
 // reference writes as per-partition IPC blocks, kept on the device for the NVLink exchange.
 struct PartitionNode : ExecNode {
@@ -759,7 +838,7 @@ struct PartitionNode : ExecNode {
         Batch in;
         if (!child->next(in)) return false;
         TraceSpan ts("partition");
-        to_device(in);
+        columns_to_device(in, ctx);
         int64_t n = in.n_rows;
         cudaStream_t st = ctx->stream;
         HashKeyCols kc;
@@ -770,7 +849,7 @@ struct PartitionNode : ExecNode {
             HashKeyCol& k = kc.col[kc.n++];
             k.data = c.data ? c.data->ptr : nullptr;
             k.validity = c.validity ? (const unsigned char*)c.validity->ptr : nullptr;
-            k.kind = hash_key_kind(c);
+            k.kind = key_kind(c);
             switch (k.kind) {
             case HK_DICT8: case HK_DICT16: case HK_DICT32: {
                 std::vector<int32_t> off{0};
@@ -804,82 +883,295 @@ struct PartitionNode : ExecNode {
         cuda_check(launch_partition(kc, n, (unsigned)n_parts, nullptr, (unsigned*)pids->ptr, (int*)hist->ptr, (long long*)base->ptr, (long long*)chunk_tmp->ptr,
                                     (long long*)starts->ptr, (long long*)row_idx->ptr, st), "partition launches");
         ctx->kernel_launches += 6;
-        out.n_rows = n;
-        out.cols.clear();
-        for (auto& c : in.cols) {
-            Column o = c;
-            if (c.offsets) throw Unsupported("repartitioning plain string columns (dictionary-encode them first)");
-            int w = phys_bytes(c.is_dict && c.phys == Phys::I32 ? Phys::Dict32 : c.phys);
-            if (w == 0) { // bit-packed booleans: gather to bytes, repack
-                auto bytes = std::make_shared<DeviceBuf>((size_t)n + 16);
-                launch_gather_bits(c.data->ptr, (const long long*)row_idx->ptr, n, bytes->ptr, st);
-                o.data = std::make_shared<DeviceBuf>((size_t)(n + 31) / 32 * 4 + 8);
-                launch_bytes_to_bitmap((const unsigned char*)bytes->ptr, n, (uint32_t*)o.data->ptr, st);
-                o.bool_bytes = bytes;
-                ctx->kernel_launches += 2;
-            } else {
-                o.data = std::make_shared<DeviceBuf>((size_t)std::max<int64_t>(n, 1) * w);
-                launch_gather(c.data->ptr, w, (const long long*)row_idx->ptr, n, o.data->ptr, st);
-                ctx->kernel_launches++;
-                if (c.type.id == TypeId::Bool) o.bool_bytes = o.data; // aggregate outputs keep booleans one byte per row
-            }
-            if (c.validity) {
-                auto bytes = std::make_shared<DeviceBuf>((size_t)n + 16);
-                launch_gather_bits(c.validity->ptr, (const long long*)row_idx->ptr, n, bytes->ptr, st);
-                o.validity = std::make_shared<DeviceBuf>((size_t)(n + 31) / 32 * 4 + 8);
-                launch_bytes_to_bitmap((const unsigned char*)bytes->ptr, n, (uint32_t*)o.validity->ptr, st);
-                o.valid_bytes = bytes;
-                ctx->kernel_launches += 2;
-            }
-            out.cols.push_back(o);
-        }
-        cuda_check(cudaGetLastError(), "partition gathers");
+        gather_columns(in, (const long long*)row_idx->ptr, n, out, ctx, "repartitioning");
         ctx->partition_starts.assign((size_t)n_parts + 1, 0);
         cuda_check(cudaMemcpyAsync(ctx->partition_starts.data(), starts->ptr, (size_t)(n_parts + 1) * 8, cudaMemcpyDeviceToHost, st), "starts D2H"); ctx->d2h_bytes += (int64_t)((size_t)(n_parts + 1) * 8);
         ctx->check_device_errors();
         return true;
     }
+};
 
-    // small host-resident aggregate results -> device columns
-    void to_device(Batch& b) {
-        for (auto& c : b.cols) {
-            if (!c.on_host) continue;
-            size_t n = (size_t)b.n_rows;
-            if (c.type.is_string()) { // dictionary-encode on the host: these are group keys of a dense aggregate (a handful of rows)
-                auto d = std::make_shared<Dictionary>();
-                std::vector<int32_t> codes(n);
-                for (size_t r = 0; r < n; r++) {
-                    std::string v((const char*)c.h_data.data() + c.h_offsets[r], (size_t)(c.h_offsets[r + 1] - c.h_offsets[r]));
-                    auto it = std::find(d->values.begin(), d->values.end(), v);
-                    if (it == d->values.end()) { codes[r] = (int32_t)d->values.size(); d->values.push_back(v); }
-                    else codes[r] = (int32_t)(it - d->values.begin());
-                }
-                c.data = std::make_shared<DeviceBuf>(n * 4 + 16);
-                if (n) cuda_check(cudaMemcpyAsync(c.data->ptr, codes.data(), n * 4, cudaMemcpyHostToDevice, ctx->stream), "keys H2D");
-                cuda_check(cudaStreamSynchronize(ctx->stream), "keys H2D sync");
-                c.is_dict = true; c.dict = d; c.phys = Phys::I32;
-            } else if (c.type.id == TypeId::Bool) {
-                std::vector<uint8_t> bits((n + 7) / 8 + 8, 0);
-                for (size_t r = 0; r < n; r++) if (c.h_data[r]) bits[r >> 3] |= (uint8_t)(1u << (r & 7));
-                c.data = std::make_shared<DeviceBuf>(bits.size());
-                cuda_check(cudaMemcpyAsync(c.data->ptr, bits.data(), bits.size(), cudaMemcpyHostToDevice, ctx->stream), "bool H2D");
-                cuda_check(cudaStreamSynchronize(ctx->stream), "bool H2D sync");
-                c.phys = Phys::Bitmap;
-            } else {
-                c.data = std::make_shared<DeviceBuf>(c.h_data.size() + 16);
-                if (!c.h_data.empty()) cuda_check(cudaMemcpyAsync(c.data->ptr, c.h_data.data(), c.h_data.size(), cudaMemcpyHostToDevice, ctx->stream), "col H2D");
-                cuda_check(cudaStreamSynchronize(ctx->stream), "col H2D sync");
-                c.phys = phys_of(c.type);
+// =================================================================================================
+// sort (SortExec(LexOrdering).with_fetch(fetch) then GlobalLimitExec(skip), planner.rs:1488-1522)
+// =================================================================================================
+// The output is the child's rows in a stable order of the keys (ties keep the input order: batches as they arrive, rows in order
+// within a batch), rows [skip, fetch).  Without a fetch, or with one above spark.comet.b200.chunkRows, the child is drained and its
+// batches concatenated on the device, sorted once and emitted as one batch.  With a smaller fetch (TopK) at most `fetch` candidate rows
+// are kept between chunks: each chunk is sorted, its first `fetch` rows are sorted together with the candidates (which come first, being
+// earlier input) and the first `fetch` of those become the next candidates, so device memory is bounded by fetch + one chunk.  Keys are
+// built again every round from the columns: a string's rank changes as its dictionary grows.
+struct SortNode : ExecNode {
+    ExecContext* ctx;
+    ExecNodeP child;
+    std::vector<SortKey> keys; // expr: Bound child column
+    int64_t fetch = -1, skip = 0;
+    bool done = false;
+    struct Rank { const Dictionary* dict = nullptr; size_t n = 0; DeviceBufP table; };
+    std::vector<Rank> ranks; // per key: code -> byte-order rank of the dictionary it was built for
+
+    bool topk() const { return fetch >= 0 && fetch <= ctx->chunk_rows; }
+
+    bool next(Batch& out) override {
+        if (done) return false;
+        done = true;
+        if (fetch == 0) return false;
+        TraceSpan ts("sort");
+        Batch all, in;
+        bool any = false;
+        if (topk()) {
+            while (child->next(in)) {
+                arrive(in);
+                if (in.n_rows == 0) continue;
+                // the chunk's own first `fetch` rows, then those merged behind the candidates (earlier input: first among equal keys)
+                Batch top;
+                sort_rows(in, 0, std::min<int64_t>(fetch, in.n_rows), top);
+                in = Batch();
+                if (any) {
+                    Batch u = concat({all, top});
+                    sort_rows(u, 0, std::min<int64_t>(fetch, u.n_rows), all);
+                } else all = std::move(top);
+                any = true;
             }
-            if (!c.h_valid.empty()) {
-                std::vector<uint8_t> bits((n + 7) / 8 + 8, 0);
-                for (size_t r = 0; r < n; r++) if (c.h_valid[r]) bits[r >> 3] |= (uint8_t)(1u << (r & 7));
-                c.validity = std::make_shared<DeviceBuf>(bits.size());
-                cuda_check(cudaMemcpyAsync(c.validity->ptr, bits.data(), bits.size(), cudaMemcpyHostToDevice, ctx->stream), "validity H2D");
-                cuda_check(cudaStreamSynchronize(ctx->stream), "validity H2D sync");
+        } else {
+            std::vector<Batch> batches;
+            while (child->next(in)) {
+                arrive(in);
+                if (in.n_rows > 0) batches.push_back(std::move(in));
+                in = Batch();
             }
-            c.on_host = false;
+            any = !batches.empty();
+            if (any) all = batches.size() == 1 ? std::move(batches[0]) : concat(batches);
         }
+        if (!any) return false;
+        const int64_t lo = std::min(skip, all.n_rows), hi = fetch >= 0 ? std::min(fetch, all.n_rows) : all.n_rows;
+        if (hi <= lo) return false;
+        if (topk() && lo == 0) { out = std::move(all); return true; } // the candidates are already in order
+        sort_rows(all, lo, hi, out);
+        return true;
+    }
+
+    void arrive(Batch& b) {
+        columns_to_device(b, ctx);
+        for (auto& c : b.cols)
+            if (c.offsets) throw Unsupported("sorting plain string columns (dictionary-encode them first)");
+    }
+
+    // b's rows in one batch (`bs` non-empty, every batch on the device): values and validity appended in order; dictionary-coded strings
+    // that carry different Dictionary objects are recoded into one (the first batch's entries, then the others' new entries)
+    Batch concat(const std::vector<Batch>& bs) {
+        cudaStream_t st = ctx->stream;
+        Batch out;
+        for (auto& b : bs) out.n_rows += b.n_rows;
+        const size_t n = (size_t)out.n_rows;
+        std::vector<DeviceBufP> temps;
+        for (size_t j = 0; j < bs[0].cols.size(); j++) {
+            const Column& c0 = bs[0].cols[j];
+            Column o;
+            o.type = c0.type;
+            o.phys = c0.phys;
+            o.is_dict = c0.is_dict;
+            o.dict = c0.dict;
+            bool same = true, nulls = false;
+            for (auto& b : bs) {
+                const Column& c = b.cols[j];
+                if (c.phys != c0.phys || c.dict != c0.dict || c.is_dict != c0.is_dict) same = false;
+                if (c.validity) nulls = true;
+            }
+            if (!same && !c0.is_dict) throw Unsupported("sort input whose batches store column " + std::to_string(j) + " in different layouts");
+            if (same) {
+                const int w = phys_bytes(c0.is_dict && c0.phys == Phys::I32 ? Phys::Dict32 : c0.phys);
+                o.data = std::make_shared<DeviceBuf>(w == 0 ? (n + 31) / 32 * 4 + 8 : std::max<size_t>(n, 1) * (size_t)w);
+                if (w == 0) cuda_check(cudaMemsetAsync(o.data->ptr, 0, o.data->bytes, st), "memset bools");
+                int64_t row = 0;
+                for (auto& b : bs) {
+                    const Column& c = b.cols[j];
+                    if (w == 0) { launch_bitmap_append((uint32_t*)o.data->ptr, row, (const uint8_t*)c.data->ptr, 0, b.n_rows, st); ctx->kernel_launches++; }
+                    else cuda_check(cudaMemcpyAsync((char*)o.data->ptr + (size_t)row * w, c.data->ptr, (size_t)b.n_rows * w, cudaMemcpyDeviceToDevice, st), "concat column");
+                    row += b.n_rows;
+                }
+            } else { // dictionary codes -> int32 codes of one dictionary
+                auto d = std::make_shared<Dictionary>(*c0.dict);
+                std::unordered_map<std::string, int32_t> code_of;
+                for (size_t k = d->values.size(); k-- > 0;) code_of[d->values[k]] = (int32_t)k;
+                o.phys = Phys::I32;
+                o.dict = d;
+                o.data = std::make_shared<DeviceBuf>(std::max<size_t>(n, 1) * 4);
+                int64_t row = 0;
+                for (auto& b : bs) {
+                    const Column& c = b.cols[j];
+                    std::vector<int32_t> table(c.dict->values.size());
+                    for (size_t k = 0; k < table.size(); k++) {
+                        if (c.dict == c0.dict) { table[k] = (int32_t)k; continue; }
+                        auto it = code_of.find(c.dict->values[k]);
+                        if (it == code_of.end()) { it = code_of.emplace(c.dict->values[k], (int32_t)d->values.size()).first; d->values.push_back(c.dict->values[k]); }
+                        table[k] = it->second;
+                    }
+                    auto dt = std::make_shared<DeviceBuf>(table.size() * 4 + 4);
+                    temps.push_back(dt);
+                    if (!table.empty()) cuda_check(cudaMemcpyAsync(dt->ptr, table.data(), table.size() * 4, cudaMemcpyHostToDevice, st), "H2D remap table");
+                    cuda_check(cudaStreamSynchronize(st), "remap table copy"); // table is a loop temporary
+                    const int w = c.phys == Phys::I8 ? 1 : c.phys == Phys::I16 ? 2 : 4;
+                    launch_remap_codes(c.data->ptr, w, b.n_rows, (const int*)dt->ptr, (int)table.size(), (int*)o.data->ptr + row, st);
+                    ctx->kernel_launches++;
+                    row += b.n_rows;
+                }
+            }
+            if (nulls) {
+                o.validity = std::make_shared<DeviceBuf>((n + 31) / 32 * 4 + 8);
+                cuda_check(cudaMemsetAsync(o.validity->ptr, 0, o.validity->bytes, st), "memset validity");
+                int64_t row = 0;
+                for (auto& b : bs) {
+                    const Column& c = b.cols[j];
+                    launch_bitmap_append((uint32_t*)o.validity->ptr, row, c.validity ? (const uint8_t*)c.validity->ptr : nullptr, 0, b.n_rows, st);
+                    ctx->kernel_launches++;
+                    row += b.n_rows;
+                }
+                o.null_count = -1;
+            }
+            out.cols.push_back(o);
+        }
+        cuda_check(cudaGetLastError(), "concat launches");
+        return out;
+    }
+
+    // the code -> rank table of dictionary d: equal strings get equal ranks, ranks follow unsigned byte order.  Rebuilt when the
+    // column carries another dictionary or its dictionary has grown.
+    const uint32_t* rank_table(size_t key, const DictionaryP& d) {
+        Rank& r = ranks[key];
+        if (r.table && r.dict == d.get() && r.n == d->values.size()) return (const uint32_t*)r.table->ptr;
+        const std::vector<std::string>& v = d->values;
+        std::vector<uint32_t> order(v.size()), rank(v.size() + 1, 0);
+        for (size_t i = 0; i < v.size(); i++) order[i] = (uint32_t)i;
+        std::sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return v[a] < v[b]; }); // char_traits<char>: unsigned bytes
+        uint32_t next = 0;
+        for (size_t i = 0; i < order.size(); i++) {
+            if (i > 0 && v[order[i]] != v[order[i - 1]]) next++;
+            rank[order[i]] = next;
+        }
+        r.table = std::make_shared<DeviceBuf>(rank.size() * 4);
+        cuda_check(cudaMemcpyAsync(r.table->ptr, rank.data(), rank.size() * 4, cudaMemcpyHostToDevice, ctx->stream), "H2D sort ranks");
+        cuda_check(cudaStreamSynchronize(ctx->stream), "sort ranks copy");
+        ctx->h2d_bytes += (int64_t)(rank.size() * 4);
+        r.dict = d.get();
+        r.n = v.size();
+        return (const uint32_t*)r.table->ptr;
+    }
+
+    // the stable order of m rows whose keys (`words` words each) are in keys0, by the given digits: row indices [0, m)
+    DeviceBufP radix_order(DeviceBufP keys0, int words, int64_t m, const std::vector<int>& digits) {
+        cudaStream_t st = ctx->stream;
+        const int64_t nt = sort_tiles(m);
+        auto keys1 = std::make_shared<DeviceBuf>((size_t)m * words * 8);
+        auto idx0 = std::make_shared<DeviceBuf>((size_t)m * 4), idx1 = std::make_shared<DeviceBuf>((size_t)m * 4);
+        auto hist = std::make_shared<DeviceBuf>((size_t)nt * 256 * 4), chunk_off = std::make_shared<DeviceBuf>((size_t)(nt * 256 / 4096 + 2) * 4);
+        auto total = std::make_shared<DeviceBuf>(8);
+        RadixScratch s{{(unsigned long long*)keys0->ptr, (unsigned long long*)keys1->ptr}, {(unsigned*)idx0->ptr, (unsigned*)idx1->ptr},
+                       (unsigned*)hist->ptr, (unsigned*)chunk_off->ptr, (long long*)total->ptr};
+        int r = 0;
+        cuda_check(launch_sort_passes(s, words, m, digits.data(), (int)digits.size(), &r, st), "sort passes");
+        ctx->kernel_launches += digits.empty() ? 1 : 4 * (int64_t)digits.size();
+        ctx->sort_passes += (int64_t)digits.size();
+        ctx->sort_pass_rows += m * (int64_t)digits.size();
+        return r ? idx1 : idx0; // the other buffers go back to the stream-ordered pool
+    }
+
+    // out = b's rows [lo, hi) of the stable order of the keys.  When only the first rows are wanted (lo = 0, hi < n: TopK), an MSD radix
+    // select finds the key of row hi - 1 of that order, the rows up to it are compacted (the smaller keys, then the equal ones in input
+    // order) and only those are sorted.
+    void sort_rows(const Batch& b, int64_t lo, int64_t hi, Batch& out) {
+        const int64_t n = b.n_rows;
+        if (n >= ((int64_t)1 << 32)) throw Unsupported("sorting 2^32 rows or more");
+        cudaStream_t st = ctx->stream;
+        cb::SortKeyCols kc;
+        memset(&kc, 0, sizeof(kc));
+        kc.n = (int)keys.size();
+        kc.err = ctx->d_err;
+        ranks.resize(keys.size());
+        int bits = 0;
+        for (size_t k = keys.size(); k-- > 0;) { // the last key is the least significant field
+            const Column& c = b.cols.at((size_t)keys[k].expr->index);
+            cb::SortKeyCol& f = kc.col[k];
+            f.kind = key_kind(c);
+            f.bits = sort_key_bits(c.type);
+            f.desc = keys[k].descending;
+            f.nulls_first = keys[k].nulls_first;
+            f.has_null = c.validity != nullptr;
+            f.data = c.data ? c.data->ptr : nullptr;
+            f.validity = c.validity ? (const uint8_t*)c.validity->ptr : nullptr;
+            if (c.is_dict) {
+                f.rank = rank_table(k, c.dict);
+                f.n_rank = (int)c.dict->values.size();
+            }
+            f.off = bits;
+            bits += f.bits + f.has_null;
+        }
+        const int W = kc.words = std::max(1, (bits + 63) / 64);
+        auto keys0 = std::make_shared<DeviceBuf>((size_t)n * W * 8);
+        auto and_or = std::make_shared<DeviceBuf>(2 * cb::SK_MAX_WORDS * 8);
+        cuda_check(cudaMemsetAsync(and_or->ptr, 0xff, (size_t)W * 8, st), "memset key and");
+        cuda_check(cudaMemsetAsync((char*)and_or->ptr + W * 8, 0, (size_t)W * 8, st), "memset key or");
+        launch_sort_keys(kc, n, (unsigned long long*)keys0->ptr, (unsigned long long*)and_or->ptr, st);
+        cuda_check(cudaGetLastError(), "k_sort_keys launch");
+        ctx->kernel_launches++;
+        ctx->sort_rows += n;
+        uint64_t h_and_or[2 * cb::SK_MAX_WORDS];
+        cuda_check(cudaMemcpyAsync(h_and_or, and_or->ptr, (size_t)W * 16, cudaMemcpyDeviceToHost, st), "D2H key and / or");
+        ctx->check_device_errors(); // also synchronises; a dictionary code outside its dictionary fails here
+        std::vector<int> digits; // the 8-bit digits that differ between rows, least significant first
+        for (int d = 0; d < (bits + 7) / 8; d++) {
+            const int w = W - 1 - d / 8, sh = (d % 8) * 8;
+            if (((h_and_or[w] ^ h_and_or[W + w]) >> sh) & 0xff) digits.push_back(d);
+        }
+        if (lo > 0 || hi >= n) {
+            DeviceBufP idx = radix_order(keys0, W, n, digits);
+            keys0.reset();
+            gather_columns(b, (const unsigned*)idx->ptr + lo, hi - lo, out, ctx, "sorting");
+            ctx->check_device_errors();
+            return;
+        }
+        // select: bits equal in every row are decided already; then one histogram per differing digit, most significant first
+        SortSelectKey p;
+        for (int j = 0; j < W; j++) { p.mask[j] = ~(h_and_or[j] ^ h_and_or[W + j]); p.want[j] = h_and_or[j] & p.mask[j]; }
+        int64_t r = hi; // the selected key's rank among the rows that match p
+        auto hist = std::make_shared<DeviceBuf>(256 * 4);
+        std::vector<uint32_t> hh(256);
+        for (size_t q = digits.size(); q-- > 0;) {
+            const int d = digits[q], w = W - 1 - d / 8, sh = (d % 8) * 8;
+            cuda_check(cudaMemsetAsync(hist->ptr, 0, 256 * 4, st), "memset select histogram");
+            cuda_check(launch_sort_select_hist((const unsigned long long*)keys0->ptr, W, n, p, d, (unsigned*)hist->ptr, st), "select histogram");
+            ctx->kernel_launches++;
+            ctx->sort_select_rows += n;
+            cuda_check(cudaMemcpyAsync(hh.data(), hist->ptr, 256 * 4, cudaMemcpyDeviceToHost, st), "D2H select histogram");
+            cuda_check(cudaStreamSynchronize(st), "select histogram sync");
+            int v = 0;
+            for (; v < 255 && r > (int64_t)hh[(size_t)v]; v++) r -= hh[(size_t)v];
+            p.mask[w] |= (uint64_t)0xff << sh;
+            p.want[w] |= (uint64_t)v << sh;
+        }
+        const size_t nb = (size_t)(n + 1023) / 1024;
+        auto eq = std::make_shared<DeviceBuf>((size_t)n + 16), keep = std::make_shared<DeviceBuf>((size_t)n + 16);
+        auto counts = std::make_shared<DeviceBuf>(nb * 4 + 4), offsets = std::make_shared<DeviceBuf>(nb * 8 + 8), kept = std::make_shared<DeviceBuf>(8);
+        cuda_check(launch_sort_select_keep((const unsigned long long*)keys0->ptr, W, n, p, r, (unsigned char*)eq->ptr, (int*)counts->ptr,
+                                           (long long*)offsets->ptr, (long long*)kept->ptr, (unsigned char*)keep->ptr, st), "select keep");
+        launch_compact_plan((const unsigned char*)keep->ptr, n, (int*)counts->ptr, (long long*)offsets->ptr, (long long*)kept->ptr, st);
+        auto rows = std::make_shared<DeviceBuf>((size_t)n * 4);
+        launch_sort_iota((unsigned*)rows->ptr, n, st);
+        auto ckeys = std::make_shared<DeviceBuf>((size_t)hi * W * 8), crows = std::make_shared<DeviceBuf>((size_t)hi * 4);
+        launch_compact_scatter((const unsigned char*)keep->ptr, n, (const long long*)offsets->ptr, keys0->ptr, W * 8, ckeys->ptr, st);
+        launch_compact_scatter((const unsigned char*)keep->ptr, n, (const long long*)offsets->ptr, rows->ptr, 4, crows->ptr, st);
+        cuda_check(cudaGetLastError(), "select compaction");
+        ctx->kernel_launches += 9;
+        int64_t m = 0;
+        cuda_check(cudaMemcpyAsync(&m, kept->ptr, 8, cudaMemcpyDeviceToHost, st), "D2H kept rows");
+        cuda_check(cudaStreamSynchronize(st), "select sync");
+        if (m != hi) throw ExecError(15, "", "internal: TopK selection kept " + std::to_string(m) + " rows for a fetch of " + std::to_string(hi));
+        keys0.reset(); rows.reset(); eq.reset(); keep.reset();
+        DeviceBufP order = radix_order(ckeys, W, m, digits);
+        auto idx = std::make_shared<DeviceBuf>((size_t)m * 4);
+        launch_gather(crows->ptr, 4, (const unsigned*)order->ptr, m, idx->ptr, st); // compacted position -> row of b
+        ctx->kernel_launches++;
+        gather_columns(b, (const unsigned*)idx->ptr, m, out, ctx, "sorting");
+        ctx->check_device_errors();
     }
 };
 
@@ -938,8 +1230,20 @@ static ExecNodeP build_node(const OperatorP& op, ExecContext* ctx, PlanInputs* i
             if (ci < 0 || ci >= (int)cur->schema.size()) throw PlanError("hash-partition key out of range");
             Column c;
             c.type = cur->schema[(size_t)ci];
-            hash_key_kind(c);
+            key_kind(c);
         }
+        return n;
+    }
+    if (cur->kind == OpKind::Sort) {
+        auto n = std::make_shared<SortNode>();
+        n->ctx = ctx;
+        n->child = build_node(cur->children[0], ctx, inputs, build_only, assume);
+        n->schema = cur->schema;
+        n->keys = cur->sort_keys;
+        n->fetch = cur->fetch;
+        n->skip = std::max<int64_t>(cur->skip, 0);
+        for (auto& k : n->keys)
+            if (k.expr->index < 0 || k.expr->index >= (int)cur->schema.size()) throw PlanError("sort key out of range");
         return n;
     }
     if (cur->kind == OpKind::HashAgg) { agg_op = cur; cur = cur->children[0]; }
@@ -987,9 +1291,11 @@ std::vector<GeneratedKernel> plan_kernels_for_build(const OperatorP& op, const s
         if (auto f = std::dynamic_pointer_cast<FusedBase>(n)) {
             for (const PipelineSpec& s : f->build_specs()) out.push_back(generate_pipeline(s));
             n = f->child;
+        } else if (auto pn = std::dynamic_pointer_cast<PartitionNode>(n)) {
+            n = pn->child;
         } else {
-            auto pn = std::dynamic_pointer_cast<PartitionNode>(n);
-            n = pn ? pn->child : nullptr;
+            auto sn = std::dynamic_pointer_cast<SortNode>(n);
+            n = sn ? sn->child : nullptr;
         }
     }
     return out;

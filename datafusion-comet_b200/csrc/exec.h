@@ -104,6 +104,8 @@ struct ExecContext {
     int64_t scan_pruned_row_groups = 0, scan_pruned_rows = 0; // Parquet row groups skipped by statistics (parquet_exec.rs:143-196)
     int64_t scan_pruned_pages = 0, scan_page_pruned_rows = 0;  // data pages / rows of kept row groups skipped by the page index
     int64_t agg_strategies = 0;   // CB200_AGG_* bits of the aggregate strategies that ran
+    int64_t sort_rows = 0, sort_passes = 0, sort_pass_rows = 0; // rows Sort operators radix-sorted, the digit passes they ran, rows moved
+    int64_t sort_select_rows = 0; // rows TopK's radix select read (one read per digit step)
     std::vector<int64_t> partition_starts; // last ShuffleWriter batch: partition p = rows [starts[p], starts[p+1])
     void check_device_errors();
     void collect_timing();

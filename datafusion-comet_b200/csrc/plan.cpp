@@ -733,11 +733,64 @@ static OperatorP decode_operator(PbReader r) { // Operator operator.proto:32-86
         have = true;
         break;
     }
+    case 103: { // Sort operator.proto:641-645 (planner.rs:1488-1522); TopK is the same message with fetch / skip (CometExecUtils.getTopKNativePlan)
+        op->kind = OpKind::Sort;
+        while (b.next()) {
+            if (b.field == 1 && b.wire == 2) {
+                PbReader e = b.sub();
+                bool have_order = false;
+                SortKey k;
+                while (e.next()) {
+                    if (e.field != 19 || e.wire != 2) { e.skip(); continue; } // SortOrder expr.proto:385-389
+                    have_order = true;
+                    PbReader so = e.sub();
+                    while (so.next()) {
+                        if (so.field == 1) k.expr = decode_expr(so.sub());
+                        else if (so.field == 2) k.descending = so.i64() == 1;
+                        else if (so.field == 3) k.nulls_first = so.i64() == 0;
+                        else so.skip();
+                    }
+                }
+                if (!have_order || !k.expr) throw PlanError("sort key is not a SortOrder with a child");
+                op->sort_keys.push_back(k);
+            } else if (b.field == 3 || b.field == 4) {
+                const int32_t v = (int32_t)b.i64(); // optional int32
+                if (v < 0) throw PlanError(std::string("sort ") + (b.field == 3 ? "fetch" : "skip") + " is negative");
+                (b.field == 3 ? op->fetch : op->skip) = v;
+            } else b.skip();
+        }
+        const auto& cs = child_schema();
+        if (op->sort_keys.empty()) throw PlanError("sort without keys");
+        if (op->sort_keys.size() > MAX_SORT_KEYS) throw Unsupported("more than 8 sort keys");
+        int bits = 0;
+        for (auto& k : op->sort_keys) {
+            resolve(*k.expr, cs);
+            if (k.expr->kind != ExprKind::Bound) throw Unsupported("computed sort keys (only plain column keys)");
+            bits += sort_key_bits(k.expr->type) + 1; // every key may hold NULLs: one null bit each
+        }
+        if (bits > MAX_SORT_KEY_BITS) throw Unsupported("sort keys of " + std::to_string(bits) + " bits (at most 256 bits of packed key)");
+        op->schema = cs;
+        have = true;
+        break;
+    }
     default:
         throw Unsupported("operator field " + std::to_string(f) + " is outside the GPU hot path");
     }
     if (!have) throw PlanError("operator not decoded");
     return op;
+}
+
+int sort_key_bits(const DType& t) {
+    switch (t.id) {
+    case TypeId::Bool: return 1;
+    case TypeId::Int8: return 8;
+    case TypeId::Int16: return 16;
+    case TypeId::Int32: case TypeId::Date: case TypeId::Float32: return 32;
+    case TypeId::Int64: case TypeId::Timestamp: case TypeId::TimestampNtz: case TypeId::Float64: return 64;
+    case TypeId::Decimal: return t.precision <= 18 ? 64 : 128;
+    case TypeId::String: return 32; // the rank of a dictionary code
+    default: throw Unsupported("sort key of type " + t.str());
+    }
 }
 
 OperatorP decode_plan(const uint8_t* data, size_t len) {

@@ -101,7 +101,14 @@ struct AggExpr {
     ExprP filter;                // FILTER (WHERE ...) clause, Partial mode only
 };
 
-enum class OpKind { Scan, ShuffleScan, NativeScan, Projection, Filter, HashAgg, ShuffleWriter };
+enum class OpKind { Scan, ShuffleScan, NativeScan, Projection, Filter, HashAgg, ShuffleWriter, Sort };
+
+// one ORDER BY key (SortOrder expr.proto:385-389, planner.rs:927-950 create_sort_expr): arrow SortOptions{descending, nulls_first}
+struct SortKey {
+    ExprP expr;               // a Bound column reference of the child
+    bool descending = false;  // direction == 1
+    bool nulls_first = true;  // null_ordering == 0
+};
 
 struct StructField {
     std::string name;
@@ -137,7 +144,16 @@ struct Operator {
     // ShuffleWriter (hash partitioning only)
     std::vector<ExprP> hash_exprs;
     int num_partitions = 0;
+    // Sort (operator.proto:641-645): the output is sorted[skip : fetch] (SortExec::with_fetch, then GlobalLimitExec(skip));
+    // -1 = the field is absent
+    std::vector<SortKey> sort_keys;
+    int64_t fetch = -1, skip = -1;
 };
+
+// Sort keys at most: 8 keys, 256 bits of packed key (value bits by declared type plus one null bit per key, sort_key_bits)
+enum { MAX_SORT_KEYS = 8, MAX_SORT_KEY_BITS = 256 };
+// value bits of a sort key of type t in the packed row key; throws Unsupported for types outside the sort
+int sort_key_bits(const DType& t);
 
 // Decode + resolve types.  Throws Unsupported for anything outside the GPU hot path and PlanError
 // for malformed plans.

@@ -189,6 +189,10 @@ typedef struct cb200_stats {
     int64_t agg_strategies;    /* OR of CB200_AGG_* over the plan's aggregates: which accumulation strategies ran */
     int64_t scan_pruned_pages; /* Parquet data pages of read columns not uploaded because the page index rules the pushed filters out */
     int64_t scan_page_pruned_rows; /* rows of row groups the statistics kept that the page index ruled out */
+    int64_t sort_rows;         /* rows Sort operators built keys for and radix-sorted (TopK: every chunk and every merge with the candidates) */
+    int64_t sort_passes;       /* radix passes they ran: one per 8-bit key digit that is not the same in every row */
+    int64_t sort_pass_rows;    /* rows those passes moved, summed over the passes */
+    int64_t sort_select_rows;  /* rows TopK's radix select read, summed over its digit steps */
 } cb200_stats;
 #define CB200_AGG_DENSE 1      /* thread-private accumulators over dictionary / bool key codes (and ungrouped aggregates) */
 #define CB200_AGG_TABLE 2      /* global key table */
