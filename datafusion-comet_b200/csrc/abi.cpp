@@ -3,7 +3,7 @@
 
 #include "abi_internal.h"
 #include "parquet_kernels.h"
-#include "exec.h"
+#include "exec_internal.h"
 #include "jit.h"
 #include "plan.h"
 #include "proto_wire.h"
@@ -208,7 +208,7 @@ int64_t cb200_execute_device(cb200_plan* plan, cb200_device_column* cols, int32_
                 o.validity = c.validity ? c.validity->ptr : nullptr;
                 o.validity_bytes = c.valid_bytes ? c.valid_bytes->ptr : nullptr;
                 o.bool_bytes = c.bool_bytes ? c.bool_bytes->ptr : nullptr;
-                if (c.is_dict) { o.n_dict = (int)c.dict->values.size(); o.value_width = phys_bytes(c.phys == Phys::I32 ? Phys::Dict32 : c.phys); }
+                if (c.is_dict) { o.n_dict = (int)c.dict->values().size(); o.value_width = phys_bytes(c.phys); }
             }
         }
     });
@@ -251,7 +251,7 @@ int cb200_table_add_column(cb200_table* t, int32_t type_id, int32_t precision, i
             if (!c.type.is_string()) throw PlanError("dictionary values on a non-string column");
             c.is_dict = true;
             c.dict = std::make_shared<Dictionary>();
-            for (int i = 0; i < n_dict; i++) c.dict->values.push_back(dict_values[i]);
+            for (int i = 0; i < n_dict; i++) c.dict->append(dict_values[i]);
             c.phys = value_width == 1 ? Phys::I8 : value_width == 2 ? Phys::I16 : Phys::I32;
             if (value_width != 1 && value_width != 2 && value_width != 4) throw PlanError("dictionary codes must be 1, 2 or 4 bytes wide");
         } else if (c.type.is_string()) {
@@ -262,16 +262,7 @@ int cb200_table_add_column(cb200_table* t, int32_t type_id, int32_t precision, i
         } else {
             int w = c.type.arrow_width();
             if (value_width != w) throw PlanError("value_width " + std::to_string(value_width) + " does not match " + c.type.str());
-            switch (c.type.id) {
-            case TypeId::Bool: c.phys = Phys::Bitmap; break;
-            case TypeId::Int8: c.phys = Phys::I8; break;
-            case TypeId::Int16: c.phys = Phys::I16; break;
-            case TypeId::Int32: case TypeId::Date: c.phys = Phys::I32; break;
-            case TypeId::Float32: c.phys = Phys::F32; break;
-            case TypeId::Float64: c.phys = Phys::F64; break;
-            case TypeId::Decimal: c.phys = Phys::I128; break;
-            default: c.phys = Phys::I64; break;
-            }
+            c.phys = phys_of(c.type);
         }
         if (((uintptr_t)dev_values & 15) || ((uintptr_t)dev_validity & 15)) throw PlanError("device buffers must be 16-byte aligned");
         size_t bytes = value_width == 0 ? (n + 7) / 8 : n * (size_t)value_width;
@@ -286,9 +277,10 @@ int cb200_table_add_column(cb200_table* t, int32_t type_id, int32_t precision, i
 const char* cb200_plan_dict_value(cb200_plan* plan, int32_t col, int32_t i, int32_t* len) {
     if (!plan || col < 0 || col >= (int)plan->last.cols.size()) return nullptr;
     const Column& c = plan->last.cols[(size_t)col];
-    if (!c.is_dict || !c.dict || i < 0 || i >= (int)c.dict->values.size()) return nullptr;
-    if (len) *len = (int32_t)c.dict->values[(size_t)i].size();
-    return c.dict->values[(size_t)i].data();
+    if (!c.is_dict || !c.dict || i < 0 || i >= (int)c.dict->values().size()) return nullptr;
+    const std::string& v = c.dict->values()[(size_t)i];
+    if (len) *len = (int32_t)v.size();
+    return v.data();
 }
 
 int cb200_table_add_column_bytes(cb200_table* t, int32_t type_id, int32_t precision, int32_t scale, int32_t value_width, const void* dev_values,

@@ -131,7 +131,7 @@ struct DenseState {
                 if (isnull) { c.h_valid[r] = 0; any_null = true; }
                 if (is_bool) c.h_data.push_back(isnull ? 0 : (uint8_t)codes[r]);
                 else {
-                    if (!isnull) { const std::string& s = key_dicts[k]->values.at((size_t)codes[r]); c.h_data.insert(c.h_data.end(), s.begin(), s.end()); }
+                    if (!isnull) { const std::string& s = key_dicts[k]->values().at((size_t)codes[r]); c.h_data.insert(c.h_data.end(), s.begin(), s.end()); }
                     c.h_offsets.push_back((int32_t)c.h_data.size());
                 }
             }
@@ -263,7 +263,7 @@ struct IdRows {
         for (size_t i = 0; i < g.out_cols.size(); i++) {
             Column c;
             c.type = g.out_cols[i].type;
-            c.phys = c.type.id == TypeId::Bool ? Phys::I8 : (c.type.is_string() ? Phys::I32 : phys_of(c.type));
+            c.phys = kernel_out_phys(c.type);
             c.data = std::make_shared<DeviceBuf>(rows_alloc * g.out_bytes[i]);
             vbytes.push_back(std::make_shared<DeviceBuf>(rows_alloc));
             fp.out[i] = (cb::u8*)c.data->ptr;
@@ -279,9 +279,7 @@ struct IdRows {
             for (size_t i = 0; i < out.cols.size(); i++) {
                 Column& c = out.cols[i];
                 c.valid_bytes = vbytes[i];
-                c.validity = std::make_shared<DeviceBuf>((size_t)(n_out + 31) / 32 * 4 + 8);
-                launch_bytes_to_bitmap((const unsigned char*)vbytes[i]->ptr, n_out, (uint32_t*)c.validity->ptr, ctx->stream);
-                ctx->kernel_launches++;
+                c.validity = bytes_to_bitmap(vbytes[i], n_out, ctx);
                 c.null_count = -1;
                 if (c.type.id == TypeId::Bool) c.bool_bytes = c.data;
             }
@@ -506,7 +504,7 @@ struct AggNode : FusedBase {
         if (!c.type.is_string()) return -1; // integer / date / decimal keys: hash aggregation
         if (c.is_dict) {
             key_dicts[k] = c.dict;
-            return (int)c.dict->values.size();
+            return (int)c.dict->values().size();
         }
         // plain Utf8 -> device dictionary builder
         if (!dev_dicts[k]) {
@@ -551,7 +549,7 @@ struct AggNode : FusedBase {
             for (int i = dd.host_known; i < n_codes; i++) {
                 std::string s((size_t)len[(size_t)i], '\0');
                 if (len[(size_t)i]) cuda_check(cudaMemcpy(&s[0], dd.d.bytes + off[(size_t)i], (size_t)len[(size_t)i], cudaMemcpyDeviceToHost), "dict bytes");
-                key_dicts[k]->values.push_back(s);
+                key_dicts[k]->append(s); // the device builder hands out codes in order: entry i is code i
             }
             dd.host_known = n_codes;
         }

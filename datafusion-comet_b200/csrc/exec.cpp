@@ -8,7 +8,6 @@
 #include <cstdlib>
 #include <ctime>
 #include <mutex>
-#include <unordered_map>
 
 namespace cb200 {
 
@@ -189,7 +188,7 @@ void StrMasks::bind(cb::PipeParams& p, const PipelineSpec& spec, const Batch& b,
             m.dev.lit = base + o_lit;
         }
         if (m.dict != c.dict) { m.dict = c.dict; m.done = 0; }
-        const std::vector<std::string>& vals = c.dict->values;
+        const std::vector<std::string>& vals = c.dict->values();
         const int64_t n = (int64_t)vals.size();
         if (n > INT32_MAX) throw Unsupported("string predicate over a dictionary of more than 2^31 entries");
         const size_t words = (size_t)(n + 31) / 32;
@@ -224,6 +223,23 @@ void StrMasks::bind(cb::PipeParams& p, const PipelineSpec& spec, const Batch& b,
         p.smask[j].bits = (const cb::u32*)m.bits->ptr;
         p.smask[j].n_entries = (cb::i32)n;
     }
+}
+
+// =================================================================================================
+// bitmaps
+// =================================================================================================
+DeviceBufP bytes_to_bitmap(const DeviceBufP& bytes, int64_t n, ExecContext* ctx) {
+    auto bits = std::make_shared<DeviceBuf>(bitmap_bytes(n));
+    launch_bytes_to_bitmap((const unsigned char*)bytes->ptr, n, (uint32_t*)bits->ptr, ctx->stream);
+    ctx->kernel_launches++;
+    return bits;
+}
+
+// n bytes (nonzero = set) as a host bitmap, 8 bytes of slack behind it
+static std::vector<uint8_t> pack_bits(const uint8_t* bytes, size_t n) {
+    std::vector<uint8_t> out((n + 7) / 8 + 8, 0);
+    for (size_t i = 0; i < n; i++) if (bytes[i]) out[i >> 3] |= (uint8_t)(1u << (i & 7));
+    return out;
 }
 
 // =================================================================================================
@@ -343,11 +359,7 @@ struct StreamSource : ExecNode {
         std::vector<int32_t> remap((size_t)d->length);
         bool identity = true;
         for (int64_t k = 0; k < d->length; k++) {
-            std::string v(chars + off[k], (size_t)(off[k + 1] - off[k]));
-            auto it = std::find(g.values.begin(), g.values.end(), v);
-            int32_t code;
-            if (it == g.values.end()) { code = (int32_t)g.values.size(); g.values.push_back(v); }
-            else code = (int32_t)(it - g.values.begin());
+            const int32_t code = g.intern(std::string(chars + off[k], (size_t)(off[k + 1] - off[k])));
             remap[(size_t)k] = code;
             if (code != k) identity = false;
         }
@@ -519,18 +531,9 @@ struct TableSource : ExecNode {
     bool next(Batch& out) override {
         if (done) return false;
         if (table->needs_packing && !packed) { // byte-per-row validity / booleans (received from an exchange) -> Arrow bitmaps, once
-            size_t n = (size_t)table->n_rows;
             for (auto& c : table->cols) {
-                if (c.valid_bytes && !c.validity) {
-                    c.validity = std::make_shared<DeviceBuf>((n + 31) / 32 * 4 + 8);
-                    launch_bytes_to_bitmap((const unsigned char*)c.valid_bytes->ptr, table->n_rows, (uint32_t*)c.validity->ptr, ctx->stream);
-                    ctx->kernel_launches++;
-                }
-                if (c.bool_bytes && !c.data) {
-                    c.data = std::make_shared<DeviceBuf>((n + 31) / 32 * 4 + 8);
-                    launch_bytes_to_bitmap((const unsigned char*)c.bool_bytes->ptr, table->n_rows, (uint32_t*)c.data->ptr, ctx->stream);
-                    ctx->kernel_launches++;
-                }
+                if (c.valid_bytes && !c.validity) c.validity = bytes_to_bitmap(c.valid_bytes, table->n_rows, ctx);
+                if (c.bool_bytes && !c.data) c.data = bytes_to_bitmap(c.bool_bytes, table->n_rows, ctx);
             }
             packed = true;
         }
@@ -548,7 +551,7 @@ struct TableSource : ExecNode {
                     v->owner = b;
                     b = v;
                 };
-                const int w = phys_bytes(c.is_dict && c.phys == Phys::I32 ? Phys::Dict32 : c.phys);
+                const int w = phys_bytes(c.phys);
                 if (w == 0) slice(c.data, 1, 8);
                 else slice(c.data, (size_t)w, 1);
                 slice(c.validity, 1, 8);
@@ -662,18 +665,17 @@ struct SelectNode : FusedBase {
         for (size_t i = 0; i < g.out_cols.size(); i++) {
             Column& c = out.cols[i];
             c.type = g.out_cols[i].type;
-            c.phys = c.type.id == TypeId::Bool ? Phys::I8 : phys_of(c.type);
+            c.phys = kernel_out_phys(c.type);
             if (c.type.is_string()) { // dictionary codes pass through; the dictionary is the source column's
                 const Column& src = in.cols.at((size_t)outputs[i]->index);
                 if (!src.is_dict) throw Unsupported("plain Utf8 columns through a fused filter/projection (dictionary-encoded strings only)");
-                c.phys = Phys::I32;
                 c.is_dict = true;
                 c.dict = src.dict;
             }
             c.data = std::make_shared<DeviceBuf>((size_t)in.n_rows * g.out_bytes[i]);
             p.out[i] = (cb::u8*)c.data->ptr;
             if (g.out_cols[i].nullable) {
-                c.validity = std::make_shared<DeviceBuf>((size_t)(in.n_rows + 31) / 32 * 4 + 8);
+                c.validity = std::make_shared<DeviceBuf>(bitmap_bytes(in.n_rows));
                 cuda_check(cudaMemsetAsync(c.validity->ptr, 0, c.validity->bytes, st), "memset out validity");
                 p.out_valid[i] = (cb::u32*)c.validity->ptr;
                 c.null_count = -1;
@@ -725,8 +727,7 @@ struct SelectNode : FusedBase {
 // =================================================================================================
 // The HK_* kind of a key column (device/cb_sortkey.h), for hash partitioning and the sort.  The logical type decides how Spark hashes
 // a value (utils.rs: i8 / i16 / i32 / date as i32, decimal(p <= 18) as i64, wider decimals as 16 bytes) and how many bits its sort key
-// takes; the physical layout decides how it is read.  The Parquet scan keeps INT32-backed int8 / int16 / decimal(p <= 9) columns 4 bytes
-// wide, decimals with p <= 18 8 bytes wide (device tables too), and aggregate outputs keep booleans one byte per row.
+// takes; the stored layout (DESIGN.md, "Data layout in HBM") decides how it is read.
 static int key_kind(const Column& c) {
     const Phys ph = c.phys;
     switch (c.type.id) {
@@ -756,19 +757,14 @@ static void columns_to_device(Batch& b, ExecContext* ctx) {
         if (c.type.is_string()) { // dictionary-encode on the host: these are group keys of a dense aggregate (a handful of rows)
             auto d = std::make_shared<Dictionary>();
             std::vector<int32_t> codes(n);
-            for (size_t r = 0; r < n; r++) {
-                std::string v((const char*)c.h_data.data() + c.h_offsets[r], (size_t)(c.h_offsets[r + 1] - c.h_offsets[r]));
-                auto it = std::find(d->values.begin(), d->values.end(), v);
-                if (it == d->values.end()) { codes[r] = (int32_t)d->values.size(); d->values.push_back(v); }
-                else codes[r] = (int32_t)(it - d->values.begin());
-            }
+            for (size_t r = 0; r < n; r++)
+                codes[r] = d->intern(std::string((const char*)c.h_data.data() + c.h_offsets[r], (size_t)(c.h_offsets[r + 1] - c.h_offsets[r])));
             c.data = std::make_shared<DeviceBuf>(n * 4 + 16);
             if (n) cuda_check(cudaMemcpyAsync(c.data->ptr, codes.data(), n * 4, cudaMemcpyHostToDevice, ctx->stream), "keys H2D");
             cuda_check(cudaStreamSynchronize(ctx->stream), "keys H2D sync");
             c.is_dict = true; c.dict = d; c.phys = Phys::I32;
         } else if (c.type.id == TypeId::Bool) {
-            std::vector<uint8_t> bits((n + 7) / 8 + 8, 0);
-            for (size_t r = 0; r < n; r++) if (c.h_data[r]) bits[r >> 3] |= (uint8_t)(1u << (r & 7));
+            std::vector<uint8_t> bits = pack_bits(c.h_data.data(), n);
             c.data = std::make_shared<DeviceBuf>(bits.size());
             cuda_check(cudaMemcpyAsync(c.data->ptr, bits.data(), bits.size(), cudaMemcpyHostToDevice, ctx->stream), "bool H2D");
             cuda_check(cudaStreamSynchronize(ctx->stream), "bool H2D sync");
@@ -780,8 +776,7 @@ static void columns_to_device(Batch& b, ExecContext* ctx) {
             c.phys = phys_of(c.type);
         }
         if (!c.h_valid.empty()) {
-            std::vector<uint8_t> bits((n + 7) / 8 + 8, 0);
-            for (size_t r = 0; r < n; r++) if (c.h_valid[r]) bits[r >> 3] |= (uint8_t)(1u << (r & 7));
+            std::vector<uint8_t> bits = pack_bits(c.h_valid.data(), n);
             c.validity = std::make_shared<DeviceBuf>(bits.size());
             cuda_check(cudaMemcpyAsync(c.validity->ptr, bits.data(), bits.size(), cudaMemcpyHostToDevice, ctx->stream), "validity H2D");
             cuda_check(cudaStreamSynchronize(ctx->stream), "validity H2D sync");
@@ -799,14 +794,13 @@ template <typename I> static void gather_columns(const Batch& in, const I* row_i
     for (auto& c : in.cols) {
         Column o = c;
         if (c.offsets) throw Unsupported(std::string(op) + " plain string columns (dictionary-encode them first)");
-        int w = phys_bytes(c.is_dict && c.phys == Phys::I32 ? Phys::Dict32 : c.phys);
+        int w = phys_bytes(c.phys);
         if (w == 0) { // bit-packed booleans: gather to bytes, repack
             auto bytes = std::make_shared<DeviceBuf>((size_t)n + 16);
             launch_gather_bits(c.data->ptr, row_idx, n, bytes->ptr, st);
-            o.data = std::make_shared<DeviceBuf>((size_t)(n + 31) / 32 * 4 + 8);
-            launch_bytes_to_bitmap((const unsigned char*)bytes->ptr, n, (uint32_t*)o.data->ptr, st);
+            ctx->kernel_launches++;
+            o.data = bytes_to_bitmap(bytes, n, ctx);
             o.bool_bytes = bytes;
-            ctx->kernel_launches += 2;
         } else {
             o.data = std::make_shared<DeviceBuf>((size_t)std::max<int64_t>(n, 1) * w);
             launch_gather(c.data->ptr, w, row_idx, n, o.data->ptr, st);
@@ -816,10 +810,9 @@ template <typename I> static void gather_columns(const Batch& in, const I* row_i
         if (c.validity) {
             auto bytes = std::make_shared<DeviceBuf>((size_t)n + 16);
             launch_gather_bits(c.validity->ptr, row_idx, n, bytes->ptr, st);
-            o.validity = std::make_shared<DeviceBuf>((size_t)(n + 31) / 32 * 4 + 8);
-            launch_bytes_to_bitmap((const unsigned char*)bytes->ptr, n, (uint32_t*)o.validity->ptr, st);
+            ctx->kernel_launches++;
+            o.validity = bytes_to_bitmap(bytes, n, ctx);
             o.valid_bytes = bytes;
-            ctx->kernel_launches += 2;
         }
         out.cols.push_back(o);
     }
@@ -854,7 +847,7 @@ struct PartitionNode : ExecNode {
             case HK_DICT8: case HK_DICT16: case HK_DICT32: {
                 std::vector<int32_t> off{0};
                 std::string chars;
-                for (auto& v : c.dict->values) { chars += v; off.push_back((int32_t)chars.size()); }
+                for (auto& v : c.dict->values()) { chars += v; off.push_back((int32_t)chars.size()); }
                 auto doff = std::make_shared<DeviceBuf>(off.size() * 4), dch = std::make_shared<DeviceBuf>(chars.size() + 16);
                 cuda_check(cudaMemcpyAsync(doff->ptr, off.data(), off.size() * 4, cudaMemcpyHostToDevice, st), "dict offsets");
                 if (!chars.empty()) cuda_check(cudaMemcpyAsync(dch->ptr, chars.data(), chars.size(), cudaMemcpyHostToDevice, st), "dict chars");
@@ -979,8 +972,8 @@ struct SortNode : ExecNode {
             }
             if (!same && !c0.is_dict) throw Unsupported("sort input whose batches store column " + std::to_string(j) + " in different layouts");
             if (same) {
-                const int w = phys_bytes(c0.is_dict && c0.phys == Phys::I32 ? Phys::Dict32 : c0.phys);
-                o.data = std::make_shared<DeviceBuf>(w == 0 ? (n + 31) / 32 * 4 + 8 : std::max<size_t>(n, 1) * (size_t)w);
+                const int w = phys_bytes(c0.phys);
+                o.data = std::make_shared<DeviceBuf>(w == 0 ? bitmap_bytes((int64_t)n) : std::max<size_t>(n, 1) * (size_t)w);
                 if (w == 0) cuda_check(cudaMemsetAsync(o.data->ptr, 0, o.data->bytes, st), "memset bools");
                 int64_t row = 0;
                 for (auto& b : bs) {
@@ -991,33 +984,26 @@ struct SortNode : ExecNode {
                 }
             } else { // dictionary codes -> int32 codes of one dictionary
                 auto d = std::make_shared<Dictionary>(*c0.dict);
-                std::unordered_map<std::string, int32_t> code_of;
-                for (size_t k = d->values.size(); k-- > 0;) code_of[d->values[k]] = (int32_t)k;
                 o.phys = Phys::I32;
                 o.dict = d;
                 o.data = std::make_shared<DeviceBuf>(std::max<size_t>(n, 1) * 4);
                 int64_t row = 0;
                 for (auto& b : bs) {
                     const Column& c = b.cols[j];
-                    std::vector<int32_t> table(c.dict->values.size());
-                    for (size_t k = 0; k < table.size(); k++) {
-                        if (c.dict == c0.dict) { table[k] = (int32_t)k; continue; }
-                        auto it = code_of.find(c.dict->values[k]);
-                        if (it == code_of.end()) { it = code_of.emplace(c.dict->values[k], (int32_t)d->values.size()).first; d->values.push_back(c.dict->values[k]); }
-                        table[k] = it->second;
-                    }
+                    const std::vector<std::string>& vals = c.dict->values();
+                    std::vector<int32_t> table(vals.size());
+                    for (size_t k = 0; k < table.size(); k++) table[k] = c.dict == c0.dict ? (int32_t)k : d->intern(vals[k]);
                     auto dt = std::make_shared<DeviceBuf>(table.size() * 4 + 4);
                     temps.push_back(dt);
                     if (!table.empty()) cuda_check(cudaMemcpyAsync(dt->ptr, table.data(), table.size() * 4, cudaMemcpyHostToDevice, st), "H2D remap table");
                     cuda_check(cudaStreamSynchronize(st), "remap table copy"); // table is a loop temporary
-                    const int w = c.phys == Phys::I8 ? 1 : c.phys == Phys::I16 ? 2 : 4;
-                    launch_remap_codes(c.data->ptr, w, b.n_rows, (const int*)dt->ptr, (int)table.size(), (int*)o.data->ptr + row, st);
+                    launch_remap_codes(c.data->ptr, phys_bytes(c.phys), b.n_rows, (const int*)dt->ptr, (int)table.size(), (int*)o.data->ptr + row, st);
                     ctx->kernel_launches++;
                     row += b.n_rows;
                 }
             }
             if (nulls) {
-                o.validity = std::make_shared<DeviceBuf>((n + 31) / 32 * 4 + 8);
+                o.validity = std::make_shared<DeviceBuf>(bitmap_bytes((int64_t)n));
                 cuda_check(cudaMemsetAsync(o.validity->ptr, 0, o.validity->bytes, st), "memset validity");
                 int64_t row = 0;
                 for (auto& b : bs) {
@@ -1038,8 +1024,8 @@ struct SortNode : ExecNode {
     // column carries another dictionary or its dictionary has grown.
     const uint32_t* rank_table(size_t key, const DictionaryP& d) {
         Rank& r = ranks[key];
-        if (r.table && r.dict == d.get() && r.n == d->values.size()) return (const uint32_t*)r.table->ptr;
-        const std::vector<std::string>& v = d->values;
+        const std::vector<std::string>& v = d->values();
+        if (r.table && r.dict == d.get() && r.n == v.size()) return (const uint32_t*)r.table->ptr;
         std::vector<uint32_t> order(v.size()), rank(v.size() + 1, 0);
         for (size_t i = 0; i < v.size(); i++) order[i] = (uint32_t)i;
         std::sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return v[a] < v[b]; }); // char_traits<char>: unsigned bytes
@@ -1100,7 +1086,7 @@ struct SortNode : ExecNode {
             f.validity = c.validity ? (const uint8_t*)c.validity->ptr : nullptr;
             if (c.is_dict) {
                 f.rank = rank_table(k, c.dict);
-                f.n_rank = (int)c.dict->values.size();
+                f.n_rank = (int)c.dict->values().size();
             }
             f.off = bits;
             bits += f.bits + f.has_null;
@@ -1338,11 +1324,6 @@ std::string arrow_format(const DType& t) {
     default: throw Unsupported("export of " + t.str());
     }
 }
-std::vector<uint8_t> pack_bits(const uint8_t* bytes, size_t n) {
-    std::vector<uint8_t> out((n + 7) / 8 + 8, 0);
-    for (size_t i = 0; i < n; i++) if (bytes[i]) out[i >> 3] |= (uint8_t)(1u << (i & 7));
-    return out;
-}
 } // namespace
 
 // bits [row0, row0 + n) of a device bitmap as a host bitmap that starts at bit 0 (Arrow export is zero-offset only, jni_api.rs:716-732)
@@ -1421,7 +1402,7 @@ void export_batch(Batch& b, ExecContext* ctx, ArrowArray* out_arrays, ArrowSchem
             }
         } else if (c.is_dict) {
             // dictionary-coded strings: fetch the codes (1, 2 or 4 bytes each, as the source delivered them), spell the strings out on the host
-            const size_t cw = c.phys == Phys::I8 ? 1 : c.phys == Phys::I16 ? 2 : 4;
+            const size_t cw = (size_t)phys_bytes(c.phys);
             std::vector<uint8_t> raw_codes(n * cw + 8);
             if (n) cuda_check(cudaMemcpyAsync(raw_codes.data(), (const uint8_t*)c.data->ptr + r0 * cw, n * cw, cudaMemcpyDeviceToHost, ctx->stream), "D2H key codes");
             cuda_check(cudaStreamSynchronize(ctx->stream), "D2H sync");
@@ -1435,7 +1416,7 @@ void export_batch(Batch& b, ExecContext* ctx, ArrowArray* out_arrays, ArrowSchem
             o[0] = 0;
             for (size_t r = 0; r < n; r++) {
                 bool valid = (vb[r >> 3] >> (r & 7)) & 1;
-                if (valid) { const std::string& sv = c.dict->values.at((size_t)codes[r]); data.insert(data.end(), sv.begin(), sv.end()); }
+                if (valid) { const std::string& sv = c.dict->values().at((size_t)codes[r]); data.insert(data.end(), sv.begin(), sv.end()); }
                 else null_count++;
                 o[r + 1] = (int32_t)data.size();
             }

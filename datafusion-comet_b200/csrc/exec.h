@@ -10,8 +10,10 @@
 #include "plan.h"
 
 #include <cuda_runtime.h>
+#include <climits>
 #include <memory>
 #include <string>
+#include <unordered_map>
 #include <vector>
 
 namespace cb200 {
@@ -52,11 +54,35 @@ struct DeviceBuf {
 };
 using DeviceBufP = std::shared_ptr<DeviceBuf>;
 
-struct Dictionary { // string dictionary of a key column (host copy; tiny)
-    std::vector<std::string> values;
+// The string dictionary of a dictionary-coded column (host copy): code i stands for values()[i].  Entries are only ever added, so a
+// code keeps its meaning as the dictionary grows.
+class Dictionary {
+  public:
+    const std::vector<std::string>& values() const { return values_; }
+    // the code of the first entry equal to v; v is appended when there is none
+    int32_t intern(std::string v) {
+        auto it = index_.find(v);
+        if (it != index_.end()) return it->second;
+        if (values_.size() >= (size_t)INT32_MAX) throw Unsupported("more than 2^31 distinct strings in one dictionary");
+        const int32_t code = (int32_t)values_.size();
+        index_.emplace(v, code);
+        values_.push_back(std::move(v));
+        return code;
+    }
+    // v as a new entry even if an equal one exists: a caller's dictionary may repeat a value, and each code keeps its own entry
+    void append(std::string v) {
+        index_.emplace(v, (int32_t)values_.size()); // no-op for a repeat: intern keeps finding the first
+        values_.push_back(std::move(v));
+    }
+
+  private:
+    std::vector<std::string> values_;
+    std::unordered_map<std::string, int32_t> index_; // value -> code of its first entry
 };
 using DictionaryP = std::shared_ptr<Dictionary>;
 
+// A device column.  Which layouts `phys` takes for each type, and which source produces each, is listed in DESIGN.md
+// ("Data layout in HBM"); phys_bytes(phys) is the width of one row of `data`, dictionary codes included.
 struct Column {
     DType type;
     Phys phys = Phys::I32;          // physical encoding of `data` (device) -- see codegen.h

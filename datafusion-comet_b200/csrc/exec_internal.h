@@ -27,6 +27,14 @@ inline Phys phys_of(const DType& t) {
     default: return Phys::I32;
     }
 }
+// the layout a generated kernel writes an output column of type t in: booleans one byte per row, strings as int32 dictionary codes
+inline Phys kernel_out_phys(const DType& t) { return t.id == TypeId::Bool ? Phys::I8 : t.is_string() ? Phys::I32 : phys_of(t); }
+
+// ---- bitmaps -------------------------------------------------------------------------------------------------------
+// bytes of a device bitmap of n rows: whole 32-bit words, plus 8 bytes of slack
+inline size_t bitmap_bytes(int64_t n) { return (size_t)(n + 31) / 32 * 4 + 8; }
+// a new device bitmap of n rows, bit r set where bytes[r] != 0 (one launch on ctx->stream, counted)
+DeviceBufP bytes_to_bitmap(const DeviceBufP& bytes, int64_t n, ExecContext* ctx);
 
 // ---- expression helpers --------------------------------------------------------------------------------------------
 inline ExprP clone_expr(const ExprP& e) {
@@ -58,7 +66,7 @@ inline void rewrite_bound(const ExprP& e, const std::map<int, int>& slot_of) {
 
 // ---- string predicate masks ----------------------------------------------------------------------------------------
 // A string predicate is decided once per dictionary entry: a device bitmask over the codes of its column, read by the pipeline kernel
-// (codegen.cpp emit_str_pred).  Dictionaries only grow and codes never change (Dictionary::values: a batch's dictionary is unified into
+// (codegen.cpp emit_str_pred).  Dictionaries only grow and codes never change (Dictionary: a batch's dictionary is unified into
 // the plan-wide one, the Parquet scan interns into one dictionary per column), so a mask is brought up to date before every launch
 // that reads it by evaluating only the entries added since the previous one.  A column that carries another Dictionary object starts
 // again from entry 0.
@@ -132,7 +140,7 @@ struct FusedBase : ExecNode {
         for (size_t i = 0; i < which.size(); i++) {
             const Column& c = b.cols[which[i]];
             if (!c.data) throw Unsupported("column " + std::to_string(which[i]) + " (" + c.type.str() + ") has no fixed-width device representation");
-            int w = phys_bytes(c.is_dict && c.phys == Phys::I32 ? Phys::Dict32 : c.phys);
+            int w = phys_bytes(c.phys);
             p.col[i] = (const cb::u8*)c.data->ptr + (w == 0 ? row0 / 8 : row0 * w);
             p.val[i] = c.validity ? (const cb::u8*)c.validity->ptr + row0 / 8 : nullptr;
         }

@@ -73,7 +73,8 @@ extern "C" const char* pi_plan(const uint8_t* plan, size_t len, long long chunk_
             o << "}";
         });
         const BatchPlan bp = plan_batches(sel.units, files, fields, chunk_rows);
-        std::vector<StringInterner> strings(fields.size());
+        std::vector<DictionaryP> dicts;
+        for (size_t c = 0; c < fields.size(); c++) dicts.push_back(std::make_shared<Dictionary>());
         o << ", \"chunk_need\": " << bp.chunk_need << ", \"batches\": [";
         for (size_t b = 0; b < bp.batches.size(); b++) {
             const std::vector<Unit> units = batch_units(sel.units, bp.batches[b]);
@@ -87,7 +88,7 @@ extern "C" const char* pi_plan(const uint8_t* plan, size_t len, long long chunk_
             for (size_t c = 0; c < fields.size(); c++) {
                 // device addresses are only recorded; host addresses point into the file images
                 const std::vector<ChunkLoc> loc = locate_chunks(up, c, [&](const UploadRange& r) { return images[r.file].data() + r.start; }, (unsigned char*)(uintptr_t)4096);
-                ColPlan cp = plan_column(files, fields[c], c, units, total, loc, strings[c]);
+                ColPlan cp = plan_column(files, fields[c], c, units, total, loc, dicts[c]);
                 o << (c ? ", " : "") << "{\"covered\": " << cp.covered << ", \"null_aware\": " << (cp.null_aware ? 1 : 0) << ", \"segs\": ";
                 segs_json(o, cp.segs);
                 o << ", \"pages\": ";

@@ -164,7 +164,7 @@ struct NativeScanSource : ExecNode {
     BatchPlan plan;
     size_t next_batch = 0;
     bool opened = false;
-    std::vector<StringInterner> strings;    // per column
+    std::vector<DictionaryP> dicts;         // per column: the plan-wide dictionary of a string column
 
     struct Slot {
         ScanBlockP chunk, work, meta, staging;
@@ -214,7 +214,7 @@ struct NativeScanSource : ExecNode {
         Selection sel = select_row_groups(open_files, file_start, file_length, fields.size(), terms);
         all_units = std::move(sel.units);
         const PageSelection ps = select_pages(all_units, open_files, fields.size(), terms);
-        strings.resize(fields.size());
+        for (size_t c = 0; c < fields.size(); c++) dicts.push_back(std::make_shared<Dictionary>());
         plan = plan_batches(all_units, open_files, fields, ctx->chunk_rows);
         if (trace_on()) fprintf(stderr, "[cb200 trace]   parquet scan: %zu row groups in %zu batches (%lld pruned by statistics, %lld data pages by the page index), chunk block %.1f MB, work block %.1f MB per slot\n",
                                 all_units.size(), plan.batches.size(), (long long)sel.pruned_row_groups, (long long)ps.pruned_pages, plan.chunk_need / 1e6, plan.work_estimate / 1e6);
@@ -273,7 +273,7 @@ struct NativeScanSource : ExecNode {
         // phase A: page tables on the host (reads only page headers)
         tt = now_ms();
         std::vector<ColPlan> plans;
-        for (size_t c = 0; c < fields.size(); c++) plans.push_back(plan_column(open_files, fields[c], c, units, total, loc[c], strings[c]));
+        for (size_t c = 0; c < fields.size(); c++) plans.push_back(plan_column(open_files, fields[c], c, units, total, loc[c], dicts[c]));
         bind_buffers(plans, total, sl);
         const double t_pages = now_ms() - tt;
         // phase B: decode kernels

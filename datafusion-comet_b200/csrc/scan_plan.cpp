@@ -385,16 +385,6 @@ UploadPlan plan_uploads(const std::vector<Unit>& units, const std::vector<ScanFi
 }
 
 // ---- columns --------------------------------------------------------------------------------------------------------
-int32_t StringInterner::code(std::string v) {
-    auto it = index.find(v);
-    if (it != index.end()) return it->second;
-    if (dict->values.size() >= (size_t)INT32_MAX) throw Unsupported("parquet: more than 2^31 distinct strings in one column");
-    const int32_t c = (int32_t)dict->values.size();
-    dict->values.push_back(v);
-    index.emplace(std::move(v), c);
-    return c;
-}
-
 static void check_annotations(const pq::SchemaElement& se, const DType& t) {
     // SchemaElement.converted_type / logicalType decide what the physical bytes MEAN; a mismatch must not be read silently
     const int ct = se.converted_type;
@@ -527,7 +517,7 @@ void set_body_offset(PqPage& d, size_t off) { d.body = (unsigned char*)(uintptr_
 // the page tables of one column over the chunks of a batch
 class ColumnPlanner {
   public:
-    ColumnPlanner(const pq::SchemaElement& se, const StructField& field, size_t c, StringInterner& strings, ColPlan& cp)
+    ColumnPlanner(const pq::SchemaElement& se, const StructField& field, size_t c, Dictionary& strings, ColPlan& cp)
         : se(se), field(field), c(c), strings(strings), cp(cp) {}
 
     void chunk(const ScanFile& f, const Unit& unit, const ChunkLoc& at) {
@@ -599,7 +589,7 @@ class ColumnPlanner {
     const pq::SchemaElement& se;
     const StructField& field;
     const size_t c;
-    StringInterner& strings;
+    Dictionary& strings; // the column's plan-wide dictionary (string columns)
     ColPlan& cp;
     std::vector<PqPage> dict_pages; // fixed-width dictionary pages (decoded into the combined dictionary)
     std::vector<uint8_t> scratch;
@@ -680,7 +670,7 @@ class ColumnPlanner {
         cp.hostdec.insert(cp.hostdec.end(), b.first, b.first + pre);
         if (se.type == pq::BYTE_ARRAY) {
             for_each_byte_array(encoding, b.first + pre, b.first + b.second, d.num_values, [&](std::string v) {
-                const int32_t code = strings.code(std::move(v));
+                const int32_t code = strings.intern(std::move(v));
                 const uint8_t* code_bytes = (const uint8_t*)&code;
                 cp.hostdec.insert(cp.hostdec.end(), code_bytes, code_bytes + 4);
             });
@@ -700,7 +690,7 @@ class ColumnPlanner {
         if (se.type == pq::BYTE_ARRAY) { // strings: unified with the plan-wide dictionary on the host; the device gets the code remap table
             const auto b = host_section(s, "dictionary page");
             ByteArrays vals{b.first, b.first + b.second, "parquet: truncated dictionary page"};
-            for (int k = 0; k < dict_size; k++) cp.remap.push_back(strings.code(vals.next()));
+            for (int k = 0; k < dict_size; k++) cp.remap.push_back(strings.intern(vals.next()));
         } else {
             PqPage dp{};
             place_body(dp, s);
@@ -767,13 +757,13 @@ class ColumnPlanner {
 } // namespace
 
 ColPlan plan_column(const std::vector<ScanFile>& files, const StructField& field, size_t c, const std::vector<Unit>& units, int64_t total,
-                    const std::vector<ChunkLoc>& loc, StringInterner& strings) {
+                    const std::vector<ChunkLoc>& loc, const DictionaryP& dict) {
     ColPlan cp;
     const pq::SchemaElement& se = files[units[0].file].leaf(c);
     column_type(se, field.type, cp);
     check_annotations(se, field.type);
-    if (se.type == pq::BYTE_ARRAY) cp.dict = strings.dict;
-    ColumnPlanner p(se, field, c, strings, cp);
+    if (se.type == pq::BYTE_ARRAY) cp.dict = dict;
+    ColumnPlanner p(se, field, c, *dict, cp);
     for (size_t u = 0; u < units.size(); u++) p.chunk(files[units[u].file], units[u], loc[u]);
     p.finish(total);
     return cp;

@@ -7,7 +7,6 @@
 #include "parquet_pages.h"
 
 #include <memory>
-#include <unordered_map>
 #include <utility>
 
 namespace cb200 {
@@ -111,14 +110,6 @@ struct UploadPlan {
 UploadPlan plan_uploads(const std::vector<Unit>& units, const std::vector<ScanFile>& files, size_t n_cols);
 
 // ---- columns -------------------------------------------------------------------------------------------------------------------
-// The plan-wide dictionary of one string column.  Dictionary pages and PLAIN pages both intern through it, so a value gets the same
-// code whichever encoding, file or batch it comes from; codes are handed out in first-occurrence order.
-struct StringInterner {
-    DictionaryP dict = std::make_shared<Dictionary>();
-    std::unordered_map<std::string, int32_t> index; // value -> code, in step with dict->values
-    int32_t code(std::string v);
-};
-
 // one column chunk of a batch: its bytes on the host and where they land on the device; for a page-pruned unit, those of each piece
 struct PieceLoc { int64_t start, end; const uint8_t* host; unsigned char* dev; };
 struct ChunkLoc {
@@ -165,8 +156,10 @@ struct ColPlan {
     size_t out_bytes = 0, validity_bytes = 0;
 };
 
+// `dict`: the plan-wide dictionary of a string column.  Dictionary pages and PLAIN pages both intern into it, so a value gets the same
+// code whichever encoding, file or batch it comes from.
 ColPlan plan_column(const std::vector<ScanFile>& files, const StructField& field, size_t c, const std::vector<Unit>& units, int64_t total,
-                    const std::vector<ChunkLoc>& loc, StringInterner& strings);
+                    const std::vector<ChunkLoc>& loc, const DictionaryP& dict);
 // every device buffer of a column, as (where the pointer goes, bytes)
 void buffer_requests(ColPlan& cp, int64_t total, std::vector<std::pair<uint8_t**, size_t>>& reqs);
 // Page bodies whose buffer has no device address at plan time hold an offset into it; this turns them into addresses, once `cp.dunc`

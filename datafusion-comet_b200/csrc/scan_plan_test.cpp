@@ -73,7 +73,8 @@ extern "C" const char* sp_plan(const uint8_t* plan, size_t len, long long chunk_
         for (auto& f : op->data_filters) collect_prune_terms(f, terms);
         const Selection sel = select_row_groups(files, op->file_start, op->file_length, fields.size(), terms);
         const BatchPlan bp = plan_batches(sel.units, files, fields, chunk_rows);
-        std::vector<StringInterner> strings(fields.size());
+        std::vector<DictionaryP> dicts;
+        for (size_t c = 0; c < fields.size(); c++) dicts.push_back(std::make_shared<Dictionary>());
         o << "{\"pruned_row_groups\": " << sel.pruned_row_groups << ", \"pruned_rows\": " << sel.pruned_rows << ", \"batches\": [";
         for (size_t b = 0; b < bp.batches.size(); b++) {
             const std::vector<Unit> units = batch_units(sel.units, bp.batches[b]);
@@ -88,16 +89,17 @@ extern "C" const char* sp_plan(const uint8_t* plan, size_t len, long long chunk_
                     const UploadRange& r = up.ranges[at.range];
                     loc.push_back({images[r.file].data() + r.start + at.off, (unsigned char*)(uintptr_t)(4096 + r.dev_off + at.off)}); // device addresses are only recorded
                 }
-                ColPlan cp = plan_column(files, fields[c], c, units, total, loc, strings[c]);
+                ColPlan cp = plan_column(files, fields[c], c, units, total, loc, dicts[c]);
                 o << (c ? ", " : "");
                 column_json(o, cp);
             }
             o << "]}";
         }
         o << "], \"dictionaries\": [";
-        for (size_t c = 0; c < strings.size(); c++) {
+        for (size_t c = 0; c < dicts.size(); c++) {
             o << (c ? ", " : "") << "[";
-            for (size_t k = 0; k < strings[c].dict->values.size(); k++) o << (k ? ", " : "") << "\"" << hex(strings[c].dict->values[k]) << "\"";
+            const std::vector<std::string>& vals = dicts[c]->values();
+            for (size_t k = 0; k < vals.size(); k++) o << (k ? ", " : "") << "\"" << hex(vals[k]) << "\"";
             o << "]";
         }
         o << "]}";
