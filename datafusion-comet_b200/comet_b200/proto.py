@@ -298,8 +298,14 @@ def filter_(child, predicate, plan_id=0):  # operator.proto:637
     return _op("filter", f_len(1, predicate), (child,), plan_id)
 
 
-def hash_agg(child, grouping, aggs, mode=PARTIAL, plan_id=0):  # operator.proto:647
+def hash_agg(child, grouping, aggs, mode=PARTIAL, plan_id=0, expr_modes=None, initial_input_buffer_offset=None):  # operator.proto:647
+    """expr_modes: one AggregateMode per aggregate (the distinct rewrite's mixed Partial / PartialMerge operator); None = all use
+    `mode`.  initial_input_buffer_offset: child column of the first state column the merging aggregates read."""
     body = b"".join(f_len(1, g) for g in grouping) + b"".join(f_len(2, a) for a in aggs) + f_varint(5, mode)
+    if expr_modes is not None:
+        body += f_len(6, b"".join(_varint(int(m)) for m in expr_modes))  # packed repeated enum
+    if initial_input_buffer_offset is not None:
+        body += f_varint(7, initial_input_buffer_offset)
     return _op("hash_agg", body, (child,), plan_id)
 
 

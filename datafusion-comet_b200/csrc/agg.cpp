@@ -362,9 +362,12 @@ struct StreamState {
 
 struct AggNode : FusedBase {
     std::vector<ExprP> keys;          // over child columns; each must be a plain column reference
-    std::vector<AggExpr> aggs;        // children/filter over child columns (Partial)
-    std::vector<std::vector<int>> state_cols; // Final: child column index of each state column
-    AggMode mode = AggMode::Partial;
+    std::vector<AggExpr> aggs;        // children/filter over child columns (Partial-mode aggregates)
+    std::vector<std::vector<int>> state_cols; // per aggregate: child column index of each state column it merges (empty: Partial)
+    AggMode mode = AggMode::Partial;  // the operator's; each aggregate has its own (AggExpr::mode)
+    bool reads_rows = true;           // some input column is read as a row value (a Partial operator, or a Partial-mode aggregate)
+    bool all_partial = true;          // every aggregate updates from rows: the input may be clustered (stream strategy)
+    std::vector<bool> is_state_col;   // per child column: a merging aggregate reads it as state
     bool ungrouped = false;
     bool emitted = false;
     std::vector<Batch> outq;          // output batches (more than one only after a dense -> hash migration)
@@ -398,7 +401,8 @@ struct AggNode : FusedBase {
 
     int assume_for(int child_col, Level lv) const {
         const DType& t = child->schema[(size_t)child_col];
-        if (!t.is_decimal() || lv == SAFE || mode != AggMode::Partial) return 0;
+        // state columns carry no range a kernel may assume: only the values Partial-mode aggregates, keys and predicates read
+        if (!t.is_decimal() || lv == SAFE || !reads_rows || is_state_col[(size_t)child_col]) return 0;
         int k = r_bitlen(r_prec_max(t.precision));
         if ((size_t)child_col < assume_bits.size() && assume_bits[(size_t)child_col] > 0) k = std::min(k, assume_bits[(size_t)child_col]);
         if (lv == TIGHT && !observed_bits.empty() && observed_bits[(size_t)child_col] >= 0) k = std::min(k, observed_bits[(size_t)child_col] + 2);
@@ -419,7 +423,7 @@ struct AggNode : FusedBase {
         for (size_t k = 0; k < keys.size(); k++) s.key_nullable.push_back(b ? key_has_null[k] : false);
         for (auto& a : aggs) {
             AggExpr c = a;
-            if (mode == AggMode::Partial) {
+            if (a.mode == AggMode::Partial) {
                 c.children = to_slots(a.children, slot_of);
                 if (a.filter) c.filter = to_slots({a.filter}, slot_of)[0];
             }
@@ -457,7 +461,7 @@ struct AggNode : FusedBase {
         bool hash = false;
         for (auto& k : keys) if (!k->type.is_string() && k->type.id != TypeId::Bool) hash = true;
         std::vector<PipelineSpec> out{make_spec(nullptr, hash ? Strategy::Table : Strategy::Dense, ungrouped ? 1 : 6)};
-        if (hash && mode == AggMode::Partial) out.push_back(make_spec(nullptr, Strategy::Stream, 6));
+        if (hash && mode == AggMode::Partial && all_partial) out.push_back(make_spec(nullptr, Strategy::Stream, 6));
         return out;
     }
 
@@ -601,7 +605,7 @@ struct AggNode : FusedBase {
         const int64_t SAMPLE = 1 << 20;
         bool have_obs = false;
         for (int ci : used_cols) if (child->schema[(size_t)ci].is_decimal() && observed_bits[(size_t)ci] >= 0) have_obs = true;
-        if (mode == AggMode::Partial && !have_obs && b.n_rows > 2 * SAMPLE) {
+        if (reads_rows && !have_obs && b.n_rows > 2 * SAMPLE) {
             // Range profile of the last plan with this very pipeline (the previous task of the same stage reads the same table):
             // start at its ranges instead of sampling again.  A profile is only a guess -- every launch validates it.
             profile_key = pipeline_signature(make_spec(&b, Strategy::Dense, n_groups, SAFE));
@@ -612,7 +616,7 @@ struct AggNode : FusedBase {
                 for (int ci : used_cols) if (child->schema[(size_t)ci].is_decimal() && observed_bits[(size_t)ci] >= 0) have_obs = true;
             }
         }
-        if (mode != AggMode::Partial) {
+        if (!reads_rows) {
             run_range(b, 0, b.n_rows, n_groups, SAFE);
         } else if (!have_obs && b.n_rows > 2 * SAMPLE) {
             // sample-then-specialise: a short launch measures the value ranges, the bulk launch runs the kernel
@@ -747,7 +751,7 @@ struct AggNode : FusedBase {
         const Kernel k = compile(make_spec(&b, Strategy::Table, 2, SAFE));
         {
             TraceSpan ts("hash.ensure_table");
-            table.ensure(ctx, k, rows, b.n_rows, child->rows_hint(), rows_scanned, mode != AggMode::Partial);
+            table.ensure(ctx, k, rows, b.n_rows, child->rows_hint(), rows_scanned, mode != AggMode::Partial || !all_partial);
         }
         launch_id_rows(b, 0, b.n_rows, k, true);
         ctx->pipeline_rows += b.n_rows;
@@ -778,7 +782,8 @@ struct AggNode : FusedBase {
     // On entering hash aggregation: are equal keys adjacent?  Run the stream kernel over the first rows of the first batch and look at
     // state rows per input row.  True: the stream strategy; false: the key table (whatever the sample allocated is dropped).
     bool sample_stream(Batch& b) {
-        if (mode != AggMode::Partial || ctx->stream_agg_min_rows < 0) return false;
+        // a merging aggregate's input is a hash-partitioned state batch, not clustered on the keys
+        if (mode != AggMode::Partial || !all_partial || ctx->stream_agg_min_rows < 0) return false;
         if (b.n_rows + std::max<int64_t>(child->rows_hint(), 0) < ctx->stream_agg_min_rows || b.n_rows == 0) return false;
         const Kernel k = compile(make_spec(&b, Strategy::Stream, 2, SAFE));
         const int64_t sample = std::min<int64_t>(b.n_rows, 1 << 20);
@@ -836,7 +841,7 @@ struct AggNode : FusedBase {
         for (size_t c = 0; c < bounds.size(); c++)
             if (child->schema[c].is_decimal() && !observed_bits.empty())
                 bounds[c] = observed_bits[c] < 0 ? 0 : (observed_bits[c] >= 127 ? RSAT : (u128r)1 << observed_bits[c]);
-        if (mode == AggMode::Partial) return expr_maxabs(*a.children[0], bounds);
+        if (a.mode == AggMode::Partial) return expr_maxabs(*a.children[0], bounds);
         return bounds[(size_t)state_cols[ai][0]];
     }
     // finalize parameters with every aggregate's certificate
@@ -849,7 +854,7 @@ struct AggNode : FusedBase {
             fp.cert_b[ai][0] = b >= RSAT ? ~0ull : (uint64_t)b;
             fp.cert_b[ai][1] = b >= RSAT ? ~0ull : (uint64_t)(b >> 64);
             // bit 63 of the high word (free: B < 2^127): B is the bound 2^bits of a value mask, i.e. addends lie in [-B, B - 1]
-            const bool direct = mode != AggMode::Partial || aggs[ai].children[0]->kind == ExprKind::Bound;
+            const bool direct = aggs[ai].mode != AggMode::Partial || aggs[ai].children[0]->kind == ExprKind::Bound;
             if (b < RSAT && b != 0 && direct) fp.cert_b[ai][1] |= 1ull << 63;
         }
         return fp;
@@ -911,22 +916,27 @@ ExecNodeP make_agg_node(const OperatorP& agg_op, const ExecNodeP& src, const std
         n->keys.push_back(k);
         roots.push_back(k);
     }
-    size_t state_at = agg_op->grouping.size();
+    n->is_state_col.assign(src->schema.size(), false);
+    n->reads_rows = agg_op->mode == AggMode::Partial;
     for (auto& a : agg_op->aggs) {
         AggExpr c = a;
-        if (agg_op->mode == AggMode::Partial) {
+        std::vector<int> sc;
+        if (a.mode == AggMode::Partial) {
+            n->reads_rows = true;
             for (auto& ch : c.children) { ch = substitute(ch, cols); roots.push_back(ch); }
             if (c.filter) { c.filter = substitute(c.filter, cols); roots.push_back(c.filter); }
         } else {
-            std::vector<int> sc;
+            n->all_partial = false;
+            // the planner placed this aggregate's state columns (plan.cpp: initial_input_buffer_offset, merging aggregates only)
             for (size_t k = 0; k < agg_state_types(a).size(); k++) {
-                ExprP e = cols.at(state_at++);
+                ExprP e = cols.at((size_t)a.state_at + k);
                 if (e->kind != ExprKind::Bound) throw Unsupported("final aggregate over computed state columns");
                 sc.push_back(e->index);
+                n->is_state_col[(size_t)e->index] = true;
                 roots.push_back(e);
             }
-            n->state_cols.push_back(sc);
         }
+        n->state_cols.push_back(sc);
         n->aggs.push_back(c);
     }
     n->assign_slots(roots);

@@ -771,7 +771,7 @@ std::string spec_signature(const PipelineSpec& s) {
     for (size_t i = 0; i < s.keys.size(); i++) { sig_expr(o, *s.keys[i]); o << (i < s.key_nullable.size() && s.key_nullable[i]) << ';'; }
     o << ";A";
     for (auto& a : s.aggs) {
-        o << (int)a.kind << ':' << a.datatype.str() << ':' << a.sum_datatype.str() << ':' << (int)a.eval_mode << '[';
+        o << (int)a.kind << ':' << (int)a.mode << ':' << a.datatype.str() << ':' << a.sum_datatype.str() << ':' << (int)a.eval_mode << '[';
         for (auto& c : a.children) { sig_expr(o, *c); o << ','; }
         o << "]F";
         if (a.filter) sig_expr(o, *a.filter);
@@ -809,8 +809,8 @@ std::vector<ExprP> str_preds_of(const PipelineSpec& spec) {
     for (auto& e : spec.predicates) walk(e);
     for (auto& e : spec.outputs) walk(e);
     for (auto& e : spec.keys) walk(e);
-    if (spec.mode == AggMode::Partial)
-        for (auto& a : spec.aggs) {
+    for (auto& a : spec.aggs)
+        if (a.mode == AggMode::Partial) {
             for (auto& c : a.children) walk(c);
             walk(a.filter);
         }
@@ -1048,7 +1048,7 @@ GeneratedKernel generate_pipeline_uncached(const PipelineSpec& spec) {
         for (size_t ai = 0; ai < spec.aggs.size(); ai++) {
             const AggExpr& a = spec.aggs[ai];
             AggLayout& L = layout[ai];
-            if (spec.mode == AggMode::Partial) {
+            if (a.mode == AggMode::Partial) {
                 // per-aggregate FILTER clause: NULL/FALSE excludes the row (sum_decimal.rs:452-458)
                 std::string cond = "true";
                 if (a.filter) {
@@ -1125,7 +1125,7 @@ GeneratedKernel generate_pipeline_uncached(const PipelineSpec& spec) {
                 }
                 }
             } else {
-                // ---- Final: merge state columns (merge_batch semantics) ----
+                // ---- Final / PartialMerge: merge state columns (merge_batch semantics) ----
                 const std::vector<int>& sc = spec.state_slots.at(ai);
                 auto col = [&](int i) { Expr b; b.kind = ExprKind::Bound; b.index = sc[i]; b.type = spec.cols[sc[i]].type; return em.emit(b); };
                 std::string tag = "agg" + std::to_string(ai);
@@ -1250,7 +1250,7 @@ GeneratedKernel generate_pipeline_uncached(const PipelineSpec& spec) {
         for (size_t ai = 0; ai < spec.aggs.size(); ai++) {
             const AggExpr& a = spec.aggs[ai];
             const AggLayout& L = layout[ai];
-            bool partial = spec.mode != AggMode::Final; // Partial and PartialMerge emit state columns
+            bool partial = a.mode != AggMode::Final; // Partial and PartialMerge emit state columns
             std::string A = "a" + std::to_string(ai);
             fin << "    { // aggregate " << ai << "\n";
             switch (a.kind) {
@@ -1316,7 +1316,7 @@ GeneratedKernel generate_pipeline_uncached(const PipelineSpec& spec) {
                     fin << "      cb::i128 s = " << T128(L.w_sum) << "; cb::i64 n = " << T64(L.w_cnt) << ";\n";
                     fin << "      bool bad = " << (L.w_bad >= 0 ? T64(L.w_bad) + " > 0" : "false") << ";\n";
                     // addends: input rows (Partial) / merged state rows (Final, PartialMerge: `n` is the merged COUNT there)
-                    fin << "      int cert = cb::sum_cert(cb::cert_level(" << (spec.mode == AggMode::Partial ? "n" : "(cb::i64)T[CB_W_ROWS * 2]") << ", fp.cert_b[" << ai
+                    fin << "      int cert = cb::sum_cert(cb::cert_level(" << (a.mode == AggMode::Partial ? "n" : "(cb::i64)T[CB_W_ROWS * 2]") << ", fp.cert_b[" << ai
                         << "][0], fp.cert_b[" << ai << "][1], " << sp << "), cb::dec_fits_p(s, " << sp << "));\n";
                     fin << "      if (n > 0 && !bad && cert == 2) cb::set_err_raw(fp.err, 2);\n";
                     fin << "      bool notnull = !bad && !(n > 0 && cert != 0);\n";
@@ -1358,11 +1358,14 @@ GeneratedKernel generate_pipeline_uncached(const PipelineSpec& spec) {
             fin << "    }\n";
         }
 
+        // claim-first probing when the input rows are state rows: a Final / PartialMerge operator, or one with a merging aggregate
+        bool merges_state = spec.mode != AggMode::Partial;
+        for (auto& a : spec.aggs) if (a.mode != AggMode::Partial) merges_state = true;
         std::ostringstream defs;
         g.ungrouped = spec.ungrouped;
         defs << "#define CB_KERNEL_AGG 1\n#define CB_WORDS " << g.n_words << "\n#define CB_G1 " << (spec.ungrouped ? 1 : 0) << "\n#define CB_W_ROWS " << w_rows
              << "\n#define CB_HASH " << (spec.hash ? 1 : 0) << "\n#define CB_KEY_WORDS " << (spec.hash ? g.key_words : 1) << "\n#define CB_STREAM " << (spec.hash && spec.stream ? 1 : 0)
-             << "\n#define CB_CAS_FIRST " << (spec.hash && spec.mode != AggMode::Partial ? 1 : 0) << "\n";
+             << "\n#define CB_CAS_FIRST " << (spec.hash && merges_state ? 1 : 0) << "\n";
         tu << header(spec, defs.str());
         tu << "constexpr __host__ __device__ int cb_word_kind(int w) { return ";
         for (size_t i = 0; i < slots.kinds.size(); i++) tu << "w == " << i << " ? " << slots.kinds[i] << " : ";

@@ -44,9 +44,9 @@ struct PipelineSpec {
     // Agg
     std::vector<ExprP> keys;              // each must be Bound to a Dict32 / Bitmap staged column (dense path)
     std::vector<bool> key_nullable;
-    std::vector<AggExpr> aggs;            // children/filter are exprs over staged cols (Partial) or state col slots (Final)
-    std::vector<std::vector<int>> state_slots; // Final mode: staged-col slot of each state column per agg
-    AggMode mode = AggMode::Partial;
+    std::vector<AggExpr> aggs;            // each by its own AggExpr::mode: children/filter over staged cols (Partial), or state_slots
+    std::vector<std::vector<int>> state_slots; // per agg: staged-col slot of each of its state columns (empty for a Partial agg)
+    AggMode mode = AggMode::Partial;      // the operator's mode; with no aggregates (keys only) it alone says whether rows are state rows
     bool ungrouped = false;
     bool hash = false;                    // high-cardinality: global open-addressing table keyed by the packed key columns
     bool masked = false;                  // Select sink: the keep decision comes from pass 1's bit mask (PipeParams::sel_mask), not from `predicates`
@@ -77,7 +77,7 @@ struct GeneratedKernel {
 GeneratedKernel generate_pipeline(const PipelineSpec& spec);
 
 // The distinct string predicates (ExprKind::StrPred) of a pipeline in mask-slot order: PipeParams::smask[i] holds the mask of entry i.
-// Order: predicates, outputs, group keys, then the arguments and FILTER clauses of Partial aggregates, each depth first.  Throws
+// Order: predicates, outputs, group keys, then the arguments and FILTER clauses of Partial-mode aggregates, each depth first.  Throws
 // Unsupported above CB_MAX_STR_PREDS.
 std::vector<ExprP> str_preds_of(const PipelineSpec& spec);
 // what one StrPred computes per dictionary entry: operation and literals.  Two nodes with equal keys over the same column share a mask.

@@ -673,6 +673,7 @@ static OperatorP decode_operator(PbReader r) { // Operator operator.proto:32-86
     case 104: { // HashAggregate operator.proto:647
         op->kind = OpKind::HashAgg;
         std::vector<int64_t> expr_modes;
+        int64_t buffer_offset = 0; // initial_input_buffer_offset
         while (b.next()) {
             if (b.field == 1) op->grouping.push_back(decode_expr(b.sub()));
             else if (b.field == 2) op->aggs.push_back(decode_agg(b.sub()));
@@ -680,31 +681,47 @@ static OperatorP decode_operator(PbReader r) { // Operator operator.proto:32-86
             else if (b.field == 6) {
                 if (b.wire == 2) { PbReader pk = b.sub(); while (pk.p < pk.end) expr_modes.push_back((int64_t)pk.varint()); }
                 else expr_modes.push_back(b.i64());
-            } else b.skip();
+            } else if (b.field == 7) buffer_offset = (int32_t)b.i64();
+            else b.skip();
         }
-        // Operator-level PartialMerge (merge state columns, emit state columns) is the Final input path with the Partial
-        // output path.  Per-expression modes that DIFFER from the operator's (the distinct rewrite: MergeAsPartialUDF,
-        // merge_as_partial.rs:54-110) are not fused.
-        for (int64_t m : expr_modes)
-            if (m != (int64_t)op->mode) throw Unsupported("aggregate expressions whose mode differs from the operator's (distinct rewrite, merge_as_partial.rs) are outside the GPU hot path");
+        if (op->mode != AggMode::Partial && op->mode != AggMode::Final && op->mode != AggMode::PartialMerge)
+            throw PlanError("unknown aggregate mode " + std::to_string((int)op->mode));
+        // Per-expression modes (the distinct rewrite, AggUtils.planAggregateWithOneDistinct): the JVM side sends them for an operator
+        // whose aggregates are {Partial, PartialMerge} (operators.scala:1740-1822).  A PartialMerge aggregate there merges state
+        // and emits state (MergeAsPartialUDF, merge_as_partial.rs:54-110); the output is state columns either way.
+        if (!expr_modes.empty() && expr_modes.size() != op->aggs.size())
+            throw PlanError("expr_modes has " + std::to_string(expr_modes.size()) + " entries for " + std::to_string(op->aggs.size()) + " aggregates");
+        bool mixed = false;
+        for (size_t i = 0; i < expr_modes.size(); i++) {
+            const int64_t m = expr_modes[i];
+            if (m != (int64_t)AggMode::Partial && m != (int64_t)AggMode::Final && m != (int64_t)AggMode::PartialMerge)
+                throw PlanError("unknown aggregate mode " + std::to_string(m));
+            if ((m == (int64_t)AggMode::Final) != (op->mode == AggMode::Final))
+                throw Unsupported("Final mixed with Partial / PartialMerge aggregate expressions is outside the GPU hot path");
+            op->aggs[i].mode = (AggMode)m;
+            if (m != (int64_t)op->mode) mixed = true;
+        }
+        if (expr_modes.empty()) for (auto& a : op->aggs) a.mode = op->mode;
         const auto& cs = child_schema();
         for (auto& g : op->grouping) { resolve(*g, cs); op->schema.push_back(g->type); }
         for (auto& a : op->aggs) {
-            resolve_agg(a, cs, op->mode);
-            if (op->mode != AggMode::Final) for (auto& t : agg_state_types(a)) op->schema.push_back(t);
+            resolve_agg(a, cs, a.mode); // Partial aggregates of a mixed operator may read any child column, state columns included
+            if (a.mode != AggMode::Final) for (auto& t : agg_state_types(a)) op->schema.push_back(t);
             else op->schema.push_back(agg_result_type(a));
         }
-        if (op->mode != AggMode::Partial) {
-            // DataFusion Final mode reads state columns positionally after the group columns
-            size_t need = op->grouping.size();
-            for (auto& a : op->aggs) need += agg_state_types(a).size();
-            if (cs.size() < need) throw PlanError("final / partial-merge aggregate: child has fewer columns than group + state columns");
-            size_t at = op->grouping.size();
-            for (auto& a : op->aggs)
-                for (auto& t : agg_state_types(a)) {
-                    if (cs[at] != t) throw PlanError("final aggregate: state column " + std::to_string(at) + " is " + cs[at].str() + ", expected " + t.str());
-                    at++;
-                }
+        // State columns of the merging aggregates: consecutive, in agg_exprs order, from initial_input_buffer_offset; the running offset
+        // advances over merging aggregates only (planner.rs:1265-1352).  A Final operator reads them right after its group columns, as
+        // does a PartialMerge one that sends no offset.
+        size_t at = mixed || (op->mode == AggMode::PartialMerge && buffer_offset != 0) ? (size_t)std::max<int64_t>(buffer_offset, 0) : op->grouping.size();
+        if (buffer_offset < 0) throw PlanError("negative initial_input_buffer_offset");
+        for (auto& a : op->aggs) {
+            if (a.mode == AggMode::Partial) continue;
+            a.state_at = (int)at;
+            for (auto& t : agg_state_types(a)) {
+                if (at >= cs.size()) throw PlanError("merging aggregate: state columns run past the child's " + std::to_string(cs.size()) + " columns");
+                if (cs[at] != t) throw PlanError("merging aggregate: state column " + std::to_string(at) + " is " + cs[at].str() + ", expected " + t.str());
+                at++;
+            }
         }
         have = true;
         break;

@@ -99,6 +99,10 @@ struct AggExpr {
     DType sum_datatype;          // Avg: sum state type
     EvalMode eval_mode = EvalMode::Legacy;
     ExprP filter;                // FILTER (WHERE ...) clause, Partial mode only
+    // this aggregate's own mode: the operator's, or its HashAggregate.expr_modes entry.  Partial updates from `children`;
+    // PartialMerge / Final merge the state columns that start at child column `state_at` (-1 for Partial).
+    AggMode mode = AggMode::Partial;
+    int state_at = -1;
 };
 
 enum class OpKind { Scan, ShuffleScan, NativeScan, Projection, Filter, HashAgg, ShuffleWriter, Sort };
@@ -140,7 +144,7 @@ struct Operator {
     // HashAgg
     std::vector<ExprP> grouping;
     std::vector<AggExpr> aggs;
-    AggMode mode = AggMode::Partial;
+    AggMode mode = AggMode::Partial; // the operator's mode (each aggregate's own: AggExpr::mode)
     // ShuffleWriter (hash partitioning only)
     std::vector<ExprP> hash_exprs;
     int num_partitions = 0;
