@@ -65,7 +65,8 @@ class Stats(C.Structure):
                 ("pipeline_rows", C.c_int64), ("h2d_bytes", C.c_int64), ("d2h_bytes", C.c_int64),
                 ("scan_pruned_row_groups", C.c_int64), ("scan_pruned_rows", C.c_int64), ("agg_strategies", C.c_int64),
                 ("scan_pruned_pages", C.c_int64), ("scan_page_pruned_rows", C.c_int64), ("sort_rows", C.c_int64),
-                ("sort_passes", C.c_int64), ("sort_pass_rows", C.c_int64), ("sort_select_rows", C.c_int64)]
+                ("sort_passes", C.c_int64), ("sort_pass_rows", C.c_int64), ("sort_select_rows", C.c_int64),
+                ("join_build_rows", C.c_int64), ("join_probe_rows", C.c_int64), ("join_out_rows", C.c_int64)]
 AGG_DENSE, AGG_TABLE, AGG_STREAM, AGG_MIGRATED = 1, 2, 4, 8  # cb200_stats.agg_strategies bits (CB200_AGG_*)
 
 

@@ -66,12 +66,14 @@ EXPR_FIELD = dict(literal=2, bound=3, add=4, subtract=5, multiply=6, divide=7, c
                   lt=13, lt_eq=14, is_null=15, is_not_null=16, **{"and": 17, "or": 18}, sort_order=19, check_overflow=25, like=26,
                   scalarFunc=31, caseWhen=38, **{"in": 39, "not": 40}, unary_minus=41, **{"if": 44}, unbound=51)  # expr.proto:30-109
 AGG_FIELD = dict(count=2, sum=3, min=4, max=5, avg=6)  # expr.proto:143-176
-OP_FIELD = dict(scan=100, projection=101, filter=102, sort=103, hash_agg=104, limit=105, shuffle_writer=106,
+OP_FIELD = dict(scan=100, projection=101, filter=102, sort=103, hash_agg=104, limit=105, shuffle_writer=106, hash_join=109,
                 native_scan=111, shuffle_scan=116)  # operator.proto:32-86
 LITERAL_FIELD = dict(bool_val=1, byte_val=2, short_val=3, int_val=4, long_val=5, float_val=6, double_val=7,
                      string_val=8, bytes_val=9, decimal_val=10, datatype=12, is_null=13)  # literal.proto:26-47
 LEGACY, TRY, ANSI = 0, 1, 2  # expr.proto:324 EvalMode
 PARTIAL, FINAL, PARTIAL_MERGE = 0, 1, 2  # operator.proto AggregateMode
+INNER, LEFT_OUTER, RIGHT_OUTER, FULL_OUTER, LEFT_SEMI, LEFT_ANTI = 0, 1, 2, 3, 4, 5  # operator.proto JoinType
+BUILD_LEFT, BUILD_RIGHT = 0, 1  # operator.proto BuildSide
 
 
 # ---- DataType (types.proto:43-114) ---------------------------------------------------------------
@@ -328,6 +330,17 @@ def sort(child, orders, fetch=None, skip=None, plan_id=0):  # Sort operator.prot
     if skip is not None:
         body += f_varint(4, skip)
     return _op("sort", body, (child,), plan_id)
+
+
+def hash_join(left, right, left_keys, right_keys, join_type, build_side, condition=None, null_aware=False, plan_id=0):
+    """HashJoin operator.proto:754-763: children (left, right), key expressions of each side."""
+    body = b"".join(f_len(1, k) for k in left_keys) + b"".join(f_len(2, k) for k in right_keys) + f_varint(3, join_type)
+    if condition is not None:
+        body += f_len(4, condition)
+    body += f_varint(5, build_side)
+    if null_aware:
+        body += f_bool(6, True)
+    return _op("hash_join", body, (left, right), plan_id)
 
 
 def struct_field(name, dt, nullable=True):  # SparkStructField operator.proto:97

@@ -354,6 +354,9 @@ int cb200_plan_stats(cb200_plan* plan, cb200_stats* out) {
     out->sort_passes = c.sort_passes;
     out->sort_pass_rows = c.sort_pass_rows;
     out->sort_select_rows = c.sort_select_rows;
+    out->join_build_rows = c.join_build_rows;
+    out->join_probe_rows = c.join_probe_rows;
+    out->join_out_rows = c.join_out_rows;
     return 0;
 }
 

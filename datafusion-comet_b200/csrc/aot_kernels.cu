@@ -664,6 +664,106 @@ void launch_sort_iota(unsigned* idx, i64 n, cudaStream_t st) {
 
 i64 sort_tiles(i64 n) { return (n + SORT_TILE - 1) / SORT_TILE; }
 
+// ---- hash join ------------------------------------------------------------------------------------------------------------------------------
+// The build side's row keys are radix-sorted, so equal keys form runs in build input order.  Each distinct key (run) owns one slot of an
+// open-addressing table, found by linear probing from its hash; a slot stores a 32-bit tag of the hash and the run, and a tag hit is
+// confirmed against the run's key words, so two keys are never merged and no collision can fail the query.
+__device__ __forceinline__ u64 join_hash(const u64* k, int W) {
+    u64 h = 0x9E3779B97F4A7C15ull;
+#pragma unroll
+    for (int j = 0; j < SK_MAX_WORDS; j++) {
+        if (j >= W) break;
+        h ^= k[j];
+        h ^= h >> 33; h *= 0xff51afd7ed558ccdull; h ^= h >> 33; h *= 0xc4ceb9fe1a85ec53ull; h ^= h >> 33; // murmur3 fmix64
+    }
+    return h;
+}
+__device__ __forceinline__ bool join_no_null(const JoinTable& t, const u64* k) {
+    bool ok = true;
+#pragma unroll
+    for (int j = 0; j < SK_MAX_WORDS; j++)
+        if (j < t.words) ok &= (k[j] & t.nullmask[j]) == t.nullmask[j];
+    return ok;
+}
+__global__ void k_join_heads(const u64* keys, int W, i64 m, u8* head) {
+    const i64 i = (i64)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m) return;
+    bool h = i == 0;
+    for (int j = 0; j < W && !h; j++) h = keys[i * W + j] != keys[(i - 1) * W + j];
+    head[i] = h;
+}
+__global__ void k_join_insert(JoinTable t, i64 n_runs) {
+    const i64 r = (i64)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n_runs) return;
+    const u64* k = t.keys + (i64)t.run_start[r] * t.words;
+    if (!join_no_null(t, k)) return;
+    const u64 h = join_hash(k, t.words), v = ((h >> 32) << 32) | (u64)(r + 1);
+    for (u64 s = h & t.mask;; s = (s + 1) & t.mask) // capacity >= 2 x runs: a free slot exists
+        if (atomicCAS((unsigned long long*)&t.slots[s], 0ull, (unsigned long long)v) == 0ull) return;
+}
+// the run of key k, or -1
+__device__ __forceinline__ i64 join_find(const JoinTable& t, const u64* k) {
+    if (!join_no_null(t, k)) return -1;
+    const u64 h = join_hash(k, t.words);
+    const u32 tag = (u32)(h >> 32);
+    for (u64 s = h & t.mask;; s = (s + 1) & t.mask) {
+        const u64 v = t.slots[s];
+        if (v == 0) return -1;
+        if ((u32)(v >> 32) != tag) continue;
+        const i64 r = (i64)(u32)v - 1;
+        const u64* b = t.keys + (i64)t.run_start[r] * t.words;
+        bool eq = true;
+#pragma unroll
+        for (int j = 0; j < SK_MAX_WORDS; j++)
+            if (j < t.words) eq &= b[j] == k[j];
+        if (eq) return r;
+    }
+}
+__global__ void __launch_bounds__(256) k_join_probe(JoinTable t, const u64* keys, i64 n, int mode, u32* counts, u32* run_of, u64* total, u8* keep) {
+    const i64 i = (i64)blockIdx.x * blockDim.x + threadIdx.x;
+    u64 c = 0;
+    if (i < n) {
+        u64 k[SK_MAX_WORDS];
+#pragma unroll
+        for (int j = 0; j < SK_MAX_WORDS; j++) k[j] = j < t.words ? keys[i * t.words + j] : 0;
+        const i64 r = join_find(t, k);
+        if (mode == CB_JOIN_COUNT) {
+            c = r < 0 ? 0 : t.run_start[r + 1] - t.run_start[r];
+            counts[i] = (u32)c;
+            run_of[i] = r < 0 ? 0xffffffffu : (u32)r;
+        } else keep[i] = (r >= 0) == (mode == CB_JOIN_SEMI);
+    }
+    if (mode != CB_JOIN_COUNT) return;
+#pragma unroll
+    for (int o = 16; o; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
+    if ((threadIdx.x & 31) == 0 && c) atomicAdd((unsigned long long*)total, (unsigned long long)c);
+}
+__global__ void k_join_emit(JoinTable t, const u32* run_of, const u32* offs, const u32* chunk_off, i64 n, i64 o0, i64 o1, u32* probe_idx, u32* build_idx) {
+    const i64 i = (i64)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const u32 r = run_of[i];
+    if (r == 0xffffffffu) return;
+    const i64 b0 = t.run_start[r], c = (i64)t.run_start[r + 1] - b0, off = (i64)offs[i] + chunk_off[i >> 12];
+    const i64 lo = max(off, o0), hi = min(off + c, o1);
+    for (i64 p = lo; p < hi; p++) {
+        probe_idx[p - o0] = (u32)i;
+        build_idx[p - o0] = t.rows[b0 + (p - off)];
+    }
+}
+void launch_join_heads(const u64* keys, int words, i64 m, u8* head, cudaStream_t st) {
+    if (m > 0) k_join_heads<<<(unsigned)((m + 255) / 256), 256, 0, st>>>(keys, words, m, head);
+}
+void launch_join_insert(const JoinTable& t, i64 n_runs, cudaStream_t st) {
+    if (n_runs > 0) k_join_insert<<<(unsigned)((n_runs + 255) / 256), 256, 0, st>>>(t, n_runs);
+}
+void launch_join_probe(const JoinTable& t, const u64* keys, i64 n, int mode, u32* counts, u32* run_of, u64* total, u8* keep, cudaStream_t st) {
+    if (n > 0) k_join_probe<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(t, keys, n, mode, counts, run_of, total, keep);
+}
+void launch_join_emit(const JoinTable& t, const u32* run_of, const u32* offs, const u32* chunk_off, i64 n, i64 o0, i64 o1, u32* probe_idx, u32* build_idx,
+                      cudaStream_t st) {
+    if (n > 0 && o1 > o0) k_join_emit<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(t, run_of, offs, chunk_off, n, o0, o1, probe_idx, build_idx);
+}
+
 template <int W> static cudaError_t sort_pass(const RadixScratch& s, i64 n, int digit, int from, bool first, cudaStream_t st) {
     const i64 nt = sort_tiles(n);
     k_sort_hist<W><<<(unsigned)nt, 256, 0, st>>>(s.keys[from], n, digit, nt, s.hist);

@@ -87,6 +87,34 @@ cudaError_t launch_sort_select_keep(const unsigned long long* keys, int words, l
                                     int* counts, long long* offsets, long long* total, unsigned char* keep, cudaStream_t st);
 void launch_sort_iota(unsigned* idx, long long n, cudaStream_t st); // idx[i] = i
 
+// ---- hash join: build keys sorted by the radix sort, one table slot per distinct key, probe by lookup ------------------------------------
+// Row keys are the sort's (device/cb_sortkey.h), `words` words per row, every key field with a null bit that is set on a valid value:
+// a key has no NULL field iff (k[j] & nullmask[j]) == nullmask[j] for every word.  The build side's keys[m] are sorted with their row
+// indices rows[m]; run r of equal keys is sorted rows [run_start[r], run_start[r + 1]).  slots[mask + 1]: 0 = empty, otherwise
+// (hash tag << 32) | (run + 1).
+struct JoinTable {
+    const unsigned long long* keys;
+    const unsigned* rows;
+    const unsigned* run_start;
+    unsigned long long* slots;
+    unsigned long long mask;
+    int words;
+    unsigned long long nullmask[cb::SK_MAX_WORDS];
+};
+// head[i] = 1 where sorted key i differs from key i - 1 (row 0 always): the run heads
+void launch_join_heads(const unsigned long long* keys, int words, long long m, unsigned char* head, cudaStream_t st);
+// every run r < n_runs whose key has no NULL field gets one slot
+void launch_join_insert(const JoinTable& t, long long n_runs, cudaStream_t st);
+enum { CB_JOIN_COUNT = 0, CB_JOIN_SEMI = 1, CB_JOIN_ANTI = 2 };
+// one lookup per probe key (NULL fields match nothing).  CB_JOIN_COUNT: counts[i] = matching build rows, run_of[i] = their run (~0 when
+// none), *total += the sum of counts (64-bit; the caller zeroes it).  CB_JOIN_SEMI / ANTI: keep[i] = a match exists / none does.
+void launch_join_probe(const JoinTable& t, const unsigned long long* keys, long long n, int mode, unsigned* counts, unsigned* run_of,
+                       unsigned long long* total, unsigned char* keep, cudaStream_t st);
+// inner join pairs at output positions [o0, o1): probe row i's matches occupy [off_i, off_i + count_i), off_i = offs[i] + chunk_off[i / 4096]
+// (launch_scan_u32 over the counts); probe_idx[p - o0] = i, build_idx[p - o0] = the build row, in build input order
+void launch_join_emit(const JoinTable& t, const unsigned* run_of, const unsigned* offs, const unsigned* chunk_off, long long n, long long o0,
+                      long long o1, unsigned* probe_idx, unsigned* build_idx, cudaStream_t st);
+
 // device values -> the Arrow layout of their logical type, rows [0, n): what the hand-off (Arrow export, cb200_execute_device) gives out
 enum { CB_SEXT32_TO_128, CB_SEXT64_TO_128, CB_NARROW32_TO_8, CB_NARROW32_TO_16, CB_BITS_TO_BYTES };
 void launch_to_arrow_layout(int conv, const void* in, long long n, void* out, cudaStream_t st);

@@ -884,6 +884,119 @@ struct PartitionNode : ExecNode {
     }
 };
 
+// ---- shared by Sort and HashJoin -------------------------------------------------------------------------------------------------
+// the rows of bs in one batch (`bs` non-empty, every batch on the device): values and validity appended in order; dictionary-coded strings
+// that carry different Dictionary objects are recoded into one (the first batch's entries, then the others' new entries)
+static Batch concat_batches(const std::vector<Batch>& bs, ExecContext* ctx, const char* op) {
+    cudaStream_t st = ctx->stream;
+    Batch out;
+    for (auto& b : bs) out.n_rows += b.n_rows;
+    const size_t n = (size_t)out.n_rows;
+    std::vector<DeviceBufP> temps;
+    for (size_t j = 0; j < bs[0].cols.size(); j++) {
+        const Column& c0 = bs[0].cols[j];
+        Column o;
+        o.type = c0.type;
+        o.phys = c0.phys;
+        o.is_dict = c0.is_dict;
+        o.dict = c0.dict;
+        bool same = true, nulls = false;
+        for (auto& b : bs) {
+            const Column& c = b.cols[j];
+            if (c.phys != c0.phys || c.dict != c0.dict || c.is_dict != c0.is_dict) same = false;
+            if (c.validity) nulls = true;
+        }
+        if (!same && !c0.is_dict) throw Unsupported(std::string(op) + " input whose batches store column " + std::to_string(j) + " in different layouts");
+        if (same) {
+            const int w = phys_bytes(c0.phys);
+            o.data = std::make_shared<DeviceBuf>(w == 0 ? bitmap_bytes((int64_t)n) : std::max<size_t>(n, 1) * (size_t)w);
+            if (w == 0) cuda_check(cudaMemsetAsync(o.data->ptr, 0, o.data->bytes, st), "memset bools");
+            int64_t row = 0;
+            for (auto& b : bs) {
+                const Column& c = b.cols[j];
+                if (w == 0) { launch_bitmap_append((uint32_t*)o.data->ptr, row, (const uint8_t*)c.data->ptr, 0, b.n_rows, st); ctx->kernel_launches++; }
+                else cuda_check(cudaMemcpyAsync((char*)o.data->ptr + (size_t)row * w, c.data->ptr, (size_t)b.n_rows * w, cudaMemcpyDeviceToDevice, st), "concat column");
+                row += b.n_rows;
+            }
+        } else { // dictionary codes -> int32 codes of one dictionary
+            auto d = std::make_shared<Dictionary>(*c0.dict);
+            o.phys = Phys::I32;
+            o.dict = d;
+            o.data = std::make_shared<DeviceBuf>(std::max<size_t>(n, 1) * 4);
+            int64_t row = 0;
+            for (auto& b : bs) {
+                const Column& c = b.cols[j];
+                const std::vector<std::string>& vals = c.dict->values();
+                std::vector<int32_t> table(vals.size());
+                for (size_t k = 0; k < table.size(); k++) table[k] = c.dict == c0.dict ? (int32_t)k : d->intern(vals[k]);
+                auto dt = std::make_shared<DeviceBuf>(table.size() * 4 + 4);
+                temps.push_back(dt);
+                if (!table.empty()) cuda_check(cudaMemcpyAsync(dt->ptr, table.data(), table.size() * 4, cudaMemcpyHostToDevice, st), "H2D remap table");
+                cuda_check(cudaStreamSynchronize(st), "remap table copy"); // table is a loop temporary
+                launch_remap_codes(c.data->ptr, phys_bytes(c.phys), b.n_rows, (const int*)dt->ptr, (int)table.size(), (int*)o.data->ptr + row, st);
+                ctx->kernel_launches++;
+                row += b.n_rows;
+            }
+        }
+        if (nulls) {
+            o.validity = std::make_shared<DeviceBuf>(bitmap_bytes((int64_t)n));
+            cuda_check(cudaMemsetAsync(o.validity->ptr, 0, o.validity->bytes, st), "memset validity");
+            int64_t row = 0;
+            for (auto& b : bs) {
+                const Column& c = b.cols[j];
+                launch_bitmap_append((uint32_t*)o.validity->ptr, row, c.validity ? (const uint8_t*)c.validity->ptr : nullptr, 0, b.n_rows, st);
+                ctx->kernel_launches++;
+                row += b.n_rows;
+            }
+            o.null_count = -1;
+        }
+        out.cols.push_back(o);
+    }
+    cuda_check(cudaGetLastError(), "concat launches");
+    return out;
+}
+
+// the stable order of m rows whose keys (`words` words each) are in keys0, by the given digits: row indices [0, m); `sorted_keys`, if
+// given, receives the keys in that order
+static DeviceBufP radix_order(ExecContext* ctx, DeviceBufP keys0, int words, int64_t m, const std::vector<int>& digits, DeviceBufP* sorted_keys = nullptr) {
+    cudaStream_t st = ctx->stream;
+    const int64_t nt = sort_tiles(m);
+    auto keys1 = std::make_shared<DeviceBuf>((size_t)m * words * 8);
+    auto idx0 = std::make_shared<DeviceBuf>((size_t)m * 4), idx1 = std::make_shared<DeviceBuf>((size_t)m * 4);
+    auto hist = std::make_shared<DeviceBuf>((size_t)nt * 256 * 4), chunk_off = std::make_shared<DeviceBuf>((size_t)(nt * 256 / 4096 + 2) * 4);
+    auto total = std::make_shared<DeviceBuf>(8);
+    RadixScratch s{{(unsigned long long*)keys0->ptr, (unsigned long long*)keys1->ptr}, {(unsigned*)idx0->ptr, (unsigned*)idx1->ptr},
+                   (unsigned*)hist->ptr, (unsigned*)chunk_off->ptr, (long long*)total->ptr};
+    int r = 0;
+    cuda_check(launch_sort_passes(s, words, m, digits.data(), (int)digits.size(), &r, st), "sort passes");
+    ctx->kernel_launches += digits.empty() ? 1 : 4 * (int64_t)digits.size();
+    if (sorted_keys) *sorted_keys = r ? keys1 : keys0;
+    return r ? idx1 : idx0; // the other buffers go back to the stream-ordered pool
+}
+
+// the row keys of kc (kc.words words each) for n rows.  h_and_or[0, W) receives their AND and [W, 2W) their OR, `digits` the 8-bit
+// digits of the `bits`-bit key that are not the same in every row, least significant first.  Synchronises: a dictionary code outside its
+// dictionary fails here.
+static DeviceBufP pack_row_keys(const cb::SortKeyCols& kc, int64_t n, int bits, ExecContext* ctx, uint64_t* h_and_or, std::vector<int>& digits) {
+    cudaStream_t st = ctx->stream;
+    const int W = kc.words;
+    auto keys0 = std::make_shared<DeviceBuf>((size_t)n * W * 8);
+    auto and_or = std::make_shared<DeviceBuf>(2 * cb::SK_MAX_WORDS * 8);
+    cuda_check(cudaMemsetAsync(and_or->ptr, 0xff, (size_t)W * 8, st), "memset key and");
+    cuda_check(cudaMemsetAsync((char*)and_or->ptr + W * 8, 0, (size_t)W * 8, st), "memset key or");
+    launch_sort_keys(kc, n, (unsigned long long*)keys0->ptr, (unsigned long long*)and_or->ptr, st);
+    cuda_check(cudaGetLastError(), "k_sort_keys launch");
+    ctx->kernel_launches++;
+    cuda_check(cudaMemcpyAsync(h_and_or, and_or->ptr, (size_t)W * 16, cudaMemcpyDeviceToHost, st), "D2H key and / or");
+    ctx->check_device_errors(); // also synchronises
+    digits.clear();
+    for (int d = 0; d < (bits + 7) / 8; d++) {
+        const int w = W - 1 - d / 8, sh = (d % 8) * 8;
+        if (((h_and_or[w] ^ h_and_or[W + w]) >> sh) & 0xff) digits.push_back(d);
+    }
+    return keys0;
+}
+
 // =================================================================================================
 // sort (SortExec(LexOrdering).with_fetch(fetch) then GlobalLimitExec(skip), planner.rs:1488-1522)
 // =================================================================================================
@@ -903,6 +1016,10 @@ struct SortNode : ExecNode {
     std::vector<Rank> ranks; // per key: code -> byte-order rank of the dictionary it was built for
 
     bool topk() const { return fetch >= 0 && fetch <= ctx->chunk_rows; }
+    void count_passes(int64_t m, const std::vector<int>& digits) {
+        ctx->sort_passes += (int64_t)digits.size();
+        ctx->sort_pass_rows += m * (int64_t)digits.size();
+    }
 
     bool next(Batch& out) override {
         if (done) return false;
@@ -920,7 +1037,7 @@ struct SortNode : ExecNode {
                 sort_rows(in, 0, std::min<int64_t>(fetch, in.n_rows), top);
                 in = Batch();
                 if (any) {
-                    Batch u = concat({all, top});
+                    Batch u = concat_batches({all, top}, ctx, "sort");
                     sort_rows(u, 0, std::min<int64_t>(fetch, u.n_rows), all);
                 } else all = std::move(top);
                 any = true;
@@ -933,7 +1050,7 @@ struct SortNode : ExecNode {
                 in = Batch();
             }
             any = !batches.empty();
-            if (any) all = batches.size() == 1 ? std::move(batches[0]) : concat(batches);
+            if (any) all = batches.size() == 1 ? std::move(batches[0]) : concat_batches(batches, ctx, "sort");
         }
         if (!any) return false;
         const int64_t lo = std::min(skip, all.n_rows), hi = fetch >= 0 ? std::min(fetch, all.n_rows) : all.n_rows;
@@ -947,77 +1064,6 @@ struct SortNode : ExecNode {
         columns_to_device(b, ctx);
         for (auto& c : b.cols)
             if (c.offsets) throw Unsupported("sorting plain string columns (dictionary-encode them first)");
-    }
-
-    // b's rows in one batch (`bs` non-empty, every batch on the device): values and validity appended in order; dictionary-coded strings
-    // that carry different Dictionary objects are recoded into one (the first batch's entries, then the others' new entries)
-    Batch concat(const std::vector<Batch>& bs) {
-        cudaStream_t st = ctx->stream;
-        Batch out;
-        for (auto& b : bs) out.n_rows += b.n_rows;
-        const size_t n = (size_t)out.n_rows;
-        std::vector<DeviceBufP> temps;
-        for (size_t j = 0; j < bs[0].cols.size(); j++) {
-            const Column& c0 = bs[0].cols[j];
-            Column o;
-            o.type = c0.type;
-            o.phys = c0.phys;
-            o.is_dict = c0.is_dict;
-            o.dict = c0.dict;
-            bool same = true, nulls = false;
-            for (auto& b : bs) {
-                const Column& c = b.cols[j];
-                if (c.phys != c0.phys || c.dict != c0.dict || c.is_dict != c0.is_dict) same = false;
-                if (c.validity) nulls = true;
-            }
-            if (!same && !c0.is_dict) throw Unsupported("sort input whose batches store column " + std::to_string(j) + " in different layouts");
-            if (same) {
-                const int w = phys_bytes(c0.phys);
-                o.data = std::make_shared<DeviceBuf>(w == 0 ? bitmap_bytes((int64_t)n) : std::max<size_t>(n, 1) * (size_t)w);
-                if (w == 0) cuda_check(cudaMemsetAsync(o.data->ptr, 0, o.data->bytes, st), "memset bools");
-                int64_t row = 0;
-                for (auto& b : bs) {
-                    const Column& c = b.cols[j];
-                    if (w == 0) { launch_bitmap_append((uint32_t*)o.data->ptr, row, (const uint8_t*)c.data->ptr, 0, b.n_rows, st); ctx->kernel_launches++; }
-                    else cuda_check(cudaMemcpyAsync((char*)o.data->ptr + (size_t)row * w, c.data->ptr, (size_t)b.n_rows * w, cudaMemcpyDeviceToDevice, st), "concat column");
-                    row += b.n_rows;
-                }
-            } else { // dictionary codes -> int32 codes of one dictionary
-                auto d = std::make_shared<Dictionary>(*c0.dict);
-                o.phys = Phys::I32;
-                o.dict = d;
-                o.data = std::make_shared<DeviceBuf>(std::max<size_t>(n, 1) * 4);
-                int64_t row = 0;
-                for (auto& b : bs) {
-                    const Column& c = b.cols[j];
-                    const std::vector<std::string>& vals = c.dict->values();
-                    std::vector<int32_t> table(vals.size());
-                    for (size_t k = 0; k < table.size(); k++) table[k] = c.dict == c0.dict ? (int32_t)k : d->intern(vals[k]);
-                    auto dt = std::make_shared<DeviceBuf>(table.size() * 4 + 4);
-                    temps.push_back(dt);
-                    if (!table.empty()) cuda_check(cudaMemcpyAsync(dt->ptr, table.data(), table.size() * 4, cudaMemcpyHostToDevice, st), "H2D remap table");
-                    cuda_check(cudaStreamSynchronize(st), "remap table copy"); // table is a loop temporary
-                    launch_remap_codes(c.data->ptr, phys_bytes(c.phys), b.n_rows, (const int*)dt->ptr, (int)table.size(), (int*)o.data->ptr + row, st);
-                    ctx->kernel_launches++;
-                    row += b.n_rows;
-                }
-            }
-            if (nulls) {
-                o.validity = std::make_shared<DeviceBuf>(bitmap_bytes((int64_t)n));
-                cuda_check(cudaMemsetAsync(o.validity->ptr, 0, o.validity->bytes, st), "memset validity");
-                int64_t row = 0;
-                for (auto& b : bs) {
-                    const Column& c = b.cols[j];
-                    launch_bitmap_append((uint32_t*)o.validity->ptr, row, c.validity ? (const uint8_t*)c.validity->ptr : nullptr, 0, b.n_rows, st);
-                    ctx->kernel_launches++;
-                    row += b.n_rows;
-                }
-                o.null_count = -1;
-            }
-            out.cols.push_back(o);
-        }
-        cuda_check(cudaGetLastError(), "concat launches");
-        return out;
     }
 
     // the code -> rank table of dictionary d: equal strings get equal ranks, ranks follow unsigned byte order.  Rebuilt when the
@@ -1041,24 +1087,6 @@ struct SortNode : ExecNode {
         r.dict = d.get();
         r.n = v.size();
         return (const uint32_t*)r.table->ptr;
-    }
-
-    // the stable order of m rows whose keys (`words` words each) are in keys0, by the given digits: row indices [0, m)
-    DeviceBufP radix_order(DeviceBufP keys0, int words, int64_t m, const std::vector<int>& digits) {
-        cudaStream_t st = ctx->stream;
-        const int64_t nt = sort_tiles(m);
-        auto keys1 = std::make_shared<DeviceBuf>((size_t)m * words * 8);
-        auto idx0 = std::make_shared<DeviceBuf>((size_t)m * 4), idx1 = std::make_shared<DeviceBuf>((size_t)m * 4);
-        auto hist = std::make_shared<DeviceBuf>((size_t)nt * 256 * 4), chunk_off = std::make_shared<DeviceBuf>((size_t)(nt * 256 / 4096 + 2) * 4);
-        auto total = std::make_shared<DeviceBuf>(8);
-        RadixScratch s{{(unsigned long long*)keys0->ptr, (unsigned long long*)keys1->ptr}, {(unsigned*)idx0->ptr, (unsigned*)idx1->ptr},
-                       (unsigned*)hist->ptr, (unsigned*)chunk_off->ptr, (long long*)total->ptr};
-        int r = 0;
-        cuda_check(launch_sort_passes(s, words, m, digits.data(), (int)digits.size(), &r, st), "sort passes");
-        ctx->kernel_launches += digits.empty() ? 1 : 4 * (int64_t)digits.size();
-        ctx->sort_passes += (int64_t)digits.size();
-        ctx->sort_pass_rows += m * (int64_t)digits.size();
-        return r ? idx1 : idx0; // the other buffers go back to the stream-ordered pool
     }
 
     // out = b's rows [lo, hi) of the stable order of the keys.  When only the first rows are wanted (lo = 0, hi < n: TopK), an MSD radix
@@ -1092,24 +1120,13 @@ struct SortNode : ExecNode {
             bits += f.bits + f.has_null;
         }
         const int W = kc.words = std::max(1, (bits + 63) / 64);
-        auto keys0 = std::make_shared<DeviceBuf>((size_t)n * W * 8);
-        auto and_or = std::make_shared<DeviceBuf>(2 * cb::SK_MAX_WORDS * 8);
-        cuda_check(cudaMemsetAsync(and_or->ptr, 0xff, (size_t)W * 8, st), "memset key and");
-        cuda_check(cudaMemsetAsync((char*)and_or->ptr + W * 8, 0, (size_t)W * 8, st), "memset key or");
-        launch_sort_keys(kc, n, (unsigned long long*)keys0->ptr, (unsigned long long*)and_or->ptr, st);
-        cuda_check(cudaGetLastError(), "k_sort_keys launch");
-        ctx->kernel_launches++;
-        ctx->sort_rows += n;
         uint64_t h_and_or[2 * cb::SK_MAX_WORDS];
-        cuda_check(cudaMemcpyAsync(h_and_or, and_or->ptr, (size_t)W * 16, cudaMemcpyDeviceToHost, st), "D2H key and / or");
-        ctx->check_device_errors(); // also synchronises; a dictionary code outside its dictionary fails here
-        std::vector<int> digits; // the 8-bit digits that differ between rows, least significant first
-        for (int d = 0; d < (bits + 7) / 8; d++) {
-            const int w = W - 1 - d / 8, sh = (d % 8) * 8;
-            if (((h_and_or[w] ^ h_and_or[W + w]) >> sh) & 0xff) digits.push_back(d);
-        }
+        std::vector<int> digits;
+        DeviceBufP keys0 = pack_row_keys(kc, n, bits, ctx, h_and_or, digits);
+        ctx->sort_rows += n;
         if (lo > 0 || hi >= n) {
-            DeviceBufP idx = radix_order(keys0, W, n, digits);
+            DeviceBufP idx = radix_order(ctx, keys0, W, n, digits);
+            count_passes(n, digits);
             keys0.reset();
             gather_columns(b, (const unsigned*)idx->ptr + lo, hi - lo, out, ctx, "sorting");
             ctx->check_device_errors();
@@ -1152,12 +1169,272 @@ struct SortNode : ExecNode {
         cuda_check(cudaStreamSynchronize(st), "select sync");
         if (m != hi) throw ExecError(15, "", "internal: TopK selection kept " + std::to_string(m) + " rows for a fetch of " + std::to_string(hi));
         keys0.reset(); rows.reset(); eq.reset(); keep.reset();
-        DeviceBufP order = radix_order(ckeys, W, m, digits);
+        DeviceBufP order = radix_order(ctx, ckeys, W, m, digits);
+        count_passes(m, digits);
         auto idx = std::make_shared<DeviceBuf>((size_t)m * 4);
         launch_gather(crows->ptr, 4, (const unsigned*)order->ptr, m, idx->ptr, st); // compacted position -> row of b
         ctx->kernel_launches++;
         gather_columns(b, (const unsigned*)idx->ptr, m, out, ctx, "sorting");
         ctx->check_device_errors();
+    }
+};
+
+// =================================================================================================
+// hash join (HashJoinExec with NullEquality::NullEqualsNothing, planner.rs:2192-2266): inner, left semi and left anti
+// =================================================================================================
+// The build side is drained before the first probe batch and concatenated on the device.  Its row keys (the sort's encoding,
+// device/cb_sortkey.h) are radix-sorted, so equal keys form runs in build input order, and every run without a NULL key gets one slot of
+// an open-addressing table.  A probe batch then costs one key pass and one lookup per row; an inner join scans the match counts, writes
+// the (probe row, build row) pairs and gathers both sides, a semi / anti join compacts the probe rows it keeps.  Output order: probe rows
+// in input order, an inner-join row's matches in build input order; an inner join's output above spark.comet.b200.chunkRows rows leaves
+// in several batches.
+//
+// Equal key tuples give equal words on both sides because the field layout is fixed by the declared key types (every field has a null
+// bit, whatever a batch's validity) and a string field holds a canonical code rather than the dictionary code: the code of the first
+// equal entry of the build side's dictionary, or that dictionary's size (which no build key has) for a probe string it lacks.
+struct JoinNode : ExecNode {
+    ExecContext* ctx;
+    ExecNodeP build_child, probe_child;
+    std::vector<int> build_keys, probe_keys; // key columns of each side, in key order
+    JoinType type = JoinType::Inner;
+    bool build_left = false;
+    int bits = 0, W = 1;                     // packed key bits (fixed per plan) and words
+    cb::u64 nullmask[cb::SK_MAX_WORDS] = {0, 0, 0, 0};
+
+    bool built = false;
+    Batch build;                             // the build side's rows, concatenated
+    DeviceBufP keys, rows, run_start, slots; // sorted build keys and their rows, run starts (+ the end), the table
+    JoinTable table{};
+    uint32_t h_build_rows = 0;
+    std::vector<DeviceBufP> build_canon;     // per key: build dictionary code -> canonical code
+    struct Canon { DictionaryP dict; size_t n = 0; DeviceBufP table; };
+    std::vector<Canon> probe_canon;          // per key: the probe dictionary it was built for, code -> canonical code
+
+    Batch probe;                             // the probe batch being emitted ...
+    DeviceBufP run_of, offs, chunk_off, kept_rows;
+    int64_t total = 0, pos = 0;              // ... its output rows, and those emitted
+
+    // the key layout from the declared key types: the last key is the least significant field, each with a null bit above its value
+    void set_layout(const std::vector<DType>& key_types) {
+        bits = 0;
+        for (size_t k = key_types.size(); k-- > 0;) bits += sort_key_bits(key_types[k]) + 1;
+        W = std::max(1, (bits + 63) / 64);
+        int off = 0;
+        for (size_t k = key_types.size(); k-- > 0;) {
+            off += sort_key_bits(key_types[k]);
+            cb::sk_put(nullmask, W, off, 1, 1);
+            off++;
+        }
+    }
+
+    void arrive(Batch& b) {
+        columns_to_device(b, ctx);
+        for (auto& c : b.cols)
+            if (c.offsets) throw Unsupported("joining plain string columns (dictionary-encode them first)");
+    }
+
+    DeviceBufP upload_codes(const std::vector<uint32_t>& v) {
+        auto t = std::make_shared<DeviceBuf>(v.size() * 4 + 4);
+        if (!v.empty()) cuda_check(cudaMemcpyAsync(t->ptr, v.data(), v.size() * 4, cudaMemcpyHostToDevice, ctx->stream), "H2D join codes");
+        cuda_check(cudaStreamSynchronize(ctx->stream), "join codes copy"); // v is the caller's temporary
+        ctx->h2d_bytes += (int64_t)(v.size() * 4);
+        return t;
+    }
+    // canonical codes of key k's dictionary d on the build side: the first equal entry (a caller's dictionary may repeat values)
+    const uint32_t* build_codes(size_t k, const DictionaryP& d) {
+        const std::vector<std::string>& v = d->values();
+        std::vector<uint32_t> c(v.size());
+        for (size_t i = 0; i < v.size(); i++) c[i] = (uint32_t)d->find(v[i]);
+        build_canon[k] = upload_codes(c);
+        return (const uint32_t*)build_canon[k]->ptr;
+    }
+    // ... and on the probe side: rebuilt when the column carries another dictionary or its dictionary has grown
+    const uint32_t* probe_codes(size_t k, const DictionaryP& d) {
+        Canon& p = probe_canon[k];
+        const std::vector<std::string>& v = d->values();
+        if (p.table && p.dict == d && p.n == v.size()) return (const uint32_t*)p.table->ptr;
+        const DictionaryP& bd = build.cols[(size_t)build_keys[k]].dict;
+        const uint32_t absent = (uint32_t)bd->values().size();
+        std::vector<uint32_t> c(v.size());
+        for (size_t i = 0; i < v.size(); i++) {
+            const int32_t code = bd->find(v[i]);
+            c[i] = code < 0 ? absent : (uint32_t)code;
+        }
+        p.table = upload_codes(c);
+        p.dict = d;
+        p.n = v.size();
+        return (const uint32_t*)p.table->ptr;
+    }
+    cb::SortKeyCols key_cols(const Batch& b, const std::vector<int>& cols, bool build_side) {
+        cb::SortKeyCols kc;
+        memset(&kc, 0, sizeof(kc));
+        kc.n = (int)cols.size();
+        kc.words = W;
+        kc.err = ctx->d_err;
+        int off = 0;
+        for (size_t k = cols.size(); k-- > 0;) {
+            const Column& c = b.cols.at((size_t)cols[k]);
+            cb::SortKeyCol& f = kc.col[k];
+            f.kind = key_kind(c);
+            f.bits = sort_key_bits(c.type);
+            f.nulls_first = 1; // null bit set on a valid value
+            f.has_null = 1;
+            f.data = c.data ? c.data->ptr : nullptr;
+            f.validity = c.validity ? (const uint8_t*)c.validity->ptr : nullptr;
+            if (c.is_dict) {
+                f.rank = build_side ? build_codes(k, c.dict) : probe_codes(k, c.dict);
+                f.n_rank = (int)c.dict->values().size();
+            }
+            f.off = off;
+            off += f.bits + 1;
+        }
+        return kc;
+    }
+
+    void build_table() {
+        built = true;
+        std::vector<Batch> bs;
+        Batch in;
+        while (build_child->next(in)) {
+            arrive(in);
+            ctx->join_build_rows += in.n_rows;
+            if (in.n_rows > 0) bs.push_back(std::move(in));
+            in = Batch();
+        }
+        if (bs.empty()) return;
+        TraceSpan ts("join.build");
+        build = bs.size() == 1 ? std::move(bs[0]) : concat_batches(bs, ctx, "hash join build");
+        bs.clear();
+        const int64_t n = build.n_rows;
+        if (n >= ((int64_t)1 << 32)) throw Unsupported("a hash join build side of 2^32 rows or more");
+        cudaStream_t st = ctx->stream;
+        build_canon.assign(build_keys.size(), nullptr);
+        probe_canon.assign(build_keys.size(), Canon());
+        uint64_t h_and_or[2 * cb::SK_MAX_WORDS];
+        std::vector<int> digits;
+        DeviceBufP k0 = pack_row_keys(key_cols(build, build_keys, true), n, bits, ctx, h_and_or, digits);
+        rows = radix_order(ctx, k0, W, n, digits, &keys);
+        k0.reset();
+        const size_t nb = (size_t)(n + 1023) / 1024;
+        auto head = std::make_shared<DeviceBuf>((size_t)n + 16), iota = std::make_shared<DeviceBuf>((size_t)n * 4);
+        auto counts = std::make_shared<DeviceBuf>(nb * 4 + 4), offsets = std::make_shared<DeviceBuf>(nb * 8 + 8), d_runs = std::make_shared<DeviceBuf>(8);
+        run_start = std::make_shared<DeviceBuf>((size_t)(n + 1) * 4);
+        launch_join_heads((const unsigned long long*)keys->ptr, W, n, (unsigned char*)head->ptr, st);
+        launch_compact_plan((const unsigned char*)head->ptr, n, (int*)counts->ptr, (long long*)offsets->ptr, (long long*)d_runs->ptr, st);
+        launch_sort_iota((unsigned*)iota->ptr, n, st);
+        launch_compact_scatter((const unsigned char*)head->ptr, n, (const long long*)offsets->ptr, iota->ptr, 4, run_start->ptr, st);
+        cuda_check(cudaGetLastError(), "join run heads");
+        ctx->kernel_launches += 5;
+        int64_t n_runs = 0;
+        cuda_check(cudaMemcpyAsync(&n_runs, d_runs->ptr, 8, cudaMemcpyDeviceToHost, st), "D2H join runs");
+        cuda_check(cudaStreamSynchronize(st), "join runs sync");
+        h_build_rows = (uint32_t)n;
+        cuda_check(cudaMemcpyAsync((uint32_t*)run_start->ptr + n_runs, &h_build_rows, 4, cudaMemcpyHostToDevice, st), "H2D run end");
+        size_t cap = 1024;
+        while (cap < (size_t)n_runs * 2) cap <<= 1;
+        slots = std::make_shared<DeviceBuf>(cap * 8);
+        cuda_check(cudaMemsetAsync(slots->ptr, 0, cap * 8, st), "memset join table");
+        table.keys = (const unsigned long long*)keys->ptr;
+        table.rows = (const unsigned*)rows->ptr;
+        table.run_start = (const unsigned*)run_start->ptr;
+        table.slots = (unsigned long long*)slots->ptr;
+        table.mask = cap - 1;
+        table.words = W;
+        for (int j = 0; j < cb::SK_MAX_WORDS; j++) table.nullmask[j] = nullmask[j];
+        launch_join_insert(table, n_runs, st);
+        cuda_check(cudaGetLastError(), "k_join_insert launch");
+        ctx->kernel_launches++;
+        ctx->check_device_errors();
+    }
+
+    // the lookups of probe batch `in`: `total` output rows to emit from it
+    void probe_batch(Batch& in) {
+        TraceSpan ts("join.probe");
+        const int64_t n = in.n_rows;
+        if (n >= ((int64_t)1 << 32)) throw Unsupported("a hash join probe batch of 2^32 rows or more");
+        cudaStream_t st = ctx->stream;
+        uint64_t h_and_or[2 * cb::SK_MAX_WORDS];
+        std::vector<int> digits;
+        DeviceBufP pk = pack_row_keys(key_cols(in, probe_keys, false), n, bits, ctx, h_and_or, digits);
+        probe = std::move(in);
+        pos = 0;
+        if (type == JoinType::Inner) {
+            const size_t n_chunks = (size_t)(n + CB_SCAN_CHUNK - 1) / CB_SCAN_CHUNK;
+            run_of = std::make_shared<DeviceBuf>((size_t)n * 4);
+            offs = std::make_shared<DeviceBuf>((size_t)n * 4);
+            chunk_off = std::make_shared<DeviceBuf>((n_chunks + 1) * 4);
+            auto tot = std::make_shared<DeviceBuf>(16);
+            cuda_check(cudaMemsetAsync(tot->ptr, 0, 16, st), "memset join total");
+            launch_join_probe(table, (const unsigned long long*)pk->ptr, n, CB_JOIN_COUNT, (unsigned*)offs->ptr, (unsigned*)run_of->ptr,
+                              (unsigned long long*)tot->ptr, nullptr, st);
+            launch_scan_u32((unsigned*)offs->ptr, n, CB_SCAN_CHUNK, (unsigned*)chunk_off->ptr, (long long*)tot->ptr + 1, st);
+            cuda_check(cudaGetLastError(), "join probe");
+            ctx->kernel_launches += 3;
+            cuda_check(cudaMemcpyAsync(&total, tot->ptr, 8, cudaMemcpyDeviceToHost, st), "D2H join total");
+            ctx->check_device_errors();
+            // the scan's offsets are 32-bit
+            if (total >= ((int64_t)1 << 32)) throw Unsupported("a probe batch whose inner join output has 2^32 rows or more (lower spark.comet.b200.chunkRows)");
+        } else {
+            const size_t nb = (size_t)(n + 1023) / 1024;
+            auto keep = std::make_shared<DeviceBuf>((size_t)n + 16), iota = std::make_shared<DeviceBuf>((size_t)n * 4);
+            auto counts = std::make_shared<DeviceBuf>(nb * 4 + 4), offsets = std::make_shared<DeviceBuf>(nb * 8 + 8), kept = std::make_shared<DeviceBuf>(8);
+            kept_rows = std::make_shared<DeviceBuf>((size_t)n * 4);
+            launch_join_probe(table, (const unsigned long long*)pk->ptr, n, type == JoinType::LeftSemi ? CB_JOIN_SEMI : CB_JOIN_ANTI, nullptr, nullptr, nullptr,
+                              (unsigned char*)keep->ptr, st);
+            launch_compact_plan((const unsigned char*)keep->ptr, n, (int*)counts->ptr, (long long*)offsets->ptr, (long long*)kept->ptr, st);
+            launch_sort_iota((unsigned*)iota->ptr, n, st);
+            launch_compact_scatter((const unsigned char*)keep->ptr, n, (const long long*)offsets->ptr, iota->ptr, 4, kept_rows->ptr, st);
+            cuda_check(cudaGetLastError(), "join probe");
+            ctx->kernel_launches += 5;
+            cuda_check(cudaMemcpyAsync(&total, kept->ptr, 8, cudaMemcpyDeviceToHost, st), "D2H join kept rows");
+            ctx->check_device_errors();
+        }
+    }
+
+    // the next at most chunkRows output rows of the probe batch
+    void emit(Batch& out) {
+        const int64_t k = std::min<int64_t>(total - pos, std::max<int64_t>(ctx->chunk_rows, 1));
+        if (type == JoinType::Inner) {
+            auto pidx = std::make_shared<DeviceBuf>((size_t)k * 4), bidx = std::make_shared<DeviceBuf>((size_t)k * 4);
+            launch_join_emit(table, (const unsigned*)run_of->ptr, (const unsigned*)offs->ptr, (const unsigned*)chunk_off->ptr, probe.n_rows, pos, pos + k,
+                             (unsigned*)pidx->ptr, (unsigned*)bidx->ptr, ctx->stream);
+            cuda_check(cudaGetLastError(), "k_join_emit launch");
+            ctx->kernel_launches++;
+            Batch pb, bb;
+            gather_columns(probe, (const unsigned*)pidx->ptr, k, pb, ctx, "joining");
+            gather_columns(build, (const unsigned*)bidx->ptr, k, bb, ctx, "joining");
+            Batch& l = build_left ? bb : pb;
+            Batch& r = build_left ? pb : bb;
+            out.n_rows = k;
+            out.cols = std::move(l.cols);
+            for (auto& c : r.cols) out.cols.push_back(std::move(c));
+        } else {
+            gather_columns(probe, (const unsigned*)kept_rows->ptr + pos, k, out, ctx, "joining");
+        }
+        pos += k;
+        ctx->join_out_rows += k;
+        ctx->check_device_errors();
+        if (pos >= total) { probe = Batch(); run_of.reset(); offs.reset(); chunk_off.reset(); kept_rows.reset(); }
+    }
+
+    bool next(Batch& out) override {
+        if (!built) build_table();
+        const bool empty_build = build.n_rows == 0;
+        if (empty_build && type != JoinType::LeftAnti) return false; // nothing matches
+        for (;;) {
+            if (pos < total) { emit(out); return true; }
+            Batch in;
+            if (!probe_child->next(in)) return false;
+            arrive(in);
+            ctx->join_probe_rows += in.n_rows;
+            if (in.n_rows == 0) continue;
+            if (empty_build) { // anti: every probe row
+                ctx->join_out_rows += in.n_rows;
+                out = std::move(in);
+                return true;
+            }
+            probe_batch(in);
+        }
     }
 };
 
@@ -1232,6 +1509,28 @@ static ExecNodeP build_node(const OperatorP& op, ExecContext* ctx, PlanInputs* i
             if (k.expr->index < 0 || k.expr->index >= (int)cur->schema.size()) throw PlanError("sort key out of range");
         return n;
     }
+    if (cur->kind == OpKind::HashJoin) {
+        auto n = std::make_shared<JoinNode>();
+        n->ctx = ctx;
+        ExecNodeP left = build_node(cur->children[0], ctx, inputs, build_only, assume); // inputs are taken in Scan order: left first
+        ExecNodeP right = build_node(cur->children[1], ctx, inputs, build_only, assume);
+        n->schema = cur->schema;
+        n->type = cur->join_type;
+        n->build_left = cur->build_left;
+        std::vector<int> lk, rk;
+        std::vector<DType> key_types;
+        for (size_t i = 0; i < cur->left_keys.size(); i++) {
+            lk.push_back(cur->left_keys[i]->index);
+            rk.push_back(cur->right_keys[i]->index);
+            key_types.push_back(cur->left_keys[i]->type);
+        }
+        n->build_child = cur->build_left ? left : right;
+        n->probe_child = cur->build_left ? right : left;
+        n->build_keys = cur->build_left ? lk : rk;
+        n->probe_keys = cur->build_left ? rk : lk;
+        n->set_layout(key_types);
+        return n;
+    }
     if (cur->kind == OpKind::HashAgg) { agg_op = cur; cur = cur->children[0]; }
     std::vector<OperatorP> chain; // top-down
     while (cur->kind == OpKind::Filter || cur->kind == OpKind::Projection) { chain.push_back(cur); cur = cur->children[0]; }
@@ -1270,20 +1569,28 @@ static ExecNodeP build_node(const OperatorP& op, ExecContext* ctx, PlanInputs* i
 
 ExecNodeP build_exec(const OperatorP& op, ExecContext* ctx, PlanInputs* inputs) { return build_node(op, ctx, inputs, false, {}); }
 
-std::vector<GeneratedKernel> plan_kernels_for_build(const OperatorP& op, const std::vector<int>& assume) {
-    ExecContext defaults; // build-time tuning: the defaults (constructing one makes no CUDA call)
-    std::vector<GeneratedKernel> out;
-    for (ExecNodeP n = build_node(op, &defaults, nullptr, true, assume); n;) {
+// the pipeline kernels of the tree under n, top-down; a join's left child before its right one
+static void collect_kernels(ExecNodeP n, std::vector<GeneratedKernel>& out) {
+    while (n) {
         if (auto f = std::dynamic_pointer_cast<FusedBase>(n)) {
             for (const PipelineSpec& s : f->build_specs()) out.push_back(generate_pipeline(s));
             n = f->child;
         } else if (auto pn = std::dynamic_pointer_cast<PartitionNode>(n)) {
             n = pn->child;
+        } else if (auto jn = std::dynamic_pointer_cast<JoinNode>(n)) {
+            collect_kernels(jn->build_left ? jn->build_child : jn->probe_child, out);
+            n = jn->build_left ? jn->probe_child : jn->build_child;
         } else {
             auto sn = std::dynamic_pointer_cast<SortNode>(n);
             n = sn ? sn->child : nullptr;
         }
     }
+}
+
+std::vector<GeneratedKernel> plan_kernels_for_build(const OperatorP& op, const std::vector<int>& assume) {
+    ExecContext defaults; // build-time tuning: the defaults (constructing one makes no CUDA call)
+    std::vector<GeneratedKernel> out;
+    collect_kernels(build_node(op, &defaults, nullptr, true, assume), out);
     return out;
 }
 

@@ -74,6 +74,11 @@ class Dictionary {
         index_.emplace(v, (int32_t)values_.size()); // no-op for a repeat: intern keeps finding the first
         values_.push_back(std::move(v));
     }
+    // the code of the first entry equal to v, or -1 when there is none (nothing is added)
+    int32_t find(const std::string& v) const {
+        auto it = index_.find(v);
+        return it == index_.end() ? -1 : it->second;
+    }
 
   private:
     std::vector<std::string> values_;
@@ -132,6 +137,7 @@ struct ExecContext {
     int64_t agg_strategies = 0;   // CB200_AGG_* bits of the aggregate strategies that ran
     int64_t sort_rows = 0, sort_passes = 0, sort_pass_rows = 0; // rows Sort operators radix-sorted, the digit passes they ran, rows moved
     int64_t sort_select_rows = 0; // rows TopK's radix select read (one read per digit step)
+    int64_t join_build_rows = 0, join_probe_rows = 0, join_out_rows = 0; // hash joins: rows drained from the build side, rows probed, rows out
     std::vector<int64_t> partition_starts; // last ShuffleWriter batch: partition p = rows [starts[p], starts[p+1])
     void check_device_errors();
     void collect_timing();

@@ -790,6 +790,52 @@ static OperatorP decode_operator(PbReader r) { // Operator operator.proto:32-86
         have = true;
         break;
     }
+    case 109: { // HashJoin operator.proto:754-763 (planner.rs:2192-2266: HashJoinExec with NullEqualsNothing; BuildRight swaps the inputs)
+        op->kind = OpKind::HashJoin;
+        bool condition = false, null_aware = false;
+        int64_t join_type = 0, build_side = 0;
+        while (b.next()) {
+            if (b.field == 1 && b.wire == 2) op->left_keys.push_back(decode_expr(b.sub()));
+            else if (b.field == 2 && b.wire == 2) op->right_keys.push_back(decode_expr(b.sub()));
+            else if (b.field == 3) join_type = b.i64();
+            else if (b.field == 4) { condition = true; b.skip(); }
+            else if (b.field == 5) build_side = b.i64();
+            else if (b.field == 6) null_aware = b.i64() != 0;
+            else b.skip();
+        }
+        if (op->children.size() != 2) throw PlanError("hash join expects two children");
+        if (op->left_keys.empty()) throw PlanError("hash join without keys");
+        if (op->left_keys.size() != op->right_keys.size())
+            throw PlanError("hash join with " + std::to_string(op->left_keys.size()) + " left keys and " + std::to_string(op->right_keys.size()) + " right keys");
+        if (join_type < 0 || join_type > 5) throw PlanError("unknown join type " + std::to_string(join_type));
+        if (build_side != 0 && build_side != 1) throw PlanError("unknown build side " + std::to_string(build_side));
+        op->join_type = (JoinType)join_type;
+        op->build_left = build_side == 0;
+        const bool semi_anti = op->join_type == JoinType::LeftSemi || op->join_type == JoinType::LeftAnti;
+        if (op->join_type != JoinType::Inner && !semi_anti) throw Unsupported("outer hash joins (only inner, left semi and left anti)");
+        if (semi_anti && op->build_left) throw Unsupported("left semi / anti hash join with BuildLeft (only BuildRight)");
+        if (condition) throw Unsupported("hash join with a join condition");
+        if (null_aware) throw Unsupported("null-aware anti join (NOT IN)");
+        if (op->left_keys.size() > MAX_SORT_KEYS) throw Unsupported("more than 8 hash join keys");
+        const auto &ls = op->children[0]->schema, &rs = op->children[1]->schema;
+        int bits = 0;
+        for (size_t i = 0; i < op->left_keys.size(); i++) {
+            Expr &l = *op->left_keys[i], &r = *op->right_keys[i];
+            resolve(l, ls);
+            resolve(r, rs);
+            if (l.kind != ExprKind::Bound || r.kind != ExprKind::Bound)
+                throw Unsupported("computed hash join keys (only plain column keys: put a Projection below the join)");
+            if (l.type != r.type) throw PlanError("hash join key " + std::to_string(i) + " is " + l.type.str() + " on the left and " + r.type.str() + " on the right");
+            if (l.type.is_float()) throw Unsupported("hash join key of type " + l.type.str() + " (Spark normalises NaN and -0.0 in float keys)");
+            if (l.type.id == TypeId::Binary) throw Unsupported("hash join key of type binary");
+            bits += sort_key_bits(l.type) + 1; // the sort's key encoding: one null bit per key
+        }
+        if (bits > MAX_SORT_KEY_BITS) throw Unsupported("hash join keys of " + std::to_string(bits) + " bits (at most 256 bits of packed key)");
+        op->schema = ls;
+        if (!semi_anti) op->schema.insert(op->schema.end(), rs.begin(), rs.end());
+        have = true;
+        break;
+    }
     default:
         throw Unsupported("operator field " + std::to_string(f) + " is outside the GPU hot path");
     }

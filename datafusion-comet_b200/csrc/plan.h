@@ -105,7 +105,10 @@ struct AggExpr {
     int state_at = -1;
 };
 
-enum class OpKind { Scan, ShuffleScan, NativeScan, Projection, Filter, HashAgg, ShuffleWriter, Sort };
+enum class OpKind { Scan, ShuffleScan, NativeScan, Projection, Filter, HashAgg, ShuffleWriter, Sort, HashJoin };
+
+// operator.proto JoinType / BuildSide
+enum class JoinType : int { Inner = 0, LeftOuter = 1, RightOuter = 2, FullOuter = 3, LeftSemi = 4, LeftAnti = 5 };
 
 // one ORDER BY key (SortOrder expr.proto:385-389, planner.rs:927-950 create_sort_expr): arrow SortOptions{descending, nulls_first}
 struct SortKey {
@@ -152,6 +155,11 @@ struct Operator {
     // -1 = the field is absent
     std::vector<SortKey> sort_keys;
     int64_t fetch = -1, skip = -1;
+    // HashJoin (operator.proto:754-763): equi-join on Bound key columns of children[0] (left) and children[1] (right).  Inner: the
+    // output is the left columns, then the right ones; LeftSemi / LeftAnti: the left columns.
+    std::vector<ExprP> left_keys, right_keys;
+    JoinType join_type = JoinType::Inner;
+    bool build_left = false; // BuildLeft: the left child is the build side (the hash table), the right one is probed
 };
 
 // Sort keys at most: 8 keys, 256 bits of packed key (value bits by declared type plus one null bit per key, sort_key_bits)

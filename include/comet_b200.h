@@ -193,6 +193,9 @@ typedef struct cb200_stats {
     int64_t sort_passes;       /* radix passes they ran: one per 8-bit key digit that is not the same in every row */
     int64_t sort_pass_rows;    /* rows those passes moved, summed over the passes */
     int64_t sort_select_rows;  /* rows TopK's radix select read, summed over its digit steps */
+    int64_t join_build_rows;   /* rows HashJoin operators drained from their build side into the hash table's input */
+    int64_t join_probe_rows;   /* probe-side rows they looked up */
+    int64_t join_out_rows;     /* rows they emitted */
 } cb200_stats;
 #define CB200_AGG_DENSE 1      /* thread-private accumulators over dictionary / bool key codes (and ungrouped aggregates) */
 #define CB200_AGG_TABLE 2      /* global key table */
