@@ -78,9 +78,7 @@ struct DenseState {
             }
             memcpy(&newt[(size_t)ng * n_words * 2], &oldt[(size_t)g * n_words * 2], (size_t)n_words * 16);
         }
-        totals = std::make_shared<DeviceBuf>(newt.size() * 8);
-        cuda_check(cudaMemcpyAsync(totals->ptr, newt.data(), newt.size() * 8, cudaMemcpyHostToDevice, ctx->stream), "regroup H2D");
-        cuda_check(cudaStreamSynchronize(ctx->stream), "regroup sync");
+        totals = host_to_device(newt.data(), newt.size() * 8, ctx, "regroup H2D");
         groups = new_groups;
     }
 

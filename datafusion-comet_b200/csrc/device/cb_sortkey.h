@@ -14,7 +14,7 @@
 #define CB_SORTKEY_H
 #include "cb_math.h"
 
-// The layout of a key column, as the sources store it (exec.cpp key_kind): shared by hash partitioning and the sort.
+// The layout of a key column, as the sources store it (rows.cpp key_kind): shared by hash partitioning, the sort and the join.
 // HK_BOOL reads an Arrow bitmap, HK_BOOL8 one byte per row; HK_I32 also serves INT32-backed int8 / int16; HK_DEC_SMALL_32 is a
 // decimal(p <= 9) stored as INT32, HK_DEC_SMALL_64 (= HK_I64) / HK_DEC_LARGE_64 decimals stored in 8 bytes, *_128 in 16 bytes;
 // HK_DICT* are dictionary codes of 1, 2 or 4 bytes, HK_UTF8 plain offsets + chars.

@@ -2,7 +2,7 @@
 //
 // The reference writes the rows of every output partition as IPC blocks to local files and the reduce side fetches them
 // (native/shuffle/src/partitioners/multi_partition.rs:265-330 + Spark's block transfer).  With one process per GPU on one box the
-// same rows travel over NVLink / NVSwitch instead: the map side (PartitionNode, exec.cpp) leaves every column reordered by
+// same rows travel over NVLink / NVSwitch instead: the map side (PartitionNode, partition.cpp) leaves every column reordered by
 // partition id on the device, and cb200_exchange moves segment p of every column to rank p --
 //   counts : one ncclAllGather of the N x N row-count matrix (the "map status" Spark's driver would collect)
 //   payload: ONE ncclGroup of N sends + N receives per column buffer, straight out of the map plan's device buffers into the buffers

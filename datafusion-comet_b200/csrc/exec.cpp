@@ -1,10 +1,7 @@
-// exec.cpp -- executor: sources, filter / projection pipelines, hash repartitioning, plan building, Arrow export.
-// Aggregation is in agg.cpp.
+// exec.cpp -- executor: sources, filter / projection pipelines, plan building, Arrow export.
+// Aggregation is in agg.cpp; repartitioning, Sort and HashJoin are in partition.cpp, sort.cpp and join.cpp over rows.cpp.
 #include "exec_internal.h"
 
-#include "aot_kernels.h"
-
-#include <algorithm>
 #include <cstdlib>
 #include <ctime>
 #include <mutex>
@@ -235,8 +232,7 @@ DeviceBufP bytes_to_bitmap(const DeviceBufP& bytes, int64_t n, ExecContext* ctx)
     return bits;
 }
 
-// n bytes (nonzero = set) as a host bitmap, 8 bytes of slack behind it
-static std::vector<uint8_t> pack_bits(const uint8_t* bytes, size_t n) {
+std::vector<uint8_t> pack_bits(const uint8_t* bytes, size_t n) {
     std::vector<uint8_t> out((n + 7) / 8 + 8, 0);
     for (size_t i = 0; i < n; i++) if (bytes[i]) out[i >> 3] |= (uint8_t)(1u << (i & 7));
     return out;
@@ -420,10 +416,9 @@ struct StreamSource : ExecNode {
                         cuda_check(h2d(tmp->ptr, src, (size_t)ch->length * w), "H2D dict codes");
                         std::vector<int32_t> table = remaps[k];
                         if (table.empty()) { table.resize((size_t)ch->dictionary->length); for (size_t i = 0; i < table.size(); i++) table[i] = (int32_t)i; }
-                        auto dt = std::make_shared<DeviceBuf>(table.size() * 4 + 4);
+                        DeviceBufP dt = host_to_device(table.data(), table.size() * 4, ctx, "H2D remap table");
+                        ctx->h2d_bytes += (int64_t)(table.size() * 4);
                         temps.push_back(dt);
-                        cuda_check(h2d(dt->ptr, table.data(), table.size() * 4), "H2D remap table");
-                        cuda_check(cudaStreamSynchronize(st), "remap table copy"); // table is a stack temporary
                         launch_remap_codes(tmp->ptr, w, ch->length, (const int*)dt->ptr, (int)table.size(), (int*)col.data->ptr + row, st);
                     }
                     row += ch->length;
@@ -437,7 +432,6 @@ struct StreamSource : ExecNode {
                     total_chars += off[ch->length] - off[0];
                 }
                 if (total_chars > INT32_MAX) throw Unsupported("more than 2 GiB of string data in one chunk");
-                col.offsets = std::make_shared<DeviceBuf>((size_t)(total + 1) * 4);
                 col.chars = std::make_shared<DeviceBuf>((size_t)total_chars + 16);
                 std::vector<int32_t> offs((size_t)total + 1);
                 int64_t row = 0;
@@ -452,8 +446,8 @@ struct StreamSource : ExecNode {
                     row += ch->length;
                 }
                 offs[(size_t)total] = base;
-                cuda_check(h2d(col.offsets->ptr, offs.data(), offs.size() * 4), "H2D offsets");
-                cuda_check(cudaStreamSynchronize(st), "offsets copy");
+                col.offsets = host_to_device(offs.data(), offs.size() * 4, ctx, "H2D offsets");
+                ctx->h2d_bytes += (int64_t)(offs.size() * 4);
                 col.phys = Phys::I32;
             } else {
                 col.phys = phys_of(schema[c]);
@@ -721,723 +715,6 @@ struct SelectNode : FusedBase {
     }
 };
 
-
-// =================================================================================================
-// hash repartitioning (ShuffleWriterExec with HashPartition, native/shuffle/src/partitioners/multi_partition.rs)
-// =================================================================================================
-// The HK_* kind of a key column (device/cb_sortkey.h), for hash partitioning and the sort.  The logical type decides how Spark hashes
-// a value (utils.rs: i8 / i16 / i32 / date as i32, decimal(p <= 18) as i64, wider decimals as 16 bytes) and how many bits its sort key
-// takes; the stored layout (DESIGN.md, "Data layout in HBM") decides how it is read.
-static int key_kind(const Column& c) {
-    const Phys ph = c.phys;
-    switch (c.type.id) {
-    case TypeId::Bool: return ph == Phys::Bitmap ? HK_BOOL : HK_BOOL8;
-    case TypeId::Int8: return ph == Phys::I32 ? HK_I32 : HK_I8; // sign-extended to i32 either way
-    case TypeId::Int16: return ph == Phys::I32 ? HK_I32 : HK_I16;
-    case TypeId::Int32: case TypeId::Date: return HK_I32;
-    case TypeId::Int64: case TypeId::Timestamp: case TypeId::TimestampNtz: return HK_I64;
-    case TypeId::Float32: return HK_F32;
-    case TypeId::Float64: return HK_F64;
-    case TypeId::Decimal:
-        if (ph == Phys::I32) return HK_DEC_SMALL_32;
-        if (ph == Phys::I64) return c.type.precision <= 18 ? HK_DEC_SMALL_64 : HK_DEC_LARGE_64;
-        return c.type.precision <= 18 ? HK_DEC_SMALL_128 : HK_DEC_LARGE_128;
-    case TypeId::String: case TypeId::Binary:
-        if (!c.is_dict) return HK_UTF8;
-        return ph == Phys::I8 ? HK_DICT8 : ph == Phys::I16 ? HK_DICT16 : HK_DICT32;
-    default: throw Unsupported("hash partitioning on " + c.type.str());
-    }
-}
-
-// small host-resident aggregate results -> device columns
-static void columns_to_device(Batch& b, ExecContext* ctx) {
-    for (auto& c : b.cols) {
-        if (!c.on_host) continue;
-        size_t n = (size_t)b.n_rows;
-        if (c.type.is_string()) { // dictionary-encode on the host: these are group keys of a dense aggregate (a handful of rows)
-            auto d = std::make_shared<Dictionary>();
-            std::vector<int32_t> codes(n);
-            for (size_t r = 0; r < n; r++)
-                codes[r] = d->intern(std::string((const char*)c.h_data.data() + c.h_offsets[r], (size_t)(c.h_offsets[r + 1] - c.h_offsets[r])));
-            c.data = std::make_shared<DeviceBuf>(n * 4 + 16);
-            if (n) cuda_check(cudaMemcpyAsync(c.data->ptr, codes.data(), n * 4, cudaMemcpyHostToDevice, ctx->stream), "keys H2D");
-            cuda_check(cudaStreamSynchronize(ctx->stream), "keys H2D sync");
-            c.is_dict = true; c.dict = d; c.phys = Phys::I32;
-        } else if (c.type.id == TypeId::Bool) {
-            std::vector<uint8_t> bits = pack_bits(c.h_data.data(), n);
-            c.data = std::make_shared<DeviceBuf>(bits.size());
-            cuda_check(cudaMemcpyAsync(c.data->ptr, bits.data(), bits.size(), cudaMemcpyHostToDevice, ctx->stream), "bool H2D");
-            cuda_check(cudaStreamSynchronize(ctx->stream), "bool H2D sync");
-            c.phys = Phys::Bitmap;
-        } else {
-            c.data = std::make_shared<DeviceBuf>(c.h_data.size() + 16);
-            if (!c.h_data.empty()) cuda_check(cudaMemcpyAsync(c.data->ptr, c.h_data.data(), c.h_data.size(), cudaMemcpyHostToDevice, ctx->stream), "col H2D");
-            cuda_check(cudaStreamSynchronize(ctx->stream), "col H2D sync");
-            c.phys = phys_of(c.type);
-        }
-        if (!c.h_valid.empty()) {
-            std::vector<uint8_t> bits = pack_bits(c.h_valid.data(), n);
-            c.validity = std::make_shared<DeviceBuf>(bits.size());
-            cuda_check(cudaMemcpyAsync(c.validity->ptr, bits.data(), bits.size(), cudaMemcpyHostToDevice, ctx->stream), "validity H2D");
-            cuda_check(cudaStreamSynchronize(ctx->stream), "validity H2D sync");
-        }
-        c.on_host = false;
-    }
-}
-
-// out's columns = in's rows row_idx[0, n), in that order.  Bit-packed booleans and validity are gathered one byte per row and repacked
-// (the byte forms are kept: the exchange sends them).  `op` names the operator in the refusal of plain Utf8 columns.
-template <typename I> static void gather_columns(const Batch& in, const I* row_idx, int64_t n, Batch& out, ExecContext* ctx, const char* op) {
-    cudaStream_t st = ctx->stream;
-    out.n_rows = n;
-    out.cols.clear();
-    for (auto& c : in.cols) {
-        Column o = c;
-        if (c.offsets) throw Unsupported(std::string(op) + " plain string columns (dictionary-encode them first)");
-        int w = phys_bytes(c.phys);
-        if (w == 0) { // bit-packed booleans: gather to bytes, repack
-            auto bytes = std::make_shared<DeviceBuf>((size_t)n + 16);
-            launch_gather_bits(c.data->ptr, row_idx, n, bytes->ptr, st);
-            ctx->kernel_launches++;
-            o.data = bytes_to_bitmap(bytes, n, ctx);
-            o.bool_bytes = bytes;
-        } else {
-            o.data = std::make_shared<DeviceBuf>((size_t)std::max<int64_t>(n, 1) * w);
-            launch_gather(c.data->ptr, w, row_idx, n, o.data->ptr, st);
-            ctx->kernel_launches++;
-            if (c.type.id == TypeId::Bool) o.bool_bytes = o.data; // aggregate outputs keep booleans one byte per row
-        }
-        if (c.validity) {
-            auto bytes = std::make_shared<DeviceBuf>((size_t)n + 16);
-            launch_gather_bits(c.validity->ptr, row_idx, n, bytes->ptr, st);
-            ctx->kernel_launches++;
-            o.validity = bytes_to_bitmap(bytes, n, ctx);
-            o.valid_bytes = bytes;
-        }
-        out.cols.push_back(o);
-    }
-    cuda_check(cudaGetLastError(), "gathers");
-}
-
-// Output: the child's rows reordered so that partition p occupies rows [starts[p], starts[p+1]) -- what the
-// reference writes as per-partition IPC blocks, kept on the device for the NVLink exchange.
-struct PartitionNode : ExecNode {
-    ExecContext* ctx;
-    ExecNodeP child;
-    std::vector<int> key_cols;
-    int n_parts = 1;
-
-    bool next(Batch& out) override {
-        Batch in;
-        if (!child->next(in)) return false;
-        TraceSpan ts("partition");
-        columns_to_device(in, ctx);
-        int64_t n = in.n_rows;
-        cudaStream_t st = ctx->stream;
-        HashKeyCols kc;
-        memset(&kc, 0, sizeof(kc));
-        std::vector<DeviceBufP> keep;
-        for (int ci : key_cols) {
-            const Column& c = in.cols[(size_t)ci];
-            HashKeyCol& k = kc.col[kc.n++];
-            k.data = c.data ? c.data->ptr : nullptr;
-            k.validity = c.validity ? (const unsigned char*)c.validity->ptr : nullptr;
-            k.kind = key_kind(c);
-            switch (k.kind) {
-            case HK_DICT8: case HK_DICT16: case HK_DICT32: {
-                std::vector<int32_t> off{0};
-                std::string chars;
-                for (auto& v : c.dict->values()) { chars += v; off.push_back((int32_t)chars.size()); }
-                auto doff = std::make_shared<DeviceBuf>(off.size() * 4), dch = std::make_shared<DeviceBuf>(chars.size() + 16);
-                cuda_check(cudaMemcpyAsync(doff->ptr, off.data(), off.size() * 4, cudaMemcpyHostToDevice, st), "dict offsets");
-                if (!chars.empty()) cuda_check(cudaMemcpyAsync(dch->ptr, chars.data(), chars.size(), cudaMemcpyHostToDevice, st), "dict chars");
-                cuda_check(cudaStreamSynchronize(st), "dict upload");
-                keep.push_back(doff); keep.push_back(dch);
-                k.dict_offsets = (const int*)doff->ptr;
-                k.dict_chars = (const unsigned char*)dch->ptr;
-                break;
-            }
-            case HK_UTF8:
-                if (!c.offsets || !c.chars) throw Unsupported("string partition key without offsets/chars");
-                k.dict_offsets = (const int*)c.offsets->ptr;
-                k.dict_chars = (const unsigned char*)c.chars->ptr;
-                break;
-            default: break;
-            }
-        }
-        size_t nb = (size_t)(n + 1023) / 1024 + 1;
-        auto pids = std::make_shared<DeviceBuf>((size_t)n * 4 + 16);
-        auto hist = std::make_shared<DeviceBuf>(nb * n_parts * 4);
-        auto base = std::make_shared<DeviceBuf>(nb * n_parts * 8);
-        auto starts = std::make_shared<DeviceBuf>((size_t)(n_parts + 1) * 8);
-        auto row_idx = std::make_shared<DeviceBuf>((size_t)n * 8 + 16);
-        cuda_check(cudaMemsetAsync(starts->ptr, 0, (size_t)(n_parts + 1) * 8, st), "memset starts");
-        auto chunk_tmp = std::make_shared<DeviceBuf>((size_t)(partition_chunks(n) + 1) * n_parts * 8);
-        cuda_check(launch_partition(kc, n, (unsigned)n_parts, nullptr, (unsigned*)pids->ptr, (int*)hist->ptr, (long long*)base->ptr, (long long*)chunk_tmp->ptr,
-                                    (long long*)starts->ptr, (long long*)row_idx->ptr, st), "partition launches");
-        ctx->kernel_launches += 6;
-        gather_columns(in, (const long long*)row_idx->ptr, n, out, ctx, "repartitioning");
-        ctx->partition_starts.assign((size_t)n_parts + 1, 0);
-        cuda_check(cudaMemcpyAsync(ctx->partition_starts.data(), starts->ptr, (size_t)(n_parts + 1) * 8, cudaMemcpyDeviceToHost, st), "starts D2H"); ctx->d2h_bytes += (int64_t)((size_t)(n_parts + 1) * 8);
-        ctx->check_device_errors();
-        return true;
-    }
-};
-
-// ---- shared by Sort and HashJoin -------------------------------------------------------------------------------------------------
-// the rows of bs in one batch (`bs` non-empty, every batch on the device): values and validity appended in order; dictionary-coded strings
-// that carry different Dictionary objects are recoded into one (the first batch's entries, then the others' new entries)
-static Batch concat_batches(const std::vector<Batch>& bs, ExecContext* ctx, const char* op) {
-    cudaStream_t st = ctx->stream;
-    Batch out;
-    for (auto& b : bs) out.n_rows += b.n_rows;
-    const size_t n = (size_t)out.n_rows;
-    std::vector<DeviceBufP> temps;
-    for (size_t j = 0; j < bs[0].cols.size(); j++) {
-        const Column& c0 = bs[0].cols[j];
-        Column o;
-        o.type = c0.type;
-        o.phys = c0.phys;
-        o.is_dict = c0.is_dict;
-        o.dict = c0.dict;
-        bool same = true, nulls = false;
-        for (auto& b : bs) {
-            const Column& c = b.cols[j];
-            if (c.phys != c0.phys || c.dict != c0.dict || c.is_dict != c0.is_dict) same = false;
-            if (c.validity) nulls = true;
-        }
-        if (!same && !c0.is_dict) throw Unsupported(std::string(op) + " input whose batches store column " + std::to_string(j) + " in different layouts");
-        if (same) {
-            const int w = phys_bytes(c0.phys);
-            o.data = std::make_shared<DeviceBuf>(w == 0 ? bitmap_bytes((int64_t)n) : std::max<size_t>(n, 1) * (size_t)w);
-            if (w == 0) cuda_check(cudaMemsetAsync(o.data->ptr, 0, o.data->bytes, st), "memset bools");
-            int64_t row = 0;
-            for (auto& b : bs) {
-                const Column& c = b.cols[j];
-                if (w == 0) { launch_bitmap_append((uint32_t*)o.data->ptr, row, (const uint8_t*)c.data->ptr, 0, b.n_rows, st); ctx->kernel_launches++; }
-                else cuda_check(cudaMemcpyAsync((char*)o.data->ptr + (size_t)row * w, c.data->ptr, (size_t)b.n_rows * w, cudaMemcpyDeviceToDevice, st), "concat column");
-                row += b.n_rows;
-            }
-        } else { // dictionary codes -> int32 codes of one dictionary
-            auto d = std::make_shared<Dictionary>(*c0.dict);
-            o.phys = Phys::I32;
-            o.dict = d;
-            o.data = std::make_shared<DeviceBuf>(std::max<size_t>(n, 1) * 4);
-            int64_t row = 0;
-            for (auto& b : bs) {
-                const Column& c = b.cols[j];
-                const std::vector<std::string>& vals = c.dict->values();
-                std::vector<int32_t> table(vals.size());
-                for (size_t k = 0; k < table.size(); k++) table[k] = c.dict == c0.dict ? (int32_t)k : d->intern(vals[k]);
-                auto dt = std::make_shared<DeviceBuf>(table.size() * 4 + 4);
-                temps.push_back(dt);
-                if (!table.empty()) cuda_check(cudaMemcpyAsync(dt->ptr, table.data(), table.size() * 4, cudaMemcpyHostToDevice, st), "H2D remap table");
-                cuda_check(cudaStreamSynchronize(st), "remap table copy"); // table is a loop temporary
-                launch_remap_codes(c.data->ptr, phys_bytes(c.phys), b.n_rows, (const int*)dt->ptr, (int)table.size(), (int*)o.data->ptr + row, st);
-                ctx->kernel_launches++;
-                row += b.n_rows;
-            }
-        }
-        if (nulls) {
-            o.validity = std::make_shared<DeviceBuf>(bitmap_bytes((int64_t)n));
-            cuda_check(cudaMemsetAsync(o.validity->ptr, 0, o.validity->bytes, st), "memset validity");
-            int64_t row = 0;
-            for (auto& b : bs) {
-                const Column& c = b.cols[j];
-                launch_bitmap_append((uint32_t*)o.validity->ptr, row, c.validity ? (const uint8_t*)c.validity->ptr : nullptr, 0, b.n_rows, st);
-                ctx->kernel_launches++;
-                row += b.n_rows;
-            }
-            o.null_count = -1;
-        }
-        out.cols.push_back(o);
-    }
-    cuda_check(cudaGetLastError(), "concat launches");
-    return out;
-}
-
-// the stable order of m rows whose keys (`words` words each) are in keys0, by the given digits: row indices [0, m); `sorted_keys`, if
-// given, receives the keys in that order
-static DeviceBufP radix_order(ExecContext* ctx, DeviceBufP keys0, int words, int64_t m, const std::vector<int>& digits, DeviceBufP* sorted_keys = nullptr) {
-    cudaStream_t st = ctx->stream;
-    const int64_t nt = sort_tiles(m);
-    auto keys1 = std::make_shared<DeviceBuf>((size_t)m * words * 8);
-    auto idx0 = std::make_shared<DeviceBuf>((size_t)m * 4), idx1 = std::make_shared<DeviceBuf>((size_t)m * 4);
-    auto hist = std::make_shared<DeviceBuf>((size_t)nt * 256 * 4), chunk_off = std::make_shared<DeviceBuf>((size_t)(nt * 256 / 4096 + 2) * 4);
-    auto total = std::make_shared<DeviceBuf>(8);
-    RadixScratch s{{(unsigned long long*)keys0->ptr, (unsigned long long*)keys1->ptr}, {(unsigned*)idx0->ptr, (unsigned*)idx1->ptr},
-                   (unsigned*)hist->ptr, (unsigned*)chunk_off->ptr, (long long*)total->ptr};
-    int r = 0;
-    cuda_check(launch_sort_passes(s, words, m, digits.data(), (int)digits.size(), &r, st), "sort passes");
-    ctx->kernel_launches += digits.empty() ? 1 : 4 * (int64_t)digits.size();
-    if (sorted_keys) *sorted_keys = r ? keys1 : keys0;
-    return r ? idx1 : idx0; // the other buffers go back to the stream-ordered pool
-}
-
-// the row keys of kc (kc.words words each) for n rows.  h_and_or[0, W) receives their AND and [W, 2W) their OR, `digits` the 8-bit
-// digits of the `bits`-bit key that are not the same in every row, least significant first.  Synchronises: a dictionary code outside its
-// dictionary fails here.
-static DeviceBufP pack_row_keys(const cb::SortKeyCols& kc, int64_t n, int bits, ExecContext* ctx, uint64_t* h_and_or, std::vector<int>& digits) {
-    cudaStream_t st = ctx->stream;
-    const int W = kc.words;
-    auto keys0 = std::make_shared<DeviceBuf>((size_t)n * W * 8);
-    auto and_or = std::make_shared<DeviceBuf>(2 * cb::SK_MAX_WORDS * 8);
-    cuda_check(cudaMemsetAsync(and_or->ptr, 0xff, (size_t)W * 8, st), "memset key and");
-    cuda_check(cudaMemsetAsync((char*)and_or->ptr + W * 8, 0, (size_t)W * 8, st), "memset key or");
-    launch_sort_keys(kc, n, (unsigned long long*)keys0->ptr, (unsigned long long*)and_or->ptr, st);
-    cuda_check(cudaGetLastError(), "k_sort_keys launch");
-    ctx->kernel_launches++;
-    cuda_check(cudaMemcpyAsync(h_and_or, and_or->ptr, (size_t)W * 16, cudaMemcpyDeviceToHost, st), "D2H key and / or");
-    ctx->check_device_errors(); // also synchronises
-    digits.clear();
-    for (int d = 0; d < (bits + 7) / 8; d++) {
-        const int w = W - 1 - d / 8, sh = (d % 8) * 8;
-        if (((h_and_or[w] ^ h_and_or[W + w]) >> sh) & 0xff) digits.push_back(d);
-    }
-    return keys0;
-}
-
-// =================================================================================================
-// sort (SortExec(LexOrdering).with_fetch(fetch) then GlobalLimitExec(skip), planner.rs:1488-1522)
-// =================================================================================================
-// The output is the child's rows in a stable order of the keys (ties keep the input order: batches as they arrive, rows in order
-// within a batch), rows [skip, fetch).  Without a fetch, or with one above spark.comet.b200.chunkRows, the child is drained and its
-// batches concatenated on the device, sorted once and emitted as one batch.  With a smaller fetch (TopK) at most `fetch` candidate rows
-// are kept between chunks: each chunk is sorted, its first `fetch` rows are sorted together with the candidates (which come first, being
-// earlier input) and the first `fetch` of those become the next candidates, so device memory is bounded by fetch + one chunk.  Keys are
-// built again every round from the columns: a string's rank changes as its dictionary grows.
-struct SortNode : ExecNode {
-    ExecContext* ctx;
-    ExecNodeP child;
-    std::vector<SortKey> keys; // expr: Bound child column
-    int64_t fetch = -1, skip = 0;
-    bool done = false;
-    struct Rank { const Dictionary* dict = nullptr; size_t n = 0; DeviceBufP table; };
-    std::vector<Rank> ranks; // per key: code -> byte-order rank of the dictionary it was built for
-
-    bool topk() const { return fetch >= 0 && fetch <= ctx->chunk_rows; }
-    void count_passes(int64_t m, const std::vector<int>& digits) {
-        ctx->sort_passes += (int64_t)digits.size();
-        ctx->sort_pass_rows += m * (int64_t)digits.size();
-    }
-
-    bool next(Batch& out) override {
-        if (done) return false;
-        done = true;
-        if (fetch == 0) return false;
-        TraceSpan ts("sort");
-        Batch all, in;
-        bool any = false;
-        if (topk()) {
-            while (child->next(in)) {
-                arrive(in);
-                if (in.n_rows == 0) continue;
-                // the chunk's own first `fetch` rows, then those merged behind the candidates (earlier input: first among equal keys)
-                Batch top;
-                sort_rows(in, 0, std::min<int64_t>(fetch, in.n_rows), top);
-                in = Batch();
-                if (any) {
-                    Batch u = concat_batches({all, top}, ctx, "sort");
-                    sort_rows(u, 0, std::min<int64_t>(fetch, u.n_rows), all);
-                } else all = std::move(top);
-                any = true;
-            }
-        } else {
-            std::vector<Batch> batches;
-            while (child->next(in)) {
-                arrive(in);
-                if (in.n_rows > 0) batches.push_back(std::move(in));
-                in = Batch();
-            }
-            any = !batches.empty();
-            if (any) all = batches.size() == 1 ? std::move(batches[0]) : concat_batches(batches, ctx, "sort");
-        }
-        if (!any) return false;
-        const int64_t lo = std::min(skip, all.n_rows), hi = fetch >= 0 ? std::min(fetch, all.n_rows) : all.n_rows;
-        if (hi <= lo) return false;
-        if (topk() && lo == 0) { out = std::move(all); return true; } // the candidates are already in order
-        sort_rows(all, lo, hi, out);
-        return true;
-    }
-
-    void arrive(Batch& b) {
-        columns_to_device(b, ctx);
-        for (auto& c : b.cols)
-            if (c.offsets) throw Unsupported("sorting plain string columns (dictionary-encode them first)");
-    }
-
-    // the code -> rank table of dictionary d: equal strings get equal ranks, ranks follow unsigned byte order.  Rebuilt when the
-    // column carries another dictionary or its dictionary has grown.
-    const uint32_t* rank_table(size_t key, const DictionaryP& d) {
-        Rank& r = ranks[key];
-        const std::vector<std::string>& v = d->values();
-        if (r.table && r.dict == d.get() && r.n == v.size()) return (const uint32_t*)r.table->ptr;
-        std::vector<uint32_t> order(v.size()), rank(v.size() + 1, 0);
-        for (size_t i = 0; i < v.size(); i++) order[i] = (uint32_t)i;
-        std::sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return v[a] < v[b]; }); // char_traits<char>: unsigned bytes
-        uint32_t next = 0;
-        for (size_t i = 0; i < order.size(); i++) {
-            if (i > 0 && v[order[i]] != v[order[i - 1]]) next++;
-            rank[order[i]] = next;
-        }
-        r.table = std::make_shared<DeviceBuf>(rank.size() * 4);
-        cuda_check(cudaMemcpyAsync(r.table->ptr, rank.data(), rank.size() * 4, cudaMemcpyHostToDevice, ctx->stream), "H2D sort ranks");
-        cuda_check(cudaStreamSynchronize(ctx->stream), "sort ranks copy");
-        ctx->h2d_bytes += (int64_t)(rank.size() * 4);
-        r.dict = d.get();
-        r.n = v.size();
-        return (const uint32_t*)r.table->ptr;
-    }
-
-    // out = b's rows [lo, hi) of the stable order of the keys.  When only the first rows are wanted (lo = 0, hi < n: TopK), an MSD radix
-    // select finds the key of row hi - 1 of that order, the rows up to it are compacted (the smaller keys, then the equal ones in input
-    // order) and only those are sorted.
-    void sort_rows(const Batch& b, int64_t lo, int64_t hi, Batch& out) {
-        const int64_t n = b.n_rows;
-        if (n >= ((int64_t)1 << 32)) throw Unsupported("sorting 2^32 rows or more");
-        cudaStream_t st = ctx->stream;
-        cb::SortKeyCols kc;
-        memset(&kc, 0, sizeof(kc));
-        kc.n = (int)keys.size();
-        kc.err = ctx->d_err;
-        ranks.resize(keys.size());
-        int bits = 0;
-        for (size_t k = keys.size(); k-- > 0;) { // the last key is the least significant field
-            const Column& c = b.cols.at((size_t)keys[k].expr->index);
-            cb::SortKeyCol& f = kc.col[k];
-            f.kind = key_kind(c);
-            f.bits = sort_key_bits(c.type);
-            f.desc = keys[k].descending;
-            f.nulls_first = keys[k].nulls_first;
-            f.has_null = c.validity != nullptr;
-            f.data = c.data ? c.data->ptr : nullptr;
-            f.validity = c.validity ? (const uint8_t*)c.validity->ptr : nullptr;
-            if (c.is_dict) {
-                f.rank = rank_table(k, c.dict);
-                f.n_rank = (int)c.dict->values().size();
-            }
-            f.off = bits;
-            bits += f.bits + f.has_null;
-        }
-        const int W = kc.words = std::max(1, (bits + 63) / 64);
-        uint64_t h_and_or[2 * cb::SK_MAX_WORDS];
-        std::vector<int> digits;
-        DeviceBufP keys0 = pack_row_keys(kc, n, bits, ctx, h_and_or, digits);
-        ctx->sort_rows += n;
-        if (lo > 0 || hi >= n) {
-            DeviceBufP idx = radix_order(ctx, keys0, W, n, digits);
-            count_passes(n, digits);
-            keys0.reset();
-            gather_columns(b, (const unsigned*)idx->ptr + lo, hi - lo, out, ctx, "sorting");
-            ctx->check_device_errors();
-            return;
-        }
-        // select: bits equal in every row are decided already; then one histogram per differing digit, most significant first
-        SortSelectKey p;
-        for (int j = 0; j < W; j++) { p.mask[j] = ~(h_and_or[j] ^ h_and_or[W + j]); p.want[j] = h_and_or[j] & p.mask[j]; }
-        int64_t r = hi; // the selected key's rank among the rows that match p
-        auto hist = std::make_shared<DeviceBuf>(256 * 4);
-        std::vector<uint32_t> hh(256);
-        for (size_t q = digits.size(); q-- > 0;) {
-            const int d = digits[q], w = W - 1 - d / 8, sh = (d % 8) * 8;
-            cuda_check(cudaMemsetAsync(hist->ptr, 0, 256 * 4, st), "memset select histogram");
-            cuda_check(launch_sort_select_hist((const unsigned long long*)keys0->ptr, W, n, p, d, (unsigned*)hist->ptr, st), "select histogram");
-            ctx->kernel_launches++;
-            ctx->sort_select_rows += n;
-            cuda_check(cudaMemcpyAsync(hh.data(), hist->ptr, 256 * 4, cudaMemcpyDeviceToHost, st), "D2H select histogram");
-            cuda_check(cudaStreamSynchronize(st), "select histogram sync");
-            int v = 0;
-            for (; v < 255 && r > (int64_t)hh[(size_t)v]; v++) r -= hh[(size_t)v];
-            p.mask[w] |= (uint64_t)0xff << sh;
-            p.want[w] |= (uint64_t)v << sh;
-        }
-        const size_t nb = (size_t)(n + 1023) / 1024;
-        auto eq = std::make_shared<DeviceBuf>((size_t)n + 16), keep = std::make_shared<DeviceBuf>((size_t)n + 16);
-        auto counts = std::make_shared<DeviceBuf>(nb * 4 + 4), offsets = std::make_shared<DeviceBuf>(nb * 8 + 8), kept = std::make_shared<DeviceBuf>(8);
-        cuda_check(launch_sort_select_keep((const unsigned long long*)keys0->ptr, W, n, p, r, (unsigned char*)eq->ptr, (int*)counts->ptr,
-                                           (long long*)offsets->ptr, (long long*)kept->ptr, (unsigned char*)keep->ptr, st), "select keep");
-        launch_compact_plan((const unsigned char*)keep->ptr, n, (int*)counts->ptr, (long long*)offsets->ptr, (long long*)kept->ptr, st);
-        auto rows = std::make_shared<DeviceBuf>((size_t)n * 4);
-        launch_sort_iota((unsigned*)rows->ptr, n, st);
-        auto ckeys = std::make_shared<DeviceBuf>((size_t)hi * W * 8), crows = std::make_shared<DeviceBuf>((size_t)hi * 4);
-        launch_compact_scatter((const unsigned char*)keep->ptr, n, (const long long*)offsets->ptr, keys0->ptr, W * 8, ckeys->ptr, st);
-        launch_compact_scatter((const unsigned char*)keep->ptr, n, (const long long*)offsets->ptr, rows->ptr, 4, crows->ptr, st);
-        cuda_check(cudaGetLastError(), "select compaction");
-        ctx->kernel_launches += 9;
-        int64_t m = 0;
-        cuda_check(cudaMemcpyAsync(&m, kept->ptr, 8, cudaMemcpyDeviceToHost, st), "D2H kept rows");
-        cuda_check(cudaStreamSynchronize(st), "select sync");
-        if (m != hi) throw ExecError(15, "", "internal: TopK selection kept " + std::to_string(m) + " rows for a fetch of " + std::to_string(hi));
-        keys0.reset(); rows.reset(); eq.reset(); keep.reset();
-        DeviceBufP order = radix_order(ctx, ckeys, W, m, digits);
-        count_passes(m, digits);
-        auto idx = std::make_shared<DeviceBuf>((size_t)m * 4);
-        launch_gather(crows->ptr, 4, (const unsigned*)order->ptr, m, idx->ptr, st); // compacted position -> row of b
-        ctx->kernel_launches++;
-        gather_columns(b, (const unsigned*)idx->ptr, m, out, ctx, "sorting");
-        ctx->check_device_errors();
-    }
-};
-
-// =================================================================================================
-// hash join (HashJoinExec with NullEquality::NullEqualsNothing, planner.rs:2192-2266): inner, left semi and left anti
-// =================================================================================================
-// The build side is drained before the first probe batch and concatenated on the device.  Its row keys (the sort's encoding,
-// device/cb_sortkey.h) are radix-sorted, so equal keys form runs in build input order, and every run without a NULL key gets one slot of
-// an open-addressing table.  A probe batch then costs one key pass and one lookup per row; an inner join scans the match counts, writes
-// the (probe row, build row) pairs and gathers both sides, a semi / anti join compacts the probe rows it keeps.  Output order: probe rows
-// in input order, an inner-join row's matches in build input order; an inner join's output above spark.comet.b200.chunkRows rows leaves
-// in several batches.
-//
-// Equal key tuples give equal words on both sides because the field layout is fixed by the declared key types (every field has a null
-// bit, whatever a batch's validity) and a string field holds a canonical code rather than the dictionary code: the code of the first
-// equal entry of the build side's dictionary, or that dictionary's size (which no build key has) for a probe string it lacks.
-struct JoinNode : ExecNode {
-    ExecContext* ctx;
-    ExecNodeP build_child, probe_child;
-    std::vector<int> build_keys, probe_keys; // key columns of each side, in key order
-    JoinType type = JoinType::Inner;
-    bool build_left = false;
-    int bits = 0, W = 1;                     // packed key bits (fixed per plan) and words
-    cb::u64 nullmask[cb::SK_MAX_WORDS] = {0, 0, 0, 0};
-
-    bool built = false;
-    Batch build;                             // the build side's rows, concatenated
-    DeviceBufP keys, rows, run_start, slots; // sorted build keys and their rows, run starts (+ the end), the table
-    JoinTable table{};
-    uint32_t h_build_rows = 0;
-    std::vector<DeviceBufP> build_canon;     // per key: build dictionary code -> canonical code
-    struct Canon { DictionaryP dict; size_t n = 0; DeviceBufP table; };
-    std::vector<Canon> probe_canon;          // per key: the probe dictionary it was built for, code -> canonical code
-
-    Batch probe;                             // the probe batch being emitted ...
-    DeviceBufP run_of, offs, chunk_off, kept_rows;
-    int64_t total = 0, pos = 0;              // ... its output rows, and those emitted
-
-    // the key layout from the declared key types: the last key is the least significant field, each with a null bit above its value
-    void set_layout(const std::vector<DType>& key_types) {
-        bits = 0;
-        for (size_t k = key_types.size(); k-- > 0;) bits += sort_key_bits(key_types[k]) + 1;
-        W = std::max(1, (bits + 63) / 64);
-        int off = 0;
-        for (size_t k = key_types.size(); k-- > 0;) {
-            off += sort_key_bits(key_types[k]);
-            cb::sk_put(nullmask, W, off, 1, 1);
-            off++;
-        }
-    }
-
-    void arrive(Batch& b) {
-        columns_to_device(b, ctx);
-        for (auto& c : b.cols)
-            if (c.offsets) throw Unsupported("joining plain string columns (dictionary-encode them first)");
-    }
-
-    DeviceBufP upload_codes(const std::vector<uint32_t>& v) {
-        auto t = std::make_shared<DeviceBuf>(v.size() * 4 + 4);
-        if (!v.empty()) cuda_check(cudaMemcpyAsync(t->ptr, v.data(), v.size() * 4, cudaMemcpyHostToDevice, ctx->stream), "H2D join codes");
-        cuda_check(cudaStreamSynchronize(ctx->stream), "join codes copy"); // v is the caller's temporary
-        ctx->h2d_bytes += (int64_t)(v.size() * 4);
-        return t;
-    }
-    // canonical codes of key k's dictionary d on the build side: the first equal entry (a caller's dictionary may repeat values)
-    const uint32_t* build_codes(size_t k, const DictionaryP& d) {
-        const std::vector<std::string>& v = d->values();
-        std::vector<uint32_t> c(v.size());
-        for (size_t i = 0; i < v.size(); i++) c[i] = (uint32_t)d->find(v[i]);
-        build_canon[k] = upload_codes(c);
-        return (const uint32_t*)build_canon[k]->ptr;
-    }
-    // ... and on the probe side: rebuilt when the column carries another dictionary or its dictionary has grown
-    const uint32_t* probe_codes(size_t k, const DictionaryP& d) {
-        Canon& p = probe_canon[k];
-        const std::vector<std::string>& v = d->values();
-        if (p.table && p.dict == d && p.n == v.size()) return (const uint32_t*)p.table->ptr;
-        const DictionaryP& bd = build.cols[(size_t)build_keys[k]].dict;
-        const uint32_t absent = (uint32_t)bd->values().size();
-        std::vector<uint32_t> c(v.size());
-        for (size_t i = 0; i < v.size(); i++) {
-            const int32_t code = bd->find(v[i]);
-            c[i] = code < 0 ? absent : (uint32_t)code;
-        }
-        p.table = upload_codes(c);
-        p.dict = d;
-        p.n = v.size();
-        return (const uint32_t*)p.table->ptr;
-    }
-    cb::SortKeyCols key_cols(const Batch& b, const std::vector<int>& cols, bool build_side) {
-        cb::SortKeyCols kc;
-        memset(&kc, 0, sizeof(kc));
-        kc.n = (int)cols.size();
-        kc.words = W;
-        kc.err = ctx->d_err;
-        int off = 0;
-        for (size_t k = cols.size(); k-- > 0;) {
-            const Column& c = b.cols.at((size_t)cols[k]);
-            cb::SortKeyCol& f = kc.col[k];
-            f.kind = key_kind(c);
-            f.bits = sort_key_bits(c.type);
-            f.nulls_first = 1; // null bit set on a valid value
-            f.has_null = 1;
-            f.data = c.data ? c.data->ptr : nullptr;
-            f.validity = c.validity ? (const uint8_t*)c.validity->ptr : nullptr;
-            if (c.is_dict) {
-                f.rank = build_side ? build_codes(k, c.dict) : probe_codes(k, c.dict);
-                f.n_rank = (int)c.dict->values().size();
-            }
-            f.off = off;
-            off += f.bits + 1;
-        }
-        return kc;
-    }
-
-    void build_table() {
-        built = true;
-        std::vector<Batch> bs;
-        Batch in;
-        while (build_child->next(in)) {
-            arrive(in);
-            ctx->join_build_rows += in.n_rows;
-            if (in.n_rows > 0) bs.push_back(std::move(in));
-            in = Batch();
-        }
-        if (bs.empty()) return;
-        TraceSpan ts("join.build");
-        build = bs.size() == 1 ? std::move(bs[0]) : concat_batches(bs, ctx, "hash join build");
-        bs.clear();
-        const int64_t n = build.n_rows;
-        if (n >= ((int64_t)1 << 32)) throw Unsupported("a hash join build side of 2^32 rows or more");
-        cudaStream_t st = ctx->stream;
-        build_canon.assign(build_keys.size(), nullptr);
-        probe_canon.assign(build_keys.size(), Canon());
-        uint64_t h_and_or[2 * cb::SK_MAX_WORDS];
-        std::vector<int> digits;
-        DeviceBufP k0 = pack_row_keys(key_cols(build, build_keys, true), n, bits, ctx, h_and_or, digits);
-        rows = radix_order(ctx, k0, W, n, digits, &keys);
-        k0.reset();
-        const size_t nb = (size_t)(n + 1023) / 1024;
-        auto head = std::make_shared<DeviceBuf>((size_t)n + 16), iota = std::make_shared<DeviceBuf>((size_t)n * 4);
-        auto counts = std::make_shared<DeviceBuf>(nb * 4 + 4), offsets = std::make_shared<DeviceBuf>(nb * 8 + 8), d_runs = std::make_shared<DeviceBuf>(8);
-        run_start = std::make_shared<DeviceBuf>((size_t)(n + 1) * 4);
-        launch_join_heads((const unsigned long long*)keys->ptr, W, n, (unsigned char*)head->ptr, st);
-        launch_compact_plan((const unsigned char*)head->ptr, n, (int*)counts->ptr, (long long*)offsets->ptr, (long long*)d_runs->ptr, st);
-        launch_sort_iota((unsigned*)iota->ptr, n, st);
-        launch_compact_scatter((const unsigned char*)head->ptr, n, (const long long*)offsets->ptr, iota->ptr, 4, run_start->ptr, st);
-        cuda_check(cudaGetLastError(), "join run heads");
-        ctx->kernel_launches += 5;
-        int64_t n_runs = 0;
-        cuda_check(cudaMemcpyAsync(&n_runs, d_runs->ptr, 8, cudaMemcpyDeviceToHost, st), "D2H join runs");
-        cuda_check(cudaStreamSynchronize(st), "join runs sync");
-        h_build_rows = (uint32_t)n;
-        cuda_check(cudaMemcpyAsync((uint32_t*)run_start->ptr + n_runs, &h_build_rows, 4, cudaMemcpyHostToDevice, st), "H2D run end");
-        size_t cap = 1024;
-        while (cap < (size_t)n_runs * 2) cap <<= 1;
-        slots = std::make_shared<DeviceBuf>(cap * 8);
-        cuda_check(cudaMemsetAsync(slots->ptr, 0, cap * 8, st), "memset join table");
-        table.keys = (const unsigned long long*)keys->ptr;
-        table.rows = (const unsigned*)rows->ptr;
-        table.run_start = (const unsigned*)run_start->ptr;
-        table.slots = (unsigned long long*)slots->ptr;
-        table.mask = cap - 1;
-        table.words = W;
-        for (int j = 0; j < cb::SK_MAX_WORDS; j++) table.nullmask[j] = nullmask[j];
-        launch_join_insert(table, n_runs, st);
-        cuda_check(cudaGetLastError(), "k_join_insert launch");
-        ctx->kernel_launches++;
-        ctx->check_device_errors();
-    }
-
-    // the lookups of probe batch `in`: `total` output rows to emit from it
-    void probe_batch(Batch& in) {
-        TraceSpan ts("join.probe");
-        const int64_t n = in.n_rows;
-        if (n >= ((int64_t)1 << 32)) throw Unsupported("a hash join probe batch of 2^32 rows or more");
-        cudaStream_t st = ctx->stream;
-        uint64_t h_and_or[2 * cb::SK_MAX_WORDS];
-        std::vector<int> digits;
-        DeviceBufP pk = pack_row_keys(key_cols(in, probe_keys, false), n, bits, ctx, h_and_or, digits);
-        probe = std::move(in);
-        pos = 0;
-        if (type == JoinType::Inner) {
-            const size_t n_chunks = (size_t)(n + CB_SCAN_CHUNK - 1) / CB_SCAN_CHUNK;
-            run_of = std::make_shared<DeviceBuf>((size_t)n * 4);
-            offs = std::make_shared<DeviceBuf>((size_t)n * 4);
-            chunk_off = std::make_shared<DeviceBuf>((n_chunks + 1) * 4);
-            auto tot = std::make_shared<DeviceBuf>(16);
-            cuda_check(cudaMemsetAsync(tot->ptr, 0, 16, st), "memset join total");
-            launch_join_probe(table, (const unsigned long long*)pk->ptr, n, CB_JOIN_COUNT, (unsigned*)offs->ptr, (unsigned*)run_of->ptr,
-                              (unsigned long long*)tot->ptr, nullptr, st);
-            launch_scan_u32((unsigned*)offs->ptr, n, CB_SCAN_CHUNK, (unsigned*)chunk_off->ptr, (long long*)tot->ptr + 1, st);
-            cuda_check(cudaGetLastError(), "join probe");
-            ctx->kernel_launches += 3;
-            cuda_check(cudaMemcpyAsync(&total, tot->ptr, 8, cudaMemcpyDeviceToHost, st), "D2H join total");
-            ctx->check_device_errors();
-            // the scan's offsets are 32-bit
-            if (total >= ((int64_t)1 << 32)) throw Unsupported("a probe batch whose inner join output has 2^32 rows or more (lower spark.comet.b200.chunkRows)");
-        } else {
-            const size_t nb = (size_t)(n + 1023) / 1024;
-            auto keep = std::make_shared<DeviceBuf>((size_t)n + 16), iota = std::make_shared<DeviceBuf>((size_t)n * 4);
-            auto counts = std::make_shared<DeviceBuf>(nb * 4 + 4), offsets = std::make_shared<DeviceBuf>(nb * 8 + 8), kept = std::make_shared<DeviceBuf>(8);
-            kept_rows = std::make_shared<DeviceBuf>((size_t)n * 4);
-            launch_join_probe(table, (const unsigned long long*)pk->ptr, n, type == JoinType::LeftSemi ? CB_JOIN_SEMI : CB_JOIN_ANTI, nullptr, nullptr, nullptr,
-                              (unsigned char*)keep->ptr, st);
-            launch_compact_plan((const unsigned char*)keep->ptr, n, (int*)counts->ptr, (long long*)offsets->ptr, (long long*)kept->ptr, st);
-            launch_sort_iota((unsigned*)iota->ptr, n, st);
-            launch_compact_scatter((const unsigned char*)keep->ptr, n, (const long long*)offsets->ptr, iota->ptr, 4, kept_rows->ptr, st);
-            cuda_check(cudaGetLastError(), "join probe");
-            ctx->kernel_launches += 5;
-            cuda_check(cudaMemcpyAsync(&total, kept->ptr, 8, cudaMemcpyDeviceToHost, st), "D2H join kept rows");
-            ctx->check_device_errors();
-        }
-    }
-
-    // the next at most chunkRows output rows of the probe batch
-    void emit(Batch& out) {
-        const int64_t k = std::min<int64_t>(total - pos, std::max<int64_t>(ctx->chunk_rows, 1));
-        if (type == JoinType::Inner) {
-            auto pidx = std::make_shared<DeviceBuf>((size_t)k * 4), bidx = std::make_shared<DeviceBuf>((size_t)k * 4);
-            launch_join_emit(table, (const unsigned*)run_of->ptr, (const unsigned*)offs->ptr, (const unsigned*)chunk_off->ptr, probe.n_rows, pos, pos + k,
-                             (unsigned*)pidx->ptr, (unsigned*)bidx->ptr, ctx->stream);
-            cuda_check(cudaGetLastError(), "k_join_emit launch");
-            ctx->kernel_launches++;
-            Batch pb, bb;
-            gather_columns(probe, (const unsigned*)pidx->ptr, k, pb, ctx, "joining");
-            gather_columns(build, (const unsigned*)bidx->ptr, k, bb, ctx, "joining");
-            Batch& l = build_left ? bb : pb;
-            Batch& r = build_left ? pb : bb;
-            out.n_rows = k;
-            out.cols = std::move(l.cols);
-            for (auto& c : r.cols) out.cols.push_back(std::move(c));
-        } else {
-            gather_columns(probe, (const unsigned*)kept_rows->ptr + pos, k, out, ctx, "joining");
-        }
-        pos += k;
-        ctx->join_out_rows += k;
-        ctx->check_device_errors();
-        if (pos >= total) { probe = Batch(); run_of.reset(); offs.reset(); chunk_off.reset(); kept_rows.reset(); }
-    }
-
-    bool next(Batch& out) override {
-        if (!built) build_table();
-        const bool empty_build = build.n_rows == 0;
-        if (empty_build && type != JoinType::LeftAnti) return false; // nothing matches
-        for (;;) {
-            if (pos < total) { emit(out); return true; }
-            Batch in;
-            if (!probe_child->next(in)) return false;
-            arrive(in);
-            ctx->join_probe_rows += in.n_rows;
-            if (in.n_rows == 0) continue;
-            if (empty_build) { // anti: every probe row
-                ctx->join_out_rows += in.n_rows;
-                out = std::move(in);
-                return true;
-            }
-            probe_batch(in);
-        }
-    }
-};
-
 // =================================================================================================
 // plan -> executor tree
 // =================================================================================================
@@ -1476,60 +753,13 @@ static ExecNodeP build_source(const OperatorP& op, ExecContext* ctx, PlanInputs*
 static ExecNodeP build_node(const OperatorP& op, ExecContext* ctx, PlanInputs* inputs, bool build_only, const std::vector<int>& assume) {
     OperatorP cur = op;
     OperatorP agg_op;
-    if (cur->kind == OpKind::ShuffleWriter) {
-        auto n = std::make_shared<PartitionNode>();
-        n->ctx = ctx;
-        n->child = build_node(cur->children[0], ctx, inputs, build_only, assume);
-        n->schema = cur->schema;
-        n->n_parts = cur->num_partitions;
-        for (auto& e : cur->hash_exprs) {
-            if (e->kind != ExprKind::Bound) throw Unsupported("computed hash-partition keys (only plain column keys)");
-            n->key_cols.push_back(e->index);
-        }
-        if (n->key_cols.size() > 8) throw Unsupported("more than 8 hash-partition keys");
-        if (n->n_parts > CB_MAX_HASH_PARTITIONS)
-            throw Unsupported("hash partitioning into " + std::to_string(n->n_parts) + " partitions (at most " + std::to_string((int)CB_MAX_HASH_PARTITIONS) + ")");
-        for (int ci : n->key_cols) { // refuses key types murmur3 has no rule for
-            if (ci < 0 || ci >= (int)cur->schema.size()) throw PlanError("hash-partition key out of range");
-            Column c;
-            c.type = cur->schema[(size_t)ci];
-            key_kind(c);
-        }
-        return n;
-    }
-    if (cur->kind == OpKind::Sort) {
-        auto n = std::make_shared<SortNode>();
-        n->ctx = ctx;
-        n->child = build_node(cur->children[0], ctx, inputs, build_only, assume);
-        n->schema = cur->schema;
-        n->keys = cur->sort_keys;
-        n->fetch = cur->fetch;
-        n->skip = std::max<int64_t>(cur->skip, 0);
-        for (auto& k : n->keys)
-            if (k.expr->index < 0 || k.expr->index >= (int)cur->schema.size()) throw PlanError("sort key out of range");
-        return n;
-    }
+    if (cur->kind == OpKind::ShuffleWriter) return make_partition_node(cur, build_node(cur->children[0], ctx, inputs, build_only, assume), ctx);
+    if (cur->kind == OpKind::Sort) return make_sort_node(cur, build_node(cur->children[0], ctx, inputs, build_only, assume), ctx);
     if (cur->kind == OpKind::HashJoin) {
-        auto n = std::make_shared<JoinNode>();
-        n->ctx = ctx;
-        ExecNodeP left = build_node(cur->children[0], ctx, inputs, build_only, assume); // inputs are taken in Scan order: left first
+        // inputs are taken in Scan order: the left child is built first, in a statement of its own (argument order is unspecified)
+        ExecNodeP left = build_node(cur->children[0], ctx, inputs, build_only, assume);
         ExecNodeP right = build_node(cur->children[1], ctx, inputs, build_only, assume);
-        n->schema = cur->schema;
-        n->type = cur->join_type;
-        n->build_left = cur->build_left;
-        std::vector<int> lk, rk;
-        std::vector<DType> key_types;
-        for (size_t i = 0; i < cur->left_keys.size(); i++) {
-            lk.push_back(cur->left_keys[i]->index);
-            rk.push_back(cur->right_keys[i]->index);
-            key_types.push_back(cur->left_keys[i]->type);
-        }
-        n->build_child = cur->build_left ? left : right;
-        n->probe_child = cur->build_left ? right : left;
-        n->build_keys = cur->build_left ? lk : rk;
-        n->probe_keys = cur->build_left ? rk : lk;
-        n->set_layout(key_types);
-        return n;
+        return make_join_node(cur, left, right, ctx);
     }
     if (cur->kind == OpKind::HashAgg) { agg_op = cur; cur = cur->children[0]; }
     std::vector<OperatorP> chain; // top-down
@@ -1570,21 +800,9 @@ static ExecNodeP build_node(const OperatorP& op, ExecContext* ctx, PlanInputs* i
 ExecNodeP build_exec(const OperatorP& op, ExecContext* ctx, PlanInputs* inputs) { return build_node(op, ctx, inputs, false, {}); }
 
 // the pipeline kernels of the tree under n, top-down; a join's left child before its right one
-static void collect_kernels(ExecNodeP n, std::vector<GeneratedKernel>& out) {
-    while (n) {
-        if (auto f = std::dynamic_pointer_cast<FusedBase>(n)) {
-            for (const PipelineSpec& s : f->build_specs()) out.push_back(generate_pipeline(s));
-            n = f->child;
-        } else if (auto pn = std::dynamic_pointer_cast<PartitionNode>(n)) {
-            n = pn->child;
-        } else if (auto jn = std::dynamic_pointer_cast<JoinNode>(n)) {
-            collect_kernels(jn->build_left ? jn->build_child : jn->probe_child, out);
-            n = jn->build_left ? jn->probe_child : jn->build_child;
-        } else {
-            auto sn = std::dynamic_pointer_cast<SortNode>(n);
-            n = sn ? sn->child : nullptr;
-        }
-    }
+static void collect_kernels(const ExecNodeP& n, std::vector<GeneratedKernel>& out) {
+    for (const PipelineSpec& s : n->build_specs()) out.push_back(generate_pipeline(s));
+    for (const ExecNodeP& c : n->children()) collect_kernels(c, out);
 }
 
 std::vector<GeneratedKernel> plan_kernels_for_build(const OperatorP& op, const std::vector<int>& assume) {

@@ -95,7 +95,7 @@ struct Column {
     DictionaryP dict;
     DeviceBufP data, validity;      // device (validity: Arrow bitmap) ...
     DeviceBufP offsets, chars;      // ... device Utf8 (offsets int32[n+1], chars)
-    DeviceBufP valid_bytes;         // optional byte-per-row validity (exchange-friendly form; see PartitionNode / cb200_table_add_column_bytes)
+    DeviceBufP valid_bytes;         // optional byte-per-row validity (exchange-friendly form; see gather_columns / cb200_table_add_column_bytes)
     DeviceBufP bool_bytes;          // optional byte-per-row form of a boolean column
     int64_t null_count = 0;
     // host-resident alternative (small aggregate results)
@@ -147,6 +147,10 @@ struct ExecNode {
     std::vector<DType> schema;
     virtual ~ExecNode() {}
     virtual bool next(Batch& out) = 0; // false = end of stream
+    // the node's children in plan order (a join: left, then right, whichever side builds)
+    virtual std::vector<std::shared_ptr<ExecNode>> children() const { return {}; }
+    // build time: the pipelines this node may launch, for inputs without nulls and with dictionary-encoded strings
+    virtual std::vector<PipelineSpec> build_specs() const { return {}; }
     // predicates (over this node's output columns) that the consumer applies to every row anyway: a source may use them to skip
     // data that cannot pass (Parquet row groups whose statistics rule them out)
     virtual void push_filters(const std::vector<ExprP>&) {}

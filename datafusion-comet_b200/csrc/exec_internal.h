@@ -1,12 +1,15 @@
 // exec_internal.h -- what the executor's translation units share: the fused-pipeline node base, the physical encoding of a
-// logical type, the expression-slot helpers and the shared-memory budget of a pipeline kernel.
+// logical type, the expression-slot helpers, the shared-memory budget of a pipeline kernel, the operator factories and the row
+// primitives of the row operators.
 #pragma once
 #include "exec.h"
 
 #include "aot_kernels.h"
 #include "device/cb_params.h"
 
+#include <algorithm>
 #include <cstring>
+#include <functional>
 #include <map>
 #include <set>
 
@@ -35,6 +38,8 @@ inline Phys kernel_out_phys(const DType& t) { return t.id == TypeId::Bool ? Phys
 inline size_t bitmap_bytes(int64_t n) { return (size_t)(n + 31) / 32 * 4 + 8; }
 // a new device bitmap of n rows, bit r set where bytes[r] != 0 (one launch on ctx->stream, counted)
 DeviceBufP bytes_to_bitmap(const DeviceBufP& bytes, int64_t n, ExecContext* ctx);
+// n bytes (nonzero = set) as a host bitmap, 8 bytes of slack behind it
+std::vector<uint8_t> pack_bits(const uint8_t* bytes, size_t n);
 
 // ---- expression helpers --------------------------------------------------------------------------------------------
 inline ExprP clone_expr(const ExprP& e) {
@@ -94,8 +99,7 @@ struct FusedBase : ExecNode {
     std::vector<int> used_cols;      // child columns staged, in slot order
     std::map<int, int> slot_of;
 
-    // build time: the pipelines this node may launch, for inputs without nulls and with dictionary-encoded strings
-    virtual std::vector<PipelineSpec> build_specs() const = 0;
+    std::vector<ExecNodeP> children() const override { return {child}; }
 
     // build the staged-column list for one batch signature
     std::vector<SourceCol> stage_cols(const Batch* b) const { return stage_cols_of(b, used_cols); }
@@ -167,5 +171,51 @@ struct FusedBase : ExecNode {
 // `assume_bits`: build-time value-range assumptions per source column (see cb200_compile_plan_assume); empty at run time.
 ExecNodeP make_agg_node(const OperatorP& agg_op, const ExecNodeP& src, const std::vector<ExprP>& preds, const std::vector<ExprP>& cols, ExecContext* ctx,
                         const std::vector<int>& assume_bits);
+// partition.cpp, sort.cpp, join.cpp: the row operators over their built children; each validates its operator's fields
+ExecNodeP make_partition_node(const OperatorP& op, const ExecNodeP& child, ExecContext* ctx);
+ExecNodeP make_sort_node(const OperatorP& op, const ExecNodeP& child, ExecContext* ctx);
+ExecNodeP make_join_node(const OperatorP& op, const ExecNodeP& left, const ExecNodeP& right, ExecContext* ctx);
+
+// ---- row primitives shared by repartitioning, Sort and HashJoin (rows.cpp) ------------------------------------------
+// The HK_* kind of a key column (device/cb_sortkey.h).  The logical type decides how Spark hashes a value (utils.rs: i8 / i16 / i32 /
+// date as i32, decimal(p <= 18) as i64, wider decimals as 16 bytes) and how many bits its sort key takes; the stored layout (DESIGN.md,
+// "Data layout in HBM") decides how it is read.
+int key_kind(const Column& c);
+// a new device buffer holding host bytes [p, p + n), safe to use once this returns (it synchronises); not counted in h2d_bytes
+DeviceBufP host_to_device(const void* p, size_t n, ExecContext* ctx, const char* what);
+// small host-resident aggregate results -> device columns
+void columns_to_device(Batch& b, ExecContext* ctx);
+// a batch arriving at a Sort or join: columns_to_device, and plain Utf8 columns refused (`op`: "sorting", "joining")
+void arrive(Batch& b, ExecContext* ctx, const char* op);
+// every batch of `child`, arrived (`op` as in arrive) and concatenated (`concat_op` as in concat_batches); no rows if it has none
+Batch drain(ExecNode& child, ExecContext* ctx, const char* op, const char* concat_op);
+// out's columns = in's rows row_idx[0, n), in that order.  Bit-packed booleans and validity are gathered one byte per row and repacked
+// (the byte forms are kept: the exchange sends them).  `op` names the operator in the refusal of plain Utf8 columns.  I: long long or
+// unsigned.
+template <typename I> void gather_columns(const Batch& in, const I* row_idx, int64_t n, Batch& out, ExecContext* ctx, const char* op);
+// the rows of bs in one batch (`bs` non-empty, every batch on the device): values and validity appended in order; dictionary-coded strings
+// that carry different Dictionary objects are recoded into one (the first batch's entries, then the others' new entries)
+Batch concat_batches(const std::vector<Batch>& bs, ExecContext* ctx, const char* op);
+// column c as the row-key field at bit `off` (advanced past it), with a null bit if has_null.  The caller sets desc, nulls_first and rank.
+cb::SortKeyCol key_field(const Column& c, bool has_null, int& off);
+// the row keys of kc (W = kc.words words each) for n rows, and_or[0, W) their AND and [W, 2W) their OR, `digits` the 8-bit digits of the
+// `bits`-bit key that are not the same in every row, least significant first.  Synchronises: a dictionary code outside its dictionary
+// fails here.
+struct RowKeys { DeviceBufP keys; uint64_t and_or[2 * cb::SK_MAX_WORDS]; std::vector<int> digits; };
+RowKeys pack_row_keys(const cb::SortKeyCols& kc, int64_t n, int bits, ExecContext* ctx);
+// the stable order of m rows whose keys (`words` words each) are in keys0, by the given digits: row indices [0, m); `sorted_keys`, if
+// given, receives the keys in that order
+DeviceBufP radix_order(ExecContext* ctx, DeviceBufP keys0, int words, int64_t m, const std::vector<int>& digits, DeviceBufP* sorted_keys = nullptr);
+// The stable compaction of n rows by their keep flags (one byte per row): the kept rows' 32-bit indices in order, in a buffer of `cap`
+// rows, and their count.  Each `extra` (array, bytes per row) is compacted by the same plan into extra_out, `cap` rows each.  Reading
+// the count synchronises and checks the error flags.
+struct Compacted { DeviceBufP rows; int64_t n = 0; std::vector<DeviceBufP> extra_out; };
+Compacted compact_rows(const DeviceBufP& keep, int64_t n, int64_t cap, ExecContext* ctx, const std::vector<std::pair<DeviceBufP, int>>& extra = {});
+// A device table indexed by the codes of a column's dictionary, made on the host by `make` and counted in h2d_bytes; rebuilt when the
+// column carries another dictionary or its dictionary has grown.  Holding the dictionary keeps a new one at a freed one's address apart.
+struct DictCodes {
+    DictionaryP dict; size_t n = 0; DeviceBufP table;
+    const uint32_t* get(const DictionaryP& d, ExecContext* ctx, const std::function<std::vector<uint32_t>(const Dictionary&)>& make);
+};
 
 } // namespace cb200

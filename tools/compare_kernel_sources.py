@@ -4,8 +4,10 @@
 
 Each tree is a checkout whose libcomet_b200.so is built (`make -C datafusion-comet_b200/csrc`).  For every plan below and every
 kernel index, `native.kernel_source(plan, i)` must be identical in both trees: the TPC-H Q1 partial / final (dec and f64) and Q6
-plans, Config 1, the group-by map and final plans of bench.py, the string-predicate plans of tests/test_string_predicates_cpu.py and
-a Sort over a pipeline.  Lists every plan whose sources or kernel count differ, and then exits 1."""
+plans, Config 1, the group-by map and final plans of bench.py, the string-predicate plans of tests/test_string_predicates_cpu.py,
+a Sort over a pipeline and a ShuffleWriter over that Sort, an aggregate over an inner HashJoin of two filter pipelines (built on the
+left and on the right) and a left semi join of the same pipelines.  Lists every plan whose sources or kernel count differ, and then
+exits 1."""
 import json
 import os
 import subprocess
@@ -39,6 +41,16 @@ def plans():
     out["strpred_two_masks"] = T.filt(P.or_(P.like(c, T.slit("a%")), P.like(c, T.slit("b%"))))
     out["strpred_same_mask"] = T.filt(P.or_(P.like(c, T.slit("a%")), P.like(c, T.slit("a%"))))
     out["sort_over_filter"] = P.sort(T.filt(P.like(c, T.slit("a%"))), [P.sort_order(P.bound(0, P.INT64), descending=True)])
+    out["shuffle_writer_over_sort"] = P.shuffle_writer(out["sort_over_filter"], P.hash_partitioning([P.bound(0, P.INT64)], 8))
+    # joins: a different pipeline under each child, so the tool also sees the order their kernels are listed in
+    lt, rt = [P.INT64, P.DOUBLE, P.STRING], [P.STRING, P.INT32, P.DECIMAL(12, 2)]
+    left = P.filter_(P.scan(lt), P.gt(P.bound(1, P.DOUBLE), P.literal(0.5, P.DOUBLE)))
+    right = P.filter_(P.scan(rt), P.is_not_null(P.bound(2, P.DECIMAL(12, 2))))
+    for name, build in (("build_left", P.BUILD_LEFT), ("build_right", P.BUILD_RIGHT)):
+        j = P.hash_join(left, right, [P.bound(2, P.STRING)], [P.bound(0, P.STRING)], P.INNER, build)
+        out[f"agg_over_inner_join_{name}"] = P.hash_agg(j, [P.bound(2, P.STRING)], [P.agg_sum(P.bound(0, P.INT64), P.INT64),
+                                                         P.agg_sum(P.bound(5, P.DECIMAL(12, 2)), P.DECIMAL(22, 2))], P.PARTIAL)
+    out["left_semi_join"] = P.hash_join(left, right, [P.bound(2, P.STRING)], [P.bound(0, P.STRING)], P.LEFT_SEMI, P.BUILD_RIGHT)
     return out
 
 
