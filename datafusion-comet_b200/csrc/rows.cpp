@@ -109,6 +109,10 @@ template <typename I> void gather_columns(const Batch& in, const I* row_idx, int
 template void gather_columns<long long>(const Batch&, const long long*, int64_t, Batch&, ExecContext*, const char*);
 template void gather_columns<unsigned>(const Batch&, const unsigned*, int64_t, Batch&, ExecContext*, const char*);
 
+// A non-dictionary column whose batches store it in different layouts -- a Partial aggregate that migrates from dense to hash emits
+// its booleans first as a bitmap (the host flush), then one byte per row (kernel output) -- is brought to the Arrow layout of its type
+// in every batch first, the conversion export makes (to_arrow_layout).  Dictionary columns of different dictionaries are remapped to
+// int32 codes of one new dictionary.
 Batch concat_batches(const std::vector<Batch>& bs, ExecContext* ctx, const char* op) {
     cudaStream_t st = ctx->stream;
     Batch out;
@@ -116,26 +120,39 @@ Batch concat_batches(const std::vector<Batch>& bs, ExecContext* ctx, const char*
     const size_t n = (size_t)out.n_rows;
     std::vector<DeviceBufP> temps;
     for (size_t j = 0; j < bs[0].cols.size(); j++) {
-        const Column& c0 = bs[0].cols[j];
+        std::vector<Column> cs;
+        for (auto& b : bs) cs.push_back(b.cols[j]);
+        const Column& c0 = cs[0];
+        bool same = true, nulls = false;
+        for (const Column& c : cs) {
+            if (c.phys != c0.phys || c.dict != c0.dict || c.is_dict != c0.is_dict) same = false;
+            if (c.validity) nulls = true;
+        }
+        if (!same && !c0.is_dict) {
+            for (size_t i = 0; i < cs.size(); i++) {
+                Batch one;
+                one.n_rows = bs[i].n_rows;
+                one.cols = {cs[i]};
+                to_arrow_layout(one, ctx);
+                cs[i] = one.cols[0];
+                if (cs[i].phys != cs[0].phys || cs[i].is_dict) // arrive() refuses plain strings, the one type to_arrow_layout leaves alone
+                    throw ExecError(15, "", std::string("internal: ") + op + " input whose batches store column " + std::to_string(j) + " in different layouts");
+            }
+            same = true;
+        }
         Column o;
         o.type = c0.type;
         o.phys = c0.phys;
         o.is_dict = c0.is_dict;
         o.dict = c0.dict;
-        bool same = true, nulls = false;
-        for (auto& b : bs) {
-            const Column& c = b.cols[j];
-            if (c.phys != c0.phys || c.dict != c0.dict || c.is_dict != c0.is_dict) same = false;
-            if (c.validity) nulls = true;
-        }
-        if (!same && !c0.is_dict) throw Unsupported(std::string(op) + " input whose batches store column " + std::to_string(j) + " in different layouts");
         if (same) {
             const int w = phys_bytes(c0.phys);
             o.data = std::make_shared<DeviceBuf>(w == 0 ? bitmap_bytes((int64_t)n) : std::max<size_t>(n, 1) * (size_t)w);
             if (w == 0) cuda_check(cudaMemsetAsync(o.data->ptr, 0, o.data->bytes, st), "memset bools");
             int64_t row = 0;
-            for (auto& b : bs) {
-                const Column& c = b.cols[j];
+            for (size_t i = 0; i < cs.size(); i++) {
+                const Batch& b = bs[i];
+                const Column& c = cs[i];
                 if (w == 0) { launch_bitmap_append((uint32_t*)o.data->ptr, row, (const uint8_t*)c.data->ptr, 0, b.n_rows, st); ctx->kernel_launches++; }
                 else cuda_check(cudaMemcpyAsync((char*)o.data->ptr + (size_t)row * w, c.data->ptr, (size_t)b.n_rows * w, cudaMemcpyDeviceToDevice, st), "concat column");
                 row += b.n_rows;
