@@ -371,7 +371,9 @@ struct Emitter {
                                  ? (e.kind == ExprKind::Add ? "__dadd_rn" : e.kind == ExprKind::Sub ? "__dsub_rn" : e.kind == ExprKind::Mul ? "__dmul_rn" : "__ddiv_rn")
                                  : (e.kind == ExprKind::Add ? "__fadd_rn" : e.kind == ExprKind::Sub ? "__fsub_rn" : e.kind == ExprKind::Mul ? "__fmul_rn" : "__fdiv_rn");
             (void)opc;
-            r.v = decl(e.type, fn + "(" + l.v + ", " + rr.v + ")");
+            // Float32: the hardware returns the canonical NaN 0x7FFFFFFF; f32_x86_nan restores the reference's (x86) NaN bits
+            if (lt.id == TypeId::Float64) r.v = decl(e.type, fn + "(" + l.v + ", " + rr.v + ")");
+            else r.v = decl(e.type, "cb::f32_x86_nan(" + l.v + ", " + rr.v + ", " + fn + "(" + l.v + ", " + rr.v + "))");
             r.n = nn;
             if (e.kind == ExprKind::Div && e.eval_mode != EvalMode::Legacy) {
                 // checked_div (checked_arithmetic.rs:53-128; planner.rs:1094-1125 routes float Divide there under TRY / ANSI):
@@ -403,10 +405,11 @@ struct Emitter {
         const char* opc = e.kind == ExprKind::Add ? "+" : e.kind == ExprKind::Sub ? "-" : "*";
         if (bits < 64) {
             body << "    cb::i64 " << wide << " = (cb::i64)" << l.v << " " << opc << " (cb::i64)" << rr.v << ";\n";
-            std::string wrapped = bits == 8 ? "(cb::i32)(signed char)" + wide : bits == 16 ? "(cb::i32)(short)" + wide : "(cb::i32)" + wide;
+            std::string wrapped = "(cb::i32)cb::wrap_int(" + wide + ", " + std::to_string(bits) + ")";
             r.v = decl(e.type, wrapped);
             if (e.eval_mode != EvalMode::Legacy) {
-                std::string ovf = declb("(cb::i64)" + r.v + " != " + wide);
+                const std::string lim = std::to_string((1LL << (bits - 1)) - 1);
+                std::string ovf = declb("(" + wide + " < -" + lim + "ll - 1 || " + wide + " > " + lim + "ll)");
                 if (e.eval_mode == EvalMode::Ansi) { raise(valid + " && " + ovf, 1); r.n = nn; }
                 else r.n = or_null(nn, ovf);
             } else r.n = nn;
@@ -591,7 +594,7 @@ struct Emitter {
         else if (t.id == TypeId::Int64) r.v = decl(t, "(cb::i64)(0ull - (cb::u64)" + c.v + ")");
         else {
             int bits = t.id == TypeId::Int8 ? 8 : t.id == TypeId::Int16 ? 16 : 32;
-            r.v = decl(t, bits == 8 ? "(cb::i32)(signed char)(0u - (cb::u32)" + c.v + ")" : bits == 16 ? "(cb::i32)(short)(0u - (cb::u32)" + c.v + ")" : "(cb::i32)(0u - (cb::u32)" + c.v + ")");
+            r.v = decl(t, "(cb::i32)cb::wrap_int(-(cb::i64)" + c.v + ", " + std::to_string(bits) + ")");
         }
         if (e.fail_on_error && t.is_integer()) { // negative.rs: ANSI overflow on MIN
             std::string valid = c.n.empty() ? "true" : "!" + c.n;
@@ -635,6 +638,7 @@ struct Emitter {
             Val mv = emit(m);
             if (v.type.is_decimal()) any += (v.narrow && mv.narrow) ? " || (" + v.v + " == " + mv.v + ")" : " || cb::i128_eq(" + W(v) + ", " + W(mv) + ")";
             else if (v.type.id == TypeId::Float64) any += " || (__double_as_longlong(" + v.v + ") == __double_as_longlong(" + mv.v + "))";
+            else if (v.type.id == TypeId::Float32) any += " || (__float_as_uint(" + v.v + ") == __float_as_uint(" + mv.v + "))";
             else any += " || (" + v.v + " == " + mv.v + ")";
         }
         Val r;

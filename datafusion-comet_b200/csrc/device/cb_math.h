@@ -562,6 +562,34 @@ CB_HD float f32_neg(float x) {
 #endif
 }
 
+// Two's-complement wrap of v to a `bits`-wide integer (8, 16 or 32), sign-extended, by masking and
+// re-biasing: arrow-arith's wrapping add / sub / mul / neg of Int8 / Int16 / Int32.
+CB_HD i64 wrap_int(i64 v, int bits) {
+    const u64 m = (1ull << bits) - 1, s = 1ull << (bits - 1);
+    return (i64)((((u64)v & m) ^ s) - s);
+}
+
+// NaN bits of Float32 arithmetic.  The reference runs on x86 (SSE), where a NaN result is the first
+// NaN operand made quiet (payload and sign kept) and an invalid operation without a NaN operand
+// (Inf - Inf, 0 * Inf, 0 / 0) returns the default NaN 0xFFC00000.  The H100's .f32 add / sub / mul /
+// div return the canonical NaN 0x7FFFFFFF in all those cases (its .f64 arithmetic and the f32 -> f64
+// conversion already give the x86 bits), so the emitter passes every Float32 result `r` of `a op b`
+// through this rule.  Non-NaN results are returned unchanged.
+CB_HD float f32_x86_nan(float a, float b, float r) {
+#if defined(__CUDA_ARCH__)
+    const u32 rb = __float_as_uint(r), ab = __float_as_uint(a), bb = __float_as_uint(b);
+#else
+    u32 rb, ab, bb; __builtin_memcpy(&rb, &r, 4); __builtin_memcpy(&ab, &a, 4); __builtin_memcpy(&bb, &b, 4);
+#endif
+    if ((rb & 0x7FFFFFFFu) <= 0x7F800000u) return r;
+    const u32 out = (ab & 0x7FFFFFFFu) > 0x7F800000u ? ab | 0x00400000u : (bb & 0x7FFFFFFFu) > 0x7F800000u ? bb | 0x00400000u : 0xFFC00000u;
+#if defined(__CUDA_ARCH__)
+    return __uint_as_float(out);
+#else
+    float f; __builtin_memcpy(&f, &out, 4); return f;
+#endif
+}
+
 // ------------------------------------------------------------------------------------------------
 // double-double accumulation (float aggregates: result within 1 ULP of the exact sum)
 // ------------------------------------------------------------------------------------------------

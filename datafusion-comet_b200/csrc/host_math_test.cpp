@@ -75,6 +75,16 @@ void hm_mul_i128_wrap(int64_t n, const i128* a, const i128* b, i128* out) {
 void hm_f64_total_lt(int64_t n, const uint64_t* a, const uint64_t* b, uint8_t* out) {
     for (int64_t i = 0; i < n; i++) out[i] = f64_total_key(a[i]) < f64_total_key(b[i]);
 }
+// Float32 a op b (0 add 1 sub 2 mul 3 div) as the device computes it: the host's IEEE result with every NaN replaced by the
+// device's canonical 0x7FFFFFFF, then f32_x86_nan
+void hm_f32_arith(int op, int64_t n, const float* a, const float* b, float* out) {
+    for (int64_t i = 0; i < n; i++) {
+        volatile float x = a[i], y = b[i];
+        float r = op == 0 ? x + y : op == 1 ? x - y : op == 2 ? x * y : x / y;
+        if (r != r) { const u32 canon = 0x7FFFFFFFu; __builtin_memcpy(&r, &canon, 4); }
+        out[i] = f32_x86_nan(a[i], b[i], r);
+    }
+}
 void hm_dd_sum(int64_t n, const double* v, double* out) {
     dd a = {0.0, 0.0};
     for (int64_t i = 0; i < n; i++) dd_add_double(a, v[i]);

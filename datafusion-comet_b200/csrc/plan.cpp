@@ -303,7 +303,6 @@ static bool cast_supported(const DType& from, const DType& to) {
     }
     if (from.is_integer() && to.is_decimal()) return true;
     if (from.is_decimal() && to.is_decimal()) return true;
-    if (from.is_decimal() && to.id == TypeId::Float64) return true;
     return false;
 }
 

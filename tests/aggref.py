@@ -167,8 +167,8 @@ def exprs_columns(table, dts):
         valid = np.array([v is not None for v in vals], dtype=bool)
         if dt.name == "DECIMAL":
             cols.append((O.dec_from_ints(vals), valid))
-        elif dt.name == "DOUBLE":
-            cols.append((np.array([0.0 if v is None else v for v in vals], dtype=np.float64), valid))
+        elif dt.name in ("DOUBLE", "FLOAT"):
+            cols.append((np.array([0.0 if v is None else v for v in vals], dtype=np.float64 if dt.name == "DOUBLE" else np.float32), valid))
         elif dt.name == "BOOL":
             cols.append((np.array([bool(v) for v in vals], dtype=bool), valid))
         elif dt.name == "STRING":
@@ -185,7 +185,7 @@ def node_values(node, cols):
     dt = node.dt
     if dt.name == "DECIMAL":
         return O.dec_to_ints(v, valid)
-    if dt.name == "DOUBLE":
+    if dt.name in ("DOUBLE", "FLOAT"):
         return [float(x) if ok else None for x, ok in zip(np.asarray(v, dtype=np.float64), valid)]
     if dt.name == "BOOL":
         return [bool(x) if ok else None for x, ok in zip(v, valid)]

@@ -11,8 +11,15 @@ from oracle import oracle as O
 LEGACY, TRY, ANSI = 0, 1, 2
 
 
+OVERFLOW, DIVIDE_BY_ZERO = "ARITHMETIC_OVERFLOW", "DIVIDE_BY_ZERO"
+
+
 class AnsiError(Exception):
-    pass
+    """A Spark error in ANSI mode.  `classes`: the error classes of the failing rows (a batch may fail for more than one reason)."""
+
+    def __init__(self, *classes):
+        super().__init__(*classes)
+        self.classes = set(classes) or {OVERFLOW}
 
 
 def _valid_and(a, b):
@@ -46,8 +53,8 @@ class Lit(Node):
         valid = np.full(n, self.v is not None)
         if self.dt.name == "DECIMAL":
             return O.dec_from_ints([self.v or 0] * n), valid
-        np_dt = {"INT8": np.int64, "INT16": np.int64, "INT32": np.int64, "INT64": np.int64, "DATE": np.int64, "DOUBLE": np.float64, "FLOAT": np.float32,
-                 "BOOL": np.bool_}[self.dt.name]
+        np_dt = {"INT8": np.int64, "INT16": np.int64, "INT32": np.int64, "INT64": np.int64, "DATE": np.int64, "TIMESTAMP": np.int64, "DOUBLE": np.float64,
+                 "FLOAT": np.float32, "BOOL": np.bool_}[self.dt.name]
         return np.full(n, self.v if self.v is not None else 0, dtype=np_dt), valid
 
 
@@ -93,7 +100,7 @@ class Arith(Node):
             try:
                 out, ov = O.decimal_div(a, av, lt.scale, b, bv, rt.scale, self.dt.scale, False, self.mode)
             except O.OracleError:
-                raise AnsiError()
+                raise AnsiError(DIVIDE_BY_ZERO)
             return out, ov.astype(bool)
         valid = av & bv
         if lt.name in ("DOUBLE", "FLOAT"):             # Legacy: IEEE; TRY / ANSI: checked_div (zero divisor -> NULL / DIVIDE_BY_ZERO)
@@ -102,7 +109,7 @@ class Arith(Node):
             if self.mode != LEGACY:
                 z = valid & (b == 0)
                 if self.mode == ANSI and z.any():
-                    raise AnsiError()
+                    raise AnsiError(DIVIDE_BY_ZERO)
                 out = np.where(z, 0, out).astype(a.dtype)
                 valid = valid & ~z
             return out, valid
@@ -111,7 +118,7 @@ class Arith(Node):
         bad = valid & ((b == 0) | ((a == mn) & (b == -1)))
         if bad.any():
             if self.mode == ANSI:
-                raise AnsiError()
+                raise AnsiError(*([DIVIDE_BY_ZERO] if (valid & (b == 0)).any() else []) + ([OVERFLOW] if (valid & (a == mn) & (b == -1)).any() else []))
             if self.mode == LEGACY:
                 raise ArrowError()
         safe_b = np.where(bad | (b == 0), 1, b)
@@ -146,6 +153,11 @@ class Arith(Node):
 
 
 def _total_key(x):
+    """IEEE totalOrder as a signed integer key, in the value's own width (a float32 NaN widened to float64 loses its signalling bit)"""
+    x = np.asarray(x)
+    if x.dtype == np.float32:
+        bits = np.ascontiguousarray(x).view(np.int32)
+        return bits ^ ((bits >> 31) & np.int32(0x7FFFFFFF))
     bits = np.ascontiguousarray(x, dtype=np.float64).view(np.int64)
     return bits ^ ((bits >> 63) & np.int64(0x7FFFFFFFFFFFFFFF))
 
@@ -255,6 +267,8 @@ class Cast(Node):
     def eval(self, cols):
         a, av = self.c.eval(cols)
         f, t = self.c.dt, self.dt
+        if f == t:
+            return a, av
         if f.name == "DECIMAL" and t.name == "DECIMAL":
             try:
                 out, ov = O.decimal_rescale_check(a, av, f.scale, t.precision, t.scale, self.mode == ANSI)
@@ -267,9 +281,10 @@ class Cast(Node):
             except O.OracleError:
                 raise AnsiError()
             return out, ov.astype(bool)
-        if t.name == "DOUBLE":
-            return a.astype(np.float64), av
-        if t.name == "FLOAT":
+        if t.name == "DOUBLE":      # integers (held as int64) round once; float32 widens exactly, NaNs keep sign and payload
+            with np.errstate(invalid="ignore"):         # a signalling NaN is made quiet
+                return a.astype(np.float64), av
+        if t.name == "FLOAT":       # integers only (the planner refuses double -> float)
             return a.astype(np.float32), av
         return a.astype(np.int64), av  # widening int casts
 
@@ -282,11 +297,18 @@ class If(Node):
         return P.if_(self.c.proto(), self.a.proto(), self.b.proto())
 
     def eval(self, cols):
-        (c, cv), (a, av), (b, bv) = self.c.eval(cols), self.a.eval(cols), self.b.eval(cols)
-        take = cv & c
-        if a.ndim == 2:
-            return np.where(take[:, None], a, b), np.where(take, av, bv)
-        return np.where(take, a, b), np.where(take, av, bv)
+        """each branch is evaluated on the rows that take it only (CaseExpr evaluates THEN under the selection), so an ANSI error
+        of a row that does not take a branch is not raised"""
+        c, cv = self.c.eval(cols)
+        take = np.asarray(cv & c, dtype=bool)
+        rows = lambda m: [(np.asarray(v)[m], np.asarray(ok)[m]) for v, ok in cols]
+        (a, av), (b, bv) = self.a.eval(rows(take)), self.b.eval(rows(~take))
+        a, b = np.asarray(a), np.asarray(b)
+        out = np.zeros((len(take),) + a.shape[1:], dtype=np.result_type(a, b))
+        out[take], out[~take] = a, b
+        valid = np.zeros(len(take), dtype=bool)
+        valid[take], valid[~take] = av, bv
+        return out, valid
 
 
 class In(Node):
@@ -300,14 +322,18 @@ class In(Node):
 
     def eval(self, cols):
         a, av = self.v.eval(cols)
-        vals = np.array(O.dec_to_ints(a), dtype=object) if self.v.dt.name == "DECIMAL" else a
+        name = self.v.dt.name
+        vals = np.array(O.dec_to_ints(a), dtype=object) if name == "DECIMAL" else a
+        fdt = {"FLOAT": (np.float32, np.uint32), "DOUBLE": (np.float64, np.uint64)}.get(name)
+        if fdt:                      # floats match by their bits: IEEE totalOrder equality (NaN IN (NaN) is TRUE, 0.0 IN (-0.0) is not)
+            vals = np.ascontiguousarray(a, dtype=fdt[0]).view(fdt[1])
         hit = np.zeros(len(av), dtype=bool)
         has_null = False
         for l in self.lits:
             if l.v is None:
                 has_null = True
             else:
-                hit |= np.asarray(vals == l.v, dtype=bool)
+                hit |= np.asarray(vals == (np.array(l.v, dtype=fdt[0]).view(fdt[1]) if fdt else l.v), dtype=bool)
         out = ~hit if self.negated else hit
         valid = av & (hit | (not has_null))
         return out, valid

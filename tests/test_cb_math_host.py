@@ -282,3 +282,24 @@ def test_overflow_certificate_against_every_row_order(hm, oracle):
     assert hm.hm_cert_level(C.c_int64(2), C.c_uint64(0), C.c_uint64((B >> 64) | (1 << 63)), C.c_int(38)) == 1     # two's-complement bound: exact
     assert hm.hm_cert_level(C.c_int64(2), C.c_uint64(0), C.c_uint64(B >> 64), C.c_int(38)) == 2                    # magnitude bound: may have wrapped
     assert hm.hm_cert_level(C.c_int64(3), C.c_uint64(0), C.c_uint64((B >> 64) | (1 << 63)), C.c_int(38)) == 2
+
+
+F32_NAN_EDGES = np.array([0x7FC00000, 0xFFC00000, 0x7FC0BEEF, 0x7F800001, 0xFF800123, 0x7F800000, 0xFF800000, 0x00000000, 0x80000000,
+                          0x00000001, 0x807FFFFF, 0x7F7FFFFF, 0x3F800000, 0xC0400000], dtype=np.uint32)   # NaNs (quiet, signalling,
+                                                                                                          # payloads, signs), +-Inf, +-0, subnormals
+
+
+@pytest.mark.parametrize("op", [0, 1, 2, 3])
+def test_f32_x86_nan_rule(hm, op):
+    """cb::f32_x86_nan turns the device's canonical NaN back into the bits numpy (x86 SSE, like the reference) returns: the first NaN
+    operand made quiet, else the default NaN 0xFFC00000 for an invalid operation.  Every pair of edge values, both operand orders."""
+    n = len(F32_NAN_EDGES)
+    a = np.repeat(F32_NAN_EDGES, n).view(np.float32).copy()
+    b = np.tile(F32_NAN_EDGES, n).view(np.float32).copy()
+    out = np.zeros(n * n, dtype=np.float32)
+    hm.hm_f32_arith(C.c_int(op), C.c_int64(n * n), _p(a), _p(b), _p(out))
+    with np.errstate(all="ignore"):
+        want = [a + b, a - b, a * b, a / b][op]
+    assert np.isnan(want).sum() > n       # the pairs reach NaN operands and invalid operations
+    bad = np.nonzero(out.view(np.uint32) != want.view(np.uint32))[0]
+    assert bad.size == 0, [(hex(a.view(np.uint32)[i]), hex(b.view(np.uint32)[i]), hex(out.view(np.uint32)[i]), hex(want.view(np.uint32)[i])) for i in bad[:4]]

@@ -11,6 +11,7 @@ import pyarrow.parquet as pq
 import pytest
 
 import partref
+from sources import device_table, scan_of, write_parquet
 
 pytestmark = pytest.mark.gpu
 
@@ -264,37 +265,6 @@ def test_chunks_smaller_than_the_input(cb, oracle):
 
 
 # ---- device tables ----------------------------------------------------------------------------------------------------------------------
-def device_table(cb, tbl, types, dec8=()):
-    """tbl's columns as caller-owned device buffers: booleans as bitmaps, dictionaries as their codes, decimals named in dec8 as 8 bytes"""
-    import torch
-    t = cb.native.DeviceTable(tbl.num_rows)
-    for name, dt in zip(tbl.column_names, types):
-        a = tbl.column(name).combine_chunks()
-        valid = np.asarray(a.is_valid())
-        vbits = np.packbits(valid, bitorder="little")
-        vdev = torch.from_numpy(np.concatenate([vbits, np.zeros(16, np.uint8)])).cuda() if a.null_count else None
-        dictionary = None
-        if pa.types.is_boolean(a.type):
-            raw, width = np.packbits(np.asarray(a.fill_null(False)), bitorder="little"), 0
-        elif pa.types.is_dictionary(a.type):
-            idx = a.indices
-            width = idx.type.bit_width // 8
-            raw = np.frombuffer(idx.buffers()[1], dtype=np.uint8)[idx.offset * width:(idx.offset + len(idx)) * width]
-            dictionary = a.dictionary.to_pylist()
-        elif pa.types.is_decimal(a.type):
-            v = np.frombuffer(a.buffers()[1], dtype=np.int64)[2 * a.offset:2 * (a.offset + len(a))].reshape(-1, 2)
-            if name in dec8:
-                raw, width = v[:, 0].copy().view(np.uint8), 8
-            else:
-                raw, width = v.copy().view(np.uint8).reshape(-1), 16
-        else:
-            width = a.type.bit_width // 8
-            raw = np.frombuffer(a.buffers()[1], dtype=np.uint8)[a.offset * width:(a.offset + len(a)) * width]
-        vals = torch.from_numpy(np.concatenate([np.ascontiguousarray(raw).view(np.uint8).reshape(-1), np.zeros(16, np.uint8)])).cuda()
-        t.add(dt, vals.data_ptr(), width, vdev.data_ptr() if vdev is not None else None, a.null_count, dictionary=dictionary, keep=(vals, vdev))
-    return t
-
-
 @pytest.mark.parametrize("keys,n_parts", [("b", 7), ("i8", 200), ("i16", 200), ("d9", 200), ("d18", 4096), ("d38", 7),
                                           ("s8+i32", 200), ("f32+s16+date+ts", 6145), ("d9+d18+i64+s32+f64", 2)])
 def test_device_tables(cb, oracle, keys, n_parts):
@@ -344,19 +314,6 @@ def parquet_table(n, seed):
         "row": (cols["row"][0], P.INT64),
     }
     return out
-
-
-def write_parquet(path, cols, as_int):
-    tbl = pa.table({k: cols[k][0] for k in cols})
-    pq.write_table(tbl, path, row_group_size=40_000, data_page_size=1 << 16, use_dictionary=["sd"], store_decimal_as_integer=as_int,
-                   compression="SNAPPY")
-    return tbl
-
-
-def scan_of(cb, cols, names, path):
-    """NativeScan reading `names` as their requested types"""
-    fields = [(k, cols[k][1], True) for k in names]
-    return cb.proto.native_scan(fields, fields, [path]), [cols[k][1] for k in names]
 
 
 def expected_table(cols, names):
