@@ -9,6 +9,7 @@
 #include "device/cb_math.h"
 #include "device/cb_delta.h"
 #include "device/cb_snappy.h"
+#include "device/cb_rle.h"
 #include <algorithm>
 
 namespace cb200 {
@@ -444,7 +445,7 @@ void launch_pq_snappy_segmented(PqPage* pages, int n_pages, unsigned* ckpt, int 
 }
 
 // ---- locate levels / values inside the page body ------------------------------------------------------------------------
-__global__ void k_pq_resolve(PqPage* pages, int n_pages) {
+__global__ void k_pq_resolve(PqPage* pages, int n_pages, int* err) {
     int pi = blockIdx.x * blockDim.x + threadIdx.x;
     if (pi >= n_pages) return;
     PqPage pg = pages[pi];
@@ -452,7 +453,10 @@ __global__ void k_pq_resolve(PqPage* pages, int n_pages) {
     int left = pg.body_bytes;
     if (pg.flags & PQ_PAGE_V1_LEVELS) {
         u32 dl = left >= 4 ? ((u32)v[0] | ((u32)v[1] << 8) | ((u32)v[2] << 16) | ((u32)v[3] << 24)) : 0u;
-        if (left < 4 || dl > (u32)(left - 4)) dl = 0; // malformed: the level decoders will report the row-count mismatch
+        // malformed: an optional column's rows all carry a level, so an empty level stream is as wrong as one past the page.  Reported
+        // here -- the level decoders read def_bytes = 0 as "no levels, every row valid", which is what a required column's page means.
+        if (left < 4 || dl > (u32)(left - 4)) { dl = 0; if (pg.num_values > 0) atomicOr(err, PQ_ERR_TRUNCATED); }
+        else if (dl == 0 && pg.num_values > 0) atomicOr(err, PQ_ERR_RLE);
         pages[pi].def_ptr = v + 4;
         pages[pi].def_bytes = (int)dl;
         v += 4 + dl;
@@ -462,8 +466,8 @@ __global__ void k_pq_resolve(PqPage* pages, int n_pages) {
     pages[pi].values_bytes = left;
     pages[pi].nonnull = pg.num_values;
 }
-void launch_pq_resolve(PqPage* pages, int n_pages, cudaStream_t st) {
-    if (n_pages > 0) k_pq_resolve<<<(n_pages + 127) / 128, 128, 0, st>>>(pages, n_pages);
+void launch_pq_resolve(PqPage* pages, int n_pages, int* err, cudaStream_t st) {
+    if (n_pages > 0) k_pq_resolve<<<(n_pages + 127) / 128, 128, 0, st>>>(pages, n_pages, err);
 }
 
 // ---- PLAIN / BYTE_STREAM_SPLIT ---------------------------------------------------------------------------------
@@ -651,38 +655,11 @@ void launch_pq_dbp(PqPage* pages, int n_pages, PqMiniblock* table, int conv, voi
     else k_pq_dbp_decode<PQ_I32_TO_I64><<<grid, block, 0, st>>>(pages, table, (u8*)out);
 }
 
-// ---- RLE / bit-packed hybrid ------------------------------------------------------------------------------------------
-// walk the run headers of [p, end): calls f(is_bit_packed, count, value, data_ptr); returns values seen
-template <typename F> __device__ long long walk_hybrid(const u8* p, const u8* end, int bit_width, long long max_values, F f) {
-    long long seen = 0;
-    const int vbytes = (bit_width + 7) / 8;
-    while (p < end && seen < max_values) {
-        u32 header = 0;
-        int shift = 0;
-        while (p < end) { // ULEB128
-            u8 b = *p++;
-            header |= (u32)(b & 0x7f) << shift;
-            shift += 7;
-            if (!(b & 0x80)) break;
-        }
-        if (header & 1) { // bit-packed: (header >> 1) groups of 8 values
-            long long count = (long long)(header >> 1) * 8;
-            long long take = count < max_values - seen ? count : max_values - seen;
-            f(1, (int)take, 0u, p);
-            p += (size_t)(header >> 1) * bit_width;
-            seen += take;
-        } else {
-            long long count = header >> 1;
-            u32 v = 0;
-            for (int k = 0; k < vbytes && p + k < end; k++) v |= (u32)p[k] << (8 * k);
-            p += vbytes;
-            long long take = count < max_values - seen ? count : max_values - seen;
-            f(0, (int)take, v, p);
-            seen += take;
-        }
-    }
-    return seen;
-}
+// ---- RLE / bit-packed hybrid (device/cb_rle.h) ------------------------------------------------------------------------
+// A page's runs go into its slice of the run table, which the decode kernels spread over warps.  The slice holds num_values / 8 + 64
+// runs: enough for every stream whose RLE runs repeat a value at least 8 times, as stock writers emit them.  Legal streams may hold
+// more (Encodings.md puts no lower bound on an RLE run's length); such a page gets run_counts[page] = -1 and its values are decoded
+// straight from the stream by k_pq_rle_direct, one warp per page, instead.
 
 // LEVELS = false: the dictionary indices of the page (first byte = bit width);  true: its definition levels (bit width 1)
 template <bool LEVELS> __global__ void k_pq_rle_scan(const PqPage* pages, int n_pages, PqRun* runs, int* run_counts, int* err) {
@@ -698,9 +675,8 @@ template <bool LEVELS> __global__ void k_pq_rle_scan(const PqPage* pages, int n_
     const int cap = LEVELS ? pg.def_max_runs : pg.max_runs;
     PqRun* out = runs + (LEVELS ? pg.def_run_base : pg.run_base);
     int n = 0;
-    bool truncated = false;
     long long row = pg.dst_row;
-    long long seen = bw > 32 ? -1 : walk_hybrid(p, end, bw, want, [&](int packed, int count, u32 value, const u8* data) {
+    const long long seen = walk_hybrid(p, end, bw, want, [&](int packed, int count, u32 value, const u8* data) {
         if (n < cap) {
             PqRun r;
             r.out_row = row;
@@ -709,15 +685,14 @@ template <bool LEVELS> __global__ void k_pq_rle_scan(const PqPage* pages, int n_
             r.value = value;
             r.bit_packed = packed;
             r.bit_width = bw;
-            if (packed && data + ((long long)count * bw + 7) / 8 > end) { r.count = 0; truncated = true; } // truncated page: never read beyond it
             out[n] = r;
         }
         n++;
         row += count;
     });
-    if (n > cap || seen != want) atomicOr(err, PQ_ERR_RLE);
-    if (truncated) atomicOr(err, PQ_ERR_TRUNCATED);
-    run_counts[pi] = n < cap ? n : cap;
+    if (seen == HYB_TRUNCATED) atomicOr(err, PQ_ERR_TRUNCATED);
+    else if (seen != want) atomicOr(err, PQ_ERR_RLE);
+    run_counts[pi] = seen != want ? 0 : n <= cap ? n : -1; // -1: decoded by k_pq_rle_direct
 }
 void launch_pq_rle_scan(const PqPage* pages, int n_pages, PqRun* runs, int* run_counts, int* err, cudaStream_t st) {
     if (n_pages > 0) k_pq_rle_scan<false><<<(n_pages + 63) / 64, 64, 0, st>>>(pages, n_pages, runs, run_counts, err);
@@ -742,21 +717,40 @@ template <int DW> __global__ void k_pq_rle_decode(const PqPage* pages, const PqR
         if (!r.bit_packed) {
             for (int i = lane; i < r.count; i += 32) store_dict<DW>(dict, dict_size, r.value, out, r.out_row + i, err);
         } else {
-            const u8* src = r.src;
-            const int bw = r.bit_width;
-            const long long nbytes = ((long long)r.count * bw + 7) / 8;
-            const u32 mask = bw >= 32 ? 0xffffffffu : ((1u << bw) - 1u);
-            for (int i = lane; i < r.count; i += 32) {
-                long long bit = (long long)i * bw;
-                const u8* q = src + (bit >> 3);
-                u64 w = 0;
-                for (int k = 0; k < 5; k++) if ((bit >> 3) + k < nbytes) w |= (u64)q[k] << (8 * k); // bw <= 32: value spans at most 5 bytes
-                u32 idx = (u32)(w >> (bit & 7)) & mask;
-                store_dict<DW>(dict, dict_size, idx, out, r.out_row + i, err);
-            }
+            const long long nbytes = ((long long)r.count * r.bit_width + 7) / 8;
+            for (int i = lane; i < r.count; i += 32) store_dict<DW>(dict, dict_size, hybrid_unpack(r.src, nbytes, i, r.bit_width), out, r.out_row + i, err);
         }
     }
 }
+
+// Pages whose runs did not fit their table (run_counts = -1): one warp walks the stream again -- every lane the same headers -- and the
+// lanes share each run's values.  DW = 0: definition levels -> valid[row];  DW = 4 / 8 / 16: dictionary indices -> dictionary values.
+// The scan already validated the stream, so every run the walk hands out lies inside the page.
+constexpr int RD_WARPS = 4;
+template <int DW> __global__ void __launch_bounds__(RD_WARPS * 32) k_pq_rle_direct(const PqPage* pages, int n_pages, const int* run_counts, const void* dict_all,
+                                                                                  void* out, int* err) {
+    const int pi = blockIdx.x * RD_WARPS + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (pi >= n_pages || run_counts[pi] >= 0) return;
+    const PqPage pg = pages[pi];
+    const u8* p = DW == 0 ? pg.def_ptr : pg.values;
+    const u8* end = p + (DW == 0 ? pg.def_bytes : pg.values_bytes);
+    const int bw = DW == 0 ? 1 : *p++;
+    const void* dict = (const u8*)dict_all + (size_t)pg.dict_off * (DW ? DW : 1);
+    long long row = pg.dst_row;
+    walk_hybrid(p, end, bw, DW == 0 ? pg.num_values : pg.nonnull, [&](int packed, int count, u32 value, const u8* data) {
+        const long long nbytes = ((long long)count * bw + 7) / 8;
+        for (int i = lane; i < count; i += 32) {
+            const u32 v = packed ? hybrid_unpack(data, nbytes, i, bw) : value;
+            if (DW == 0) ((u8*)out)[row + i] = (u8)(v & 1u);
+            else store_dict<DW ? DW : 4>(dict, pg.dict_size, v, out, row + i, err);
+        }
+        row += count;
+    });
+}
+template <int DW> static void rle_direct(const PqPage* pages, int n_pages, const int* run_counts, const void* dict, void* out, int* err, cudaStream_t st) {
+    k_pq_rle_direct<DW><<<(n_pages + RD_WARPS - 1) / RD_WARPS, RD_WARPS * 32, 0, st>>>(pages, n_pages, run_counts, dict, out, err);
+}
+
 void launch_pq_rle_decode(const PqPage* pages, int n_pages, const PqRun* runs, const int* run_counts, const void* dict, int dict_width, void* out, int* err,
                           cudaStream_t st) {
     if (n_pages <= 0) return;
@@ -764,6 +758,9 @@ void launch_pq_rle_decode(const PqPage* pages, int n_pages, const PqRun* runs, c
     if (dict_width == 4) k_pq_rle_decode<4><<<grid, block, 0, st>>>(pages, runs, run_counts, dict, out, err);
     else if (dict_width == 8) k_pq_rle_decode<8><<<grid, block, 0, st>>>(pages, runs, run_counts, dict, out, err);
     else k_pq_rle_decode<16><<<grid, block, 0, st>>>(pages, runs, run_counts, dict, out, err);
+    if (dict_width == 4) rle_direct<4>(pages, n_pages, run_counts, dict, out, err, st);
+    else if (dict_width == 8) rle_direct<8>(pages, n_pages, run_counts, dict, out, err, st);
+    else rle_direct<16>(pages, n_pages, run_counts, dict, out, err, st);
 }
 
 // ---- definition levels (flat optional columns: bit width 1) ---------------------------------------------------------------
@@ -773,15 +770,14 @@ __global__ void k_pq_check_def(const PqPage* pages, int n_pages, int* err) {
     if (pi >= n_pages) return;
     const PqPage pg = pages[pi];
     if (pg.def_bytes <= 0) return;
-    const u8* p = pg.def_ptr;
-    const u8* end = p + pg.def_bytes;
     bool bad = false;
-    long long seen = walk_hybrid(p, end, 1, pg.num_values, [&](int packed, int count, u32 value, const u8* data) {
+    const long long seen = walk_hybrid(pg.def_ptr, pg.def_ptr + pg.def_bytes, 1, pg.num_values, [&](int packed, int count, u32 value, const u8* data) {
         if (!packed) { if (value != 1u) bad = true; }
-        else for (int i = 0; i < count && data + (i >> 3) < end; i++) if (!((data[i >> 3] >> (i & 7)) & 1)) { bad = true; break; }
+        else for (int i = 0; i < count; i++) if (!((data[i >> 3] >> (i & 7)) & 1)) { bad = true; break; }
     });
     if (bad) atomicOr(err, PQ_ERR_NULL_ON_FAST_PATH);
-    if (seen != pg.num_values) atomicOr(err, PQ_ERR_RLE);
+    if (seen == HYB_TRUNCATED) atomicOr(err, PQ_ERR_TRUNCATED);
+    else if (seen != pg.num_values) atomicOr(err, PQ_ERR_RLE);
 }
 void launch_pq_check_def_levels(const PqPage* pages, int n_pages, int* err, cudaStream_t st) {
     if (n_pages > 0) k_pq_check_def<<<(n_pages + 63) / 64, 64, 0, st>>>(pages, n_pages, err);
@@ -837,6 +833,7 @@ void launch_pq_def_levels(PqPage* pages, int n_pages, PqRun* runs, int* run_coun
     if (n_pages <= 0) return;
     k_pq_rle_scan<true><<<(n_pages + 63) / 64, 64, 0, st>>>(pages, n_pages, runs, run_counts, err);
     k_pq_def_expand<<<dim3(32, (unsigned)n_pages), 256, 0, st>>>(pages, runs, run_counts, valid);
+    rle_direct<0>(pages, n_pages, run_counts, nullptr, valid, err, st);
     k_pq_def_index<<<n_pages, 256, 0, st>>>(pages, valid, idx);
 }
 

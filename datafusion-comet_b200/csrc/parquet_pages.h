@@ -12,11 +12,11 @@ enum { PQ_PAGE_V1_LEVELS = 1, PQ_PAGE_SN_SERIAL = 2, PQ_PAGE_SN_BAD = 4, PQ_PAGE
 
 // Bits the decode kernels set in the scan's error word.
 enum PqErr {
-    PQ_ERR_RLE = 1,               // malformed RLE / bit-packed stream, or more runs than the page's run table holds
+    PQ_ERR_RLE = 1,               // malformed RLE / bit-packed stream (or an empty v1 level stream on a page with values)
     PQ_ERR_NULL_ON_FAST_PATH = 2, // a NULL in a chunk whose statistics say null_count = 0
     PQ_ERR_DICT_INDEX = 4,        // dictionary index out of range
     PQ_ERR_SNAPPY = 8,            // malformed Snappy page
-    PQ_ERR_TRUNCATED = 16,        // fewer encoded values than the page header declares
+    PQ_ERR_TRUNCATED = 16,        // fewer encoded values than the page header declares (incl. bit-packed runs / v1 levels past the page)
     PQ_ERR_DELTA = 32,            // malformed DELTA_BINARY_PACKED page (sizes, bit width, value count, body past the page, table overflow)
     PQ_ERR_BSS = 64,              // BYTE_STREAM_SPLIT page whose size is not (non-null values) x (value width)
 };

@@ -435,7 +435,7 @@ struct NativeScanSource : ExecNode {
         if (perr & PQ_ERR_DELTA) throw PlanError("parquet: malformed DELTA_BINARY_PACKED page (block sizes, bit width, value count or a body past the page)");
         if (perr & PQ_ERR_BSS) throw PlanError("parquet: BYTE_STREAM_SPLIT page whose size is not (non-null values) x (value width)");
         if (perr & PQ_ERR_TRUNCATED) throw PlanError("parquet: truncated page (fewer encoded values than the page header declares)");
-        if (perr & PQ_ERR_RLE) throw Unsupported("parquet: malformed RLE stream, or one with more than n/8 + 64 runs per page");
+        if (perr & PQ_ERR_RLE) throw PlanError("parquet: malformed RLE / bit-packed stream (dictionary indices or definition levels)");
         out = std::move(cur->batch);
         return true;
     }
@@ -459,13 +459,13 @@ struct NativeScanSource : ExecNode {
         PqPage* data_pages = (PqPage*)cp.dpd;
         const PqPage* dict_pages = data_pages + n_data;
         uint8_t* dense = cp.null_aware ? cp.dense : !cp.segs.empty() ? cp.dcov : cp.out; // page-pruned: decoded into covered rows first
-        launch_pq_resolve(data_pages, n_all, ds);
+        launch_pq_resolve(data_pages, n_all, derr, ds);
         ctx->kernel_launches++;
         if (cp.n_dict_pages) { launch_pq_plain(dict_pages, (int)cp.n_dict_pages, cp.conv, cp.type_length, cp.ddict, derr, ds); ctx->kernel_launches++; }
         if (cp.optional && !cp.null_aware) { launch_pq_check_def_levels(data_pages, n_data, derr, ds); ctx->kernel_launches++; }
         if (cp.null_aware) {
             launch_pq_def_levels(data_pages, n_data, (PqRun*)cp.druns, (int*)cp.dcounts, cp.dvalid, (unsigned*)cp.didx, derr, ds);
-            ctx->kernel_launches += 3;
+            ctx->kernel_launches += 4;
             col.validity = view(sl, cp.validity, cp.validity_bytes);
             col.null_count = -1;
         }
@@ -473,7 +473,7 @@ struct NativeScanSource : ExecNode {
         if (cp.run_base > 0) {
             launch_pq_rle_scan(data_pages, n_data, (PqRun*)cp.runs, (int*)cp.counts, derr, ds);
             launch_pq_rle_decode(data_pages, n_data, (const PqRun*)cp.runs, (const int*)cp.counts, cp.ddict, cp.out_w, dense, derr, ds);
-            ctx->kernel_launches += 2;
+            ctx->kernel_launches += 3;
         }
         if (cp.mb_base > 0) { // DELTA_BINARY_PACKED pages: header walk, miniblock sums, carries, decode
             launch_pq_dbp(data_pages, n_data, (PqMiniblock*)cp.dmb, cp.conv, dense, derr, ds);

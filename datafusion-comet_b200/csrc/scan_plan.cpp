@@ -709,10 +709,16 @@ class ColumnPlanner {
         if (pg.type == pq::DATA_PAGE) {
             // v1: [u32 length + definition levels (optional columns)] [values], compressed as one block
             if (optional) d.flags |= PQ_PAGE_V1_LEVELS;
+            // the level decoders read the RLE / bit-packed hybrid behind a u32 length; deprecated BIT_PACKED levels have neither
+            if (optional && pg.def_encoding != pq::RLE)
+                throw Unsupported("parquet definition level encoding " + std::to_string(pg.def_encoding) + " (column '" + field.name + "'): only RLE levels are read");
         } else {
             // v2: repetition + definition levels sit uncompressed in front of the (optionally compressed) values
             const int lv = pg.rep_levels_bytes + pg.def_levels_bytes;
             if (lv > pg.compressed_size || lv > pg.uncompressed_size) throw PlanError("parquet: data page v2 level sizes exceed the page");
+            // every row of an optional column has a level; without any, the page would read as a required column's (Arrow refuses it too)
+            if (optional && pg.def_levels_bytes <= 0 && pg.num_values > 0)
+                throw PlanError("parquet: data page v2 of optional column '" + field.name + "' has no definition levels");
             d.def_ptr = s.dev + pg.rep_levels_bytes;
             d.def_bytes = pg.def_levels_bytes;
             vals = {s.host + lv, s.dev + lv, s.comp - lv, s.unc - lv, pg.v2_compressed ? s.codec : (int)pq::UNCOMPRESSED};

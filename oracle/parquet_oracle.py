@@ -7,7 +7,7 @@ RLE_DICTIONARY), `Compression.md` (SNAPPY = raw snappy block) and google/snappy 
 Parity status: pinned on CPU against pyarrow's reader (Arrow C++, an independent implementation) over the same files the GPU
 tests use (tests/test_parquet_cpu.py); NOT pinned against the reference itself (cannot be built here).
 
-Scope = what the device decoder covers: flat columns, data pages v1 / v2, UNCOMPRESSED / SNAPPY, PLAIN and dictionary
+Scope = what the device decoder covers: flat columns, data pages v1 / v2, UNCOMPRESSED / SNAPPY / ZSTD (through pyarrow), PLAIN and dictionary
 encodings, INT32 / INT64 / FLOAT / DOUBLE / FIXED_LEN_BYTE_ARRAY (decimals) / BYTE_ARRAY (dictionary strings)."""
 import struct
 
@@ -74,7 +74,8 @@ class _T:
 def page_header(buf, pos):
     """-> (dict, position of the first byte after the header)"""
     t = _T(buf, pos)
-    h = {"type": None, "uncompressed": 0, "compressed": 0, "num_values": 0, "encoding": 0, "def_bytes": 0, "rep_bytes": 0, "v2_compressed": True}
+    h = {"type": None, "uncompressed": 0, "compressed": 0, "num_values": 0, "encoding": 0, "def_encoding": 3, "def_bytes": 0, "rep_bytes": 0,
+         "v2_compressed": True}
 
     def sub(fields):
         def f(fid, ty):
@@ -93,7 +94,7 @@ def page_header(buf, pos):
         elif fid == 3:
             h["compressed"] = t.zigzag()
         elif fid == 5:
-            t.struct(sub({1: "num_values", 2: "encoding"}))
+            t.struct(sub({1: "num_values", 2: "encoding", 3: "def_encoding"}))
         elif fid == 7:
             t.struct(sub({1: "num_values", 2: "encoding"}))
         elif fid == 8:
@@ -202,6 +203,16 @@ def plain(buf, phys, n, type_length=0):
     raise ValueError(phys)
 
 
+def _decompress(codec, raw, n):
+    if codec == "SNAPPY":
+        return snappy_decompress(raw)
+    if codec == "ZSTD":                                                          # Compression.md: a zstd frame; not restated here
+        import pyarrow as pa
+        return pa.decompress(raw, n, codec="zstd", asbytes=True)
+    assert codec == "UNCOMPRESSED", codec
+    return raw
+
+
 # ---- one column chunk ----------------------------------------------------------------------------------------------------
 def decode_chunk(file_bytes, start, total_compressed, num_values, phys, codec, optional, type_length=0):
     """-> (values as a numpy array with None-equivalent 0 at NULL rows, valid bool array).  `start` = dictionary_page_offset or
@@ -215,15 +226,16 @@ def decode_chunk(file_bytes, start, total_compressed, num_values, phys, codec, o
         raw = file_bytes[body:body + h["compressed"]]
         pos = body + h["compressed"]
         if h["type"] == 2:                                                       # DICTIONARY_PAGE
-            data = snappy_decompress(raw) if codec == "SNAPPY" else raw
+            data = _decompress(codec, raw, h["uncompressed"])
             dictionary = plain(data, phys, h["num_values"], type_length)
             continue
         if h["type"] not in (0, 3):
             continue
         n = h["num_values"]
         if h["type"] == 0:                                                       # v1: levels inside the compressed body
-            data = snappy_decompress(raw) if codec == "SNAPPY" else raw
+            data = _decompress(codec, raw, h["uncompressed"])
             if optional:
+                assert h["def_encoding"] == 3, "definition levels other than RLE (BIT_PACKED) are refused"
                 (dl,) = struct.unpack_from("<I", data, 0)
                 levels = rle_hybrid(data[4:4 + dl], 1, n)
                 data = data[4 + dl:]
@@ -231,10 +243,11 @@ def decode_chunk(file_bytes, start, total_compressed, num_values, phys, codec, o
                 levels = np.ones(n, dtype=np.int64)
         else:                                                                    # v2: levels uncompressed, in front
             lv = h["rep_bytes"] + h["def_bytes"]
-            levels = rle_hybrid(raw[h["rep_bytes"]:lv], 1, n) if optional and h["def_bytes"] else np.ones(n, dtype=np.int64)
+            assert not (optional and n and not h["def_bytes"]), "data page v2 of an optional column without definition levels"
+            levels = rle_hybrid(raw[h["rep_bytes"]:lv], 1, n) if optional else np.ones(n, dtype=np.int64)
             data = raw[lv:]
-            if codec == "SNAPPY" and h["v2_compressed"]:
-                data = snappy_decompress(data)
+            if h["v2_compressed"]:
+                data = _decompress(codec, data, h["uncompressed"] - lv)
         nn = int(levels.sum())
         if h["encoding"] == 0:
             dense = plain(data, phys, nn, type_length)
