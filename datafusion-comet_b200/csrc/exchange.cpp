@@ -13,6 +13,7 @@
 
 #include "abi_internal.h"
 #include "exec.h"
+#include "exec_internal.h"
 
 #include <dlfcn.h>
 #include <nccl.h>
@@ -163,23 +164,76 @@ int64_t cb200_exchange_layout(const int64_t* counts, int32_t world, int32_t me, 
     return total;
 }
 
+// Every rank must post the same sends and receives, so the list of buffers an exchange moves is derived from the map plan alone:
+// per column its values (the Arrow width of the type; BOOL one byte per row) and a validity byte per row -- all 1 where the local
+// column has no validity.  Whether a rank's column carries validity depends on its data (a dense Partial drops it when it saw no
+// NULL), so it is never consulted.  A map plan that emitted no batch takes part with zero rows of its output schema.
 cb200_table* cb200_exchange(cb200_comm* c, cb200_plan* plan, int64_t* n_rows_out, cb200_exchange_stats* stats, cb200_error* err) {
     return cb200_guarded(err, [&]() -> cb200_table* {
         if (!c || !plan) throw PlanError("cb200_exchange: null handle");
         TraceSpan ts("exchange");
         const int world = c->world, me = c->rank;
+        // ---- refusals that depend on the plan only, all before the first collective: a refused plan leaves no peer waiting ----------
+        const Operator& op = *plan->op;
+        if (op.kind != OpKind::ShuffleWriter) throw PlanError("cb200_exchange: the map plan is not a ShuffleWriter (run a ShuffleWriter plan with num_partitions = world size)");
+        if (op.num_partitions != world) throw PlanError("cb200_exchange: the ShuffleWriter has " + std::to_string(op.num_partitions) + " partitions, the communicator " + std::to_string(world) + " ranks");
+        for (const DType& t : op.schema)
+            if (t.is_string()) throw Unsupported("exchange of string columns (per-rank dictionaries differ)");
+        if (cb200_plan_ctx(plan).device != c->device)
+            throw PlanError("cb200_exchange: the map plan runs on device " + std::to_string(cb200_plan_ctx(plan).device) + ", the communicator on device " + std::to_string(c->device));
         const std::vector<int64_t>& starts = cb200_plan_ctx(plan).partition_starts;
+        const bool emitted = !starts.empty();
+        if (!emitted && !plan->finished) throw PlanError("cb200_exchange: the map plan has not been executed (run it until it returns its batch or end of stream)");
         Batch& b = cb200_plan_last(plan);
-        if ((int)starts.size() != world + 1) throw PlanError("cb200_exchange: the plan's last batch has " + std::to_string(starts.empty() ? 0 : starts.size() - 1) + " partitions, the communicator " + std::to_string(world) + " ranks (run a ShuffleWriter plan with num_partitions = world size first)");
+        if (emitted && ((int)starts.size() != world + 1 || (starts[(size_t)world] > starts[0] && b.cols.size() != op.schema.size())))
+            throw ExecError(15, "", "internal: the ShuffleWriter's last batch does not match its plan");
+        std::vector<int64_t> local_starts = emitted ? starts : std::vector<int64_t>((size_t)world + 1, 0);
+        const int64_t local_rows = local_starts[(size_t)world] - local_starts[0];
+        // ---- the buffers this rank moves: the same list on every rank ------------------------------------------------------------------
         cuda_check(cudaSetDevice(c->device), "cudaSetDevice");
         cudaStream_t st = c->stream;
+        set_alloc_stream(st);
+        struct Move { const char* src; char* dst; size_t w; };
+        std::vector<Move> moves;
+        DeviceBufP ones; // the validity bytes of a local column without validity
+        for (size_t j = 0; j < op.schema.size(); j++) {
+            const DType& t = op.schema[j];
+            const bool is_bool = t.id == TypeId::Bool;
+            const size_t w = is_bool ? 1 : (size_t)t.arrow_width();
+            const char *src = nullptr, *vsrc = nullptr;
+            if (local_rows > 0) { // the layouts to_arrow_layout left behind after cb200_execute / cb200_execute_device; a rank with no rows
+                                  // sends nothing, so nothing about its (possibly absent) columns can fail on it alone
+                const Column& col = b.cols[j];
+                if (col.on_host || col.is_dict || col.offsets || col.type != t) throw ExecError(15, "", "internal: ShuffleWriter column " + std::to_string(j) + " is not a device column of its plan type");
+                if (is_bool) {
+                    if (!col.bool_bytes) throw ExecError(15, "", "internal: boolean column of a ShuffleWriter batch without its byte form");
+                    src = (const char*)col.bool_bytes->ptr;
+                } else {
+                    if (!col.data || (size_t)phys_bytes(col.phys) != w) throw ExecError(15, "", "internal: ShuffleWriter column " + std::to_string(j) + " is not in the Arrow layout of " + t.str());
+                    src = (const char*)col.data->ptr;
+                }
+                if (col.validity && !col.valid_bytes) throw ExecError(15, "", "internal: nullable column of a ShuffleWriter batch without byte-per-row validity");
+                if (col.valid_bytes) vsrc = (const char*)col.valid_bytes->ptr;
+                else {
+                    if (!ones) {
+                        ones = std::make_shared<DeviceBuf>((size_t)local_starts[(size_t)world] + 16);
+                        cuda_check(cudaMemsetAsync(ones->ptr, 1, ones->bytes, st), "memset validity bytes");
+                    }
+                    vsrc = (const char*)ones->ptr;
+                }
+            }
+            moves.push_back({src, nullptr, w});
+            moves.push_back({vsrc, nullptr, 1});
+        }
         // the map plan's kernels are done (cb200_execute* synchronises), but order the streams explicitly anyway
-        cuda_check(cudaEventRecord(c->ready, cb200_plan_ctx(plan).stream), "event record");
-        cuda_check(cudaStreamWaitEvent(st, c->ready, 0), "stream wait");
+        if (local_rows > 0) {
+            cuda_check(cudaEventRecord(c->ready, cb200_plan_ctx(plan).stream), "event record");
+            cuda_check(cudaStreamWaitEvent(st, c->ready, 0), "stream wait");
+        }
         // ---- counts: the N x N matrix of rows rank s holds for rank p --------------------------------------------------------------
         std::vector<int64_t> recv_counts((size_t)world), recv_off((size_t)world);
         int64_t n_recv = 0;
-        for (int p = 0; p < world; p++) c->h_counts[p] = starts[(size_t)p + 1] - starts[(size_t)p];
+        for (int p = 0; p < world; p++) c->h_counts[p] = local_starts[(size_t)p + 1] - local_starts[(size_t)p];
         if (world > 1) {
             cuda_check(cudaMemcpyAsync(c->d_counts, c->h_counts, (size_t)world * 8, cudaMemcpyHostToDevice, st), "counts H2D");
             nccl_check(nccl().AllGather(c->d_counts, c->d_counts + world, (size_t)world, ncclInt64, c->comm, st), "ncclAllGather(counts)");
@@ -191,41 +245,28 @@ cb200_table* cb200_exchange(cb200_comm* c, cb200_plan* plan, int64_t* n_rows_out
             recv_off[0] = 0;
             n_recv = recv_counts[0];
         }
-        // ---- receive buffers = the Final plan's input table ------------------------------------------------------------------------------
-        set_alloc_stream(st);
+        // ---- receive buffers = the Final plan's input table: values + validity bytes of every column, packed at first use ---------------
         auto table = std::make_shared<DeviceTable>();
         table->n_rows = n_recv;
-        struct Move { const char* src; char* dst; size_t w; };
-        std::vector<Move> moves;
+        table->needs_packing = true;
         const size_t alloc_rows = (size_t)std::max<int64_t>(n_recv, 1);
         int64_t bytes_sent = 0, bytes_recv = 0;
-        for (auto& col : b.cols) {
-            if (col.on_host) throw Unsupported("exchange of host-resident columns (small dense aggregate states are gathered, not exchanged)");
-            if (col.is_dict) throw Unsupported("exchange of dictionary-coded string columns (per-rank dictionaries differ)");
-            if (col.offsets) throw Unsupported("exchange of plain string columns");
+        for (size_t j = 0; j < op.schema.size(); j++) {
             Column o;
-            o.type = col.type;
-            o.phys = col.phys;
-            o.null_count = col.validity || col.valid_bytes ? -1 : 0;
-            const bool is_bool = col.type.id == TypeId::Bool;
-            if (is_bool) {
-                if (!col.bool_bytes) throw ExecError(15, "", "internal: boolean column of a ShuffleWriter batch without its byte form");
-                o.bool_bytes = std::make_shared<DeviceBuf>(alloc_rows + 16);
+            o.type = op.schema[j];
+            o.null_count = -1;
+            Move& values = moves[2 * j];
+            if (o.type.id == TypeId::Bool) {
                 o.phys = Phys::Bitmap;
-                moves.push_back({(const char*)col.bool_bytes->ptr, (char*)o.bool_bytes->ptr, 1});
-                table->needs_packing = true;
+                o.bool_bytes = std::make_shared<DeviceBuf>(alloc_rows + 16);
+                values.dst = (char*)o.bool_bytes->ptr;
             } else {
-                const size_t w = (size_t)phys_bytes(col.phys);
-                if (w == 0 || !col.data) throw ExecError(15, "", "internal: column without a fixed-width device form in an exchange");
-                o.data = std::make_shared<DeviceBuf>(alloc_rows * w + 16);
-                moves.push_back({(const char*)col.data->ptr, (char*)o.data->ptr, w});
+                o.phys = phys_of(o.type);
+                o.data = std::make_shared<DeviceBuf>(alloc_rows * values.w + 16);
+                values.dst = (char*)o.data->ptr;
             }
-            if (col.validity) {
-                if (!col.valid_bytes) throw ExecError(15, "", "internal: nullable column of a ShuffleWriter batch without byte-per-row validity");
-                o.valid_bytes = std::make_shared<DeviceBuf>(alloc_rows + 16);
-                moves.push_back({(const char*)col.valid_bytes->ptr, (char*)o.valid_bytes->ptr, 1});
-                table->needs_packing = true;
-            }
+            o.valid_bytes = std::make_shared<DeviceBuf>(alloc_rows + 16);
+            moves[2 * j + 1].dst = (char*)o.valid_bytes->ptr;
             table->cols.push_back(o);
         }
         // ---- payload: per buffer, segment p -> rank p --------------------------------------------------------------------------------------
@@ -234,8 +275,8 @@ cb200_table* cb200_exchange(cb200_comm* c, cb200_plan* plan, int64_t* n_rows_out
             nccl_check(nccl().GroupStart(), "ncclGroupStart");
             for (auto& m : moves)
                 for (int p = 0; p < world; p++) {
-                    const size_t sb = (size_t)(starts[(size_t)p + 1] - starts[(size_t)p]) * m.w, rb = (size_t)recv_counts[(size_t)p] * m.w;
-                    if (sb) nccl_check(nccl().Send(m.src + (size_t)starts[(size_t)p] * m.w, sb, ncclInt8, p, c->comm, st), "ncclSend");
+                    const size_t sb = (size_t)(local_starts[(size_t)p + 1] - local_starts[(size_t)p]) * m.w, rb = (size_t)recv_counts[(size_t)p] * m.w;
+                    if (sb) nccl_check(nccl().Send(m.src + (size_t)local_starts[(size_t)p] * m.w, sb, ncclInt8, p, c->comm, st), "ncclSend");
                     if (rb) nccl_check(nccl().Recv(m.dst + (size_t)recv_off[(size_t)p] * m.w, rb, ncclInt8, p, c->comm, st), "ncclRecv");
                     bytes_sent += (int64_t)sb;
                     bytes_recv += (int64_t)rb;
@@ -251,11 +292,15 @@ cb200_table* cb200_exchange(cb200_comm* c, cb200_plan* plan, int64_t* n_rows_out
         }
         cuda_check(cudaEventRecord(c->ev1, st), "event record");
         cuda_check(cudaStreamSynchronize(st), "exchange sync"); // the map plan may be released and the table bound right after this call
+        // the table may outlive the communicator, whose stream cb200_comm_destroy destroys: its buffers are freed on the default stream
+        for (Column& o : table->cols)
+            for (DeviceBuf* buf : {o.data.get(), o.bool_bytes.get(), o.valid_bytes.get()})
+                if (buf) buf->stream = nullptr;
         if (n_rows_out) *n_rows_out = n_recv;
         if (stats) {
             float ms = 0;
             cudaEventElapsedTime(&ms, c->ev0, c->ev1);
-            stats->rows_sent = starts[(size_t)world] - starts[0];
+            stats->rows_sent = local_rows;
             stats->rows_received = n_recv;
             stats->bytes_sent = bytes_sent;
             stats->bytes_received = bytes_recv;

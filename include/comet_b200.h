@@ -142,11 +142,20 @@ typedef struct cb200_exchange_stats {
     int64_t bytes_sent, bytes_received; /* payload bytes incl. the segment this rank keeps */
     double payload_ms;                  /* CUDA-event duration of the grouped send/recv on the communicator's stream */
 } cb200_exchange_stats;
-/* The exchange itself.  `map_plan` is a ShuffleWriter(HashPartitioning(keys, world)) plan whose last cb200_execute_device batch is
- * still alive: its rows are ordered by partition id = pmod(murmur3(keys, 42), world).  Every rank calls this collectively; rank r gets
- * back a device table (owned by the library, release with cb200_table_release) holding partition r of every rank, sources in rank
- * order, rows in their map-side order -- ready to be bound as the input of the Final plan with cb200_plan_bind_table.
- * Fixed-width columns only (aggregate state: keys, sums, counts, flags).  Returns NULL on error. */
+/* The exchange itself.  `map_plan` is a ShuffleWriter(HashPartitioning(keys, world)) plan whose last cb200_execute /
+ * cb200_execute_device batch is still alive: its rows are ordered by partition id = pmod(murmur3(keys, 42), world).  Every rank calls
+ * this exactly once per map plan, collectively -- also when its map plan produced no batch (an empty partition, a filter that removed
+ * every row): that rank takes part with zero rows of the plan's output schema.  Rank r gets back a device table (owned by the
+ * library, release with cb200_table_release) holding partition r of every rank, sources in rank order, rows in their map-side order
+ * -- ready to be bound as the input of the Final plan with cb200_plan_bind_table.
+ * Every column travels as its values (the Arrow width of its type, BOOL one byte per row) plus one validity byte per row, whether or
+ * not the local column has NULLs, so every rank moves the same list of buffers and every received column has validity:
+ * bytes_sent = rows x sum(width + 1).  Fixed-width columns only (aggregate state: keys, sums, counts, flags): a plan with string
+ * columns (CB200_ERR_UNSUPPORTED), a plan that is not a ShuffleWriter or whose num_partitions is not the world size, a plan created
+ * for another device than the communicator's, and a plan that was never executed (CB200_ERR_PLAN) are refused before any collective, so a refusal leaves no peer waiting.
+ * Only the last batch moves: a map plan that emits more than one batch (a ShuffleWriter over a Scan larger than
+ * spark.comet.b200.chunkRows, or over a join) is not exchanged whole.  A ShuffleWriter over a grouped Partial emits one batch.
+ * Returns NULL on error. */
 cb200_table* cb200_exchange(cb200_comm* comm, cb200_plan* map_plan, int64_t* n_rows_out, cb200_exchange_stats* stats, cb200_error* err);
 /* receive layout of that exchange from the gathered N x N count matrix (counts[s * world + p] = rows rank s holds for rank p):
  * fills recv_counts / recv_offsets (either may be NULL), returns the rows rank `me` receives.  Pure host arithmetic. */
