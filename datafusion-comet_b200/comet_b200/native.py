@@ -66,12 +66,14 @@ class Stats(C.Structure):
                 ("scan_pruned_row_groups", C.c_int64), ("scan_pruned_rows", C.c_int64), ("agg_strategies", C.c_int64),
                 ("scan_pruned_pages", C.c_int64), ("scan_page_pruned_rows", C.c_int64), ("sort_rows", C.c_int64),
                 ("sort_passes", C.c_int64), ("sort_pass_rows", C.c_int64), ("sort_select_rows", C.c_int64),
-                ("join_build_rows", C.c_int64), ("join_probe_rows", C.c_int64), ("join_out_rows", C.c_int64)]
+                ("join_build_rows", C.c_int64), ("join_probe_rows", C.c_int64), ("join_out_rows", C.c_int64),
+                ("agg_range_levels", C.c_int64), ("agg_range_reruns", C.c_int64)]
 AGG_DENSE, AGG_TABLE, AGG_STREAM, AGG_MIGRATED = 1, 2, 4, 8  # cb200_stats.agg_strategies bits (CB200_AGG_*)
+RANGE_TIGHT, RANGE_TYPE, RANGE_SAFE = 1, 2, 4  # cb200_stats.agg_range_levels bits (CB200_RANGE_*)
 
 
 EXPORTED = ["cb200_comm_unique_id", "cb200_comm_create", "cb200_comm_destroy", "cb200_comm_rank", "cb200_comm_world", "cb200_nccl_info", "cb200_exchange",
-            "cb200_exchange_layout", "cb200_comm_allgather_small", "cb200_plan_stats", "cb200_register_memory_file", "cb200_parquet_describe", "cb200_table_add_column_bytes", "cb200_plan_dict_value", "cb200_plan_partition_starts", "cb200_compile_plan_assume", "cb200_version", "cb200_supports", "cb200_create_plan", "cb200_plan_num_columns", "cb200_execute",
+            "cb200_exchange_layout", "cb200_comm_allgather_small", "cb200_plan_stats", "cb200_register_memory_file", "cb200_parquet_describe", "cb200_table_add_column_bytes", "cb200_plan_dict_value", "cb200_plan_partition_starts", "cb200_compile_plan_assume", "cb200_reset_range_profiles", "cb200_version", "cb200_supports", "cb200_create_plan", "cb200_plan_num_columns", "cb200_execute",
             "cb200_release", "cb200_table_create", "cb200_table_add_column", "cb200_plan_bind_table",
             "cb200_table_release", "cb200_execute_device", "cb200_plan_kernel_launches", "cb200_compile_plan",
             "cb200_plan_kernel_source"]
@@ -181,6 +183,11 @@ def parquet_describe(path):
     if f(path.encode(), buf, cap, C.byref(err)) < 0:
         _raise(err)
     return json.loads(buf.value.decode())
+
+
+def reset_range_profiles():
+    """Forget the value ranges earlier dense aggregates left for later plans with the same pipeline (cb200_reset_range_profiles)."""
+    lib().cb200_reset_range_profiles()
 
 
 def kernel_source(op_bytes, index=0):

@@ -357,8 +357,12 @@ int cb200_plan_stats(cb200_plan* plan, cb200_stats* out) {
     out->join_build_rows = c.join_build_rows;
     out->join_probe_rows = c.join_probe_rows;
     out->join_out_rows = c.join_out_rows;
+    out->agg_range_levels = c.agg_range_levels;
+    out->agg_range_reruns = c.agg_range_reruns;
     return 0;
 }
+
+void cb200_reset_range_profiles(void) { reset_range_profiles(); }
 
 int cb200_compile_plan(const uint8_t* op_proto, size_t op_len, char* keys_out, size_t keys_cap, cb200_error* err) {
     return cb200_guarded(err, [&]() -> int {

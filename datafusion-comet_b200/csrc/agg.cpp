@@ -17,6 +17,11 @@ namespace cb200 {
 static std::mutex g_profile_mu;
 static std::map<std::string, std::vector<int>> g_range_profile;
 
+void reset_range_profiles() {
+    std::lock_guard<std::mutex> lk(g_profile_mu);
+    g_range_profile.clear();
+}
+
 namespace {
 
 enum class Strategy { Undecided, Dense, Table, Stream };
@@ -658,7 +663,7 @@ struct AggNode : FusedBase {
             }
             const int64_t max_rows = (int64_t)ctx->num_sms * k.g.threads * (1ll << CB_RPT_LOG2) / 1024 * 1024;
             int64_t r0 = row0;
-            while (r0 < row1 && launch_one(b, r0, std::min(row1, r0 + max_rows), n_groups, k)) r0 += max_rows;
+            while (r0 < row1 && launch_one(b, r0, std::min(row1, r0 + max_rows), n_groups, k, lv)) r0 += max_rows;
             if (r0 >= row1) return;
             if (lv == SAFE) throw ExecError(15, "", "internal: value-mask validation failed without assumptions");
             lv = lv == TIGHT ? TYPE : SAFE; // widen: observed ranges -> declared precision -> no assumption (fully checked code)
@@ -668,7 +673,7 @@ struct AggNode : FusedBase {
     }
 
     // false: the launch broke an assumption its kernel was specialised for and was discarded
-    bool launch_one(Batch& b, int64_t r0, int64_t r1, int n_groups, const Kernel& k) {
+    bool launch_one(Batch& b, int64_t r0, int64_t r1, int n_groups, const Kernel& k, Level lv) {
         cudaStream_t st = ctx->stream;
         size_t tot_bytes = (size_t)n_groups * n_words * 16;
         if (!have_totals()) {
@@ -695,7 +700,11 @@ struct AggNode : FusedBase {
         ctx->pipeline_rows += r1 - r0;
         ValueMasks masks;
         copy_vmask(masks);
-        ctx->check_device_errors(); // synchronises
+        // A launch that broke its assumptions computed on truncated values (a 16-byte 2^64 read as 64-bit 0 is a zero divisor): the
+        // errors it raised are dropped with it, and the re-run raises whatever the input really causes.  This takes every flag raised
+        // since the last synchronisation: aggregate_input checks after each consume and cb_fold raises nothing, so all of them are this
+        // launch's.  A kernel that raises errors must not be enqueued between two launch_one calls without a check of its own.
+        const int errs = ctx->take_device_errors(); // synchronises
         // validate the assumptions this kernel was specialised for; either way, remember what was seen so a retry is specialised correctly
         const std::vector<int> seen = mask_bits(k.spec, masks);
         bool ok = true;
@@ -705,8 +714,11 @@ struct AggNode : FusedBase {
         if (!ok) {
             // discard this launch: partials are simply not folded; the exact-escape accumulators must be cleared
             cuda_check(cudaMemsetAsync(dense.spill->ptr, 0, dense.spill->bytes, st), "memset spill");
+            ctx->agg_range_reruns++;
             return false;
         }
+        ctx->raise_device_errors(errs);
+        ctx->agg_range_levels |= lv == TIGHT ? CB200_RANGE_TIGHT : lv == TYPE ? CB200_RANGE_TYPE : CB200_RANGE_SAFE;
         rows_scanned += r1 - r0;
         cb::FinParams fp;
         memset(&fp, 0, sizeof(fp));

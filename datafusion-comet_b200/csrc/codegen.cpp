@@ -109,7 +109,7 @@ struct Emitter {
             u128r b = RSAT;
             if (c.type.is_decimal()) {
                 if (c.assume_bits > 0 && c.assume_bits < 127) b = (u128r)1 << c.assume_bits; // (v ^ sign) < 2^k  =>  |v| <= 2^k
-                if (c.phys == Phys::I64 || c.phys == Phys::I32) b = std::min(b, R63 - 1); // narrow storage always fits
+                if (c.phys == Phys::I64 || c.phys == Phys::I32) b = std::min(b, R63); // narrow storage: |v| <= 2^63 (INT64_MIN)
             }
             col_bounds.push_back(b);
             col_masked.push_back(s.sink == SinkKind::Agg && c.type.is_decimal());
@@ -587,8 +587,8 @@ struct Emitter {
         r.n = c.n;
         const DType& t = c.type;
         if (t.is_decimal()) {
-            if (c.narrow) { r.v = decln("-" + c.v); r.narrow = true; } // |v| < 2^63: cannot overflow
-            else r.v = declw("cb::i128_neg(" + c.v + ")");
+            if (c.narrow && bound_of(*e.children[0]) < R63) { r.v = decln("-" + c.v); r.narrow = true; } // |v| < 2^63: cannot overflow
+            else r.v = declw("cb::i128_neg(" + W(c) + ")"); // an i64 holding INT64_MIN negates to 2^63
         }
         else if (t.is_float()) r.v = decl(t, (t.id == TypeId::Float64 ? "cb::f64_neg(" : "cb::f32_neg(") + c.v + ")"); // exact sign flip, see cb_math.h
         else if (t.id == TypeId::Int64) r.v = decl(t, "(cb::i64)(0ull - (cb::u64)" + c.v + ")");
@@ -1120,6 +1120,8 @@ GeneratedKernel generate_pipeline_uncached(const PipelineSpec& spec) {
                     std::string key = v.type.is_decimal() ? (v.narrow ? v.v : "(cb::i64)" + v.v + ".lo")
                                       : v.type.id == TypeId::Float64 ? "cb::f64_total_key((cb::u64)__double_as_longlong(" + v.v + "))"
                                                                      : "(cb::i64)" + v.v;
+                    // the words hold 64-bit keys: a decimal(p <= 18) value outside them (invalid input) is refused, never compared by its low word
+                    if (v.type.is_decimal() && !v.narrow) em.raise(use + " && !cb::i128_fits_i64(" + v.v + ")", 6);
                     bool mn = a.kind == AggKind::Min;
                     std::string sk = std::string(mn ? "min|" : "max|") + v.v + "|" + condkey;
                     bool first = slots.dedup.count(std::to_string((int)(mn ? W_MIN : W_MAX)) + "|" + sk) == 0;
@@ -1215,6 +1217,7 @@ GeneratedKernel generate_pipeline_uncached(const PipelineSpec& spec) {
                                       : s.type.id == TypeId::Float64 ? "cb::f64_total_key((cb::u64)__double_as_longlong(" + s.v + "))"
                                                                      : "(cb::i64)" + s.v;
                     const std::string ok = s.n.empty() ? "true" : "!" + s.n;
+                    if (s.type.is_decimal() && !s.narrow) em.raise(ok + " && !cb::i128_fits_i64(" + s.v + ")", 6);
                     upd(mn ? "min" : "max", ok, L.w_minmax, key);
                     upd("count", ok, L.w_cnt);
                     break;

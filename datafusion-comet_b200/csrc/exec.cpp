@@ -9,7 +9,8 @@
 namespace cb200 {
 
 // error bits raised by kernels (device/cb_kernels.cuh set_err)
-enum { ERR_I128_OVERFLOW = 0, ERR_ANSI_OVERFLOW = 1, ERR_ORDER_DEPENDENT = 2, ERR_DIVIDE_BY_ZERO = 3, ERR_ARROW_DIVIDE_BY_ZERO = 4, ERR_DICT_CODE = 5 };
+enum { ERR_I128_OVERFLOW = 0, ERR_ANSI_OVERFLOW = 1, ERR_ORDER_DEPENDENT = 2, ERR_DIVIDE_BY_ZERO = 3, ERR_ARROW_DIVIDE_BY_ZERO = 4, ERR_DICT_CODE = 5,
+       ERR_WIDE_MINMAX = 6 };
 
 bool trace_on() {
     static int on = -1;
@@ -131,13 +132,17 @@ void ExecContext::collect_timing() {
     ev_pending = false;
 }
 
-void ExecContext::check_device_errors() {
+int ExecContext::take_device_errors() {
     cuda_check(cudaMemcpyAsync(h_err, d_err, sizeof(int), cudaMemcpyDeviceToHost, stream), "error flag copy");
     cuda_check(cudaStreamSynchronize(stream), "stream sync");
     collect_timing();
     int e = *h_err;
+    if (e) cudaMemsetAsync(d_err, 0, sizeof(int), stream);
+    return e;
+}
+
+void ExecContext::raise_device_errors(int e) {
     if (!e) return;
-    cudaMemsetAsync(d_err, 0, sizeof(int), stream);
     if (e & (1 << ERR_ANSI_OVERFLOW))
         throw ExecError(10, "ARITHMETIC_OVERFLOW", "[ARITHMETIC_OVERFLOW] overflow in ANSI mode");
     if (e & (1 << ERR_DIVIDE_BY_ZERO)) // SparkError::DivideByZero (spark-expr/src/error.rs)
@@ -148,6 +153,8 @@ void ExecContext::check_device_errors() {
         throw ExecError(11, "", "Arrow error: Arithmetic overflow: Overflow happened on decimal arithmetic"); // arrow-arith checked ops
     if (e & (1 << ERR_DICT_CODE)) // a valid row's dictionary code outside its dictionary: the input batch is malformed
         throw ExecError(3, "", "dictionary code out of range: a non-NULL row of a dictionary-encoded string column has a code outside its dictionary");
+    if (e & (1 << ERR_WIDE_MINMAX)) // MIN / MAX keep 64-bit keys for decimal(p <= 18); the reference compares the full i128
+        throw Unsupported("MIN / MAX of a decimal(p <= 18) input whose value does not fit 64 bits (outside its declared precision)");
     if (e & (1 << ERR_ORDER_DEPENDENT))
         throw ExecError(12, "", "SUM/AVG overflow here depends on the row order (some orderings of these rows overflow, others do not); "
                                 "the reference adds in row order -- the row-ordered fallback is not built yet, so the plan is refused rather than guessed");

@@ -38,6 +38,7 @@ bool trace_on();
 double now_ms();
 void set_alloc_stream(cudaStream_t s); // stream used by DeviceBuf allocations made on this thread
 size_t release_cached_device_memory();  // frees the library's recycled large blocks on the current device; returns the bytes released
+void reset_range_profiles();            // forgets the value ranges dense aggregates left for later plans with the same pipeline (agg.cpp)
 
 struct DeviceBuf {
     void* ptr = nullptr;
@@ -135,11 +136,15 @@ struct ExecContext {
     int64_t scan_pruned_row_groups = 0, scan_pruned_rows = 0; // Parquet row groups skipped by statistics (parquet_exec.rs:143-196)
     int64_t scan_pruned_pages = 0, scan_page_pruned_rows = 0;  // data pages / rows of kept row groups skipped by the page index
     int64_t agg_strategies = 0;   // CB200_AGG_* bits of the aggregate strategies that ran
+    int64_t agg_range_levels = 0; // CB200_RANGE_* bits of the dense launches kept
+    int64_t agg_range_reruns = 0; // dense launches discarded by value-mask validation
     int64_t sort_rows = 0, sort_passes = 0, sort_pass_rows = 0; // rows Sort operators radix-sorted, the digit passes they ran, rows moved
     int64_t sort_select_rows = 0; // rows TopK's radix select read (one read per digit step)
     int64_t join_build_rows = 0, join_probe_rows = 0, join_out_rows = 0; // hash joins: rows drained from the build side, rows probed, rows out
     std::vector<int64_t> partition_starts; // last ShuffleWriter batch: partition p = rows [starts[p], starts[p+1])
-    void check_device_errors();
+    void check_device_errors() { raise_device_errors(take_device_errors()); }
+    int take_device_errors();           // synchronises; returns the error flags the kernels raised so far and clears them
+    void raise_device_errors(int e);    // throws the error the flags `e` stand for (none: returns)
     void collect_timing();
 };
 

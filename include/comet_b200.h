@@ -205,11 +205,16 @@ typedef struct cb200_stats {
     int64_t join_build_rows;   /* rows HashJoin operators drained from their build side into the hash table's input */
     int64_t join_probe_rows;   /* probe-side rows they looked up */
     int64_t join_out_rows;     /* rows they emitted */
+    int64_t agg_range_levels;  /* OR of CB200_RANGE_* over the dense aggregate launches that were kept: which value-range assumptions ran */
+    int64_t agg_range_reruns;  /* dense aggregate launches discarded because their input broke the value range the kernel assumed */
 } cb200_stats;
 #define CB200_AGG_DENSE 1      /* thread-private accumulators over dictionary / bool key codes (and ungrouped aggregates) */
 #define CB200_AGG_TABLE 2      /* global key table */
 #define CB200_AGG_STREAM 4     /* one state row per run of equal keys */
 #define CB200_AGG_MIGRATED 8   /* a dense aggregate outgrew its group limit and moved to hashing mid-stream */
+#define CB200_RANGE_TIGHT 1    /* kernel specialised to the observed value bits + 2 */
+#define CB200_RANGE_TYPE 2     /* kernel specialised to the declared decimal precision */
+#define CB200_RANGE_SAFE 4     /* fully checked kernel, no value-range assumption */
 int cb200_plan_stats(cb200_plan* plan, cb200_stats* out);
 
 /* The library recycles device blocks >= 1 MiB on a per-device free list instead of returning them to the driver (a query step
@@ -217,6 +222,11 @@ int cb200_plan_stats(cb200_plan* plan, cb200_stats* out);
  * framework in the same process needs the memory.  Returns the bytes released.  No reference equivalent (the reference's memory
  * pools are host-side, native/core/src/execution/memory_pools/). */
 int64_t cb200_release_cached_memory(int32_t device_ordinal);
+
+/* A dense decimal aggregate over a batch of more than 2 Mi rows leaves the value ranges it observed for the next plan with the same
+ * pipeline, which then starts from them instead of sampling (a guess every launch still validates).  This forgets them, so that what
+ * a plan runs does not depend on the plans before it: for tests and diagnostics. */
+void cb200_reset_range_profiles(void);
 
 /* Build-time: generate and NVRTC-compile (sm_90a; needs no GPU) every pipeline kernel the plan would
  * use for null-free inputs; cubins land in the JIT cache that ships with the library.  Writes the

@@ -34,6 +34,8 @@ def test_stats_struct_matches_the_header(cb):
     bits = dict(re.findall(r"#define CB200_AGG_([A-Z]+) (\d+)", hdr))
     n = cb.native
     assert {k: int(v) for k, v in bits.items()} == {"DENSE": n.AGG_DENSE, "TABLE": n.AGG_TABLE, "STREAM": n.AGG_STREAM, "MIGRATED": n.AGG_MIGRATED}
+    levels = dict(re.findall(r"#define CB200_RANGE_([A-Z]+) (\d+)", hdr))
+    assert {k: int(v) for k, v in levels.items()} == {"TIGHT": n.RANGE_TIGHT, "TYPE": n.RANGE_TYPE, "SAFE": n.RANGE_SAFE}
 
 
 def test_version(cb):
