@@ -66,7 +66,7 @@ EXPR_FIELD = dict(literal=2, bound=3, add=4, subtract=5, multiply=6, divide=7, c
                   lt=13, lt_eq=14, is_null=15, is_not_null=16, **{"and": 17, "or": 18}, sort_order=19, check_overflow=25, like=26,
                   scalarFunc=31, caseWhen=38, **{"in": 39, "not": 40}, unary_minus=41, **{"if": 44}, unbound=51)  # expr.proto:30-109
 AGG_FIELD = dict(count=2, sum=3, min=4, max=5, avg=6)  # expr.proto:143-176
-OP_FIELD = dict(scan=100, projection=101, filter=102, sort=103, hash_agg=104, limit=105, shuffle_writer=106, hash_join=109,
+OP_FIELD = dict(scan=100, projection=101, filter=102, sort=103, hash_agg=104, limit=105, shuffle_writer=106, sort_merge_join=108, hash_join=109,
                 native_scan=111, shuffle_scan=116)  # operator.proto:32-86
 LITERAL_FIELD = dict(bool_val=1, byte_val=2, short_val=3, int_val=4, long_val=5, float_val=6, double_val=7,
                      string_val=8, bytes_val=9, decimal_val=10, datatype=12, is_null=13)  # literal.proto:26-47
@@ -341,6 +341,16 @@ def hash_join(left, right, left_keys, right_keys, join_type, build_side, conditi
     if null_aware:
         body += f_bool(6, True)
     return _op("hash_join", body, (left, right), plan_id)
+
+
+def sort_merge_join(left, right, left_keys, right_keys, join_type, sort_options, condition=None, plan_id=0):
+    """SortMergeJoin operator.proto:765-771: children (left, right), key expressions of each side, one SortOrder expression per key
+    (sort_order(...)).  The condition is field 5 here (4 in HashJoin)."""
+    body = b"".join(f_len(1, k) for k in left_keys) + b"".join(f_len(2, k) for k in right_keys) + f_varint(3, join_type)
+    body += b"".join(f_len(4, o) for o in sort_options)
+    if condition is not None:
+        body += f_len(5, condition)
+    return _op("sort_merge_join", body, (left, right), plan_id)
 
 
 def struct_field(name, dt, nullable=True):  # SparkStructField operator.proto:97

@@ -381,6 +381,17 @@ template <typename I> __global__ void k_gather_bits(const u8* in_bits, const I* 
     if (i < n) out_bytes[i] = bit_at(in_bits, (i64)row_idx[i]) ? 1 : 0;
 }
 
+// the gathers of NULL-extended join columns: row index CB_NULL_ROW gives zero value bytes and a clear bit.  Kept apart from the gathers
+// above, which Sort, repartitioning and inner joins run.
+template <typename T> __global__ void k_gather_rows_or_null(const T* in, const u32* row_idx, i64 n, T* out) {
+    i64 i = (i64)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) { const u32 r = row_idx[i]; out[i] = r == CB_NULL_ROW ? T{} : in[r]; }
+}
+__global__ void k_gather_bits_or_null(const u8* in_bits, const u32* row_idx, i64 n, u8* out_bytes) {
+    i64 i = (i64)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) { const u32 r = row_idx[i]; out_bytes[i] = r != CB_NULL_ROW && (!in_bits || bit_at(in_bits, (i64)r)) ? 1 : 0; }
+}
+
 i64 partition_chunks(i64 n) { const i64 nb = (n + 1023) / 1024; return (nb + PID_CHUNK - 1) / PID_CHUNK; }
 cudaError_t launch_partition(const HashKeyCols& kc, i64 n, u32 n_parts, u32* hashes, u32* pids, i32* block_hist, i64* block_base, i64* chunk_tmp,
                              i64* starts, i64* row_idx, cudaStream_t st) {
@@ -419,6 +430,19 @@ void launch_gather_bits(const void* in_bits, const i64* row_idx, i64 n, void* ou
 }
 void launch_gather_bits(const void* in_bits, const u32* row_idx, i64 n, void* out_bytes, cudaStream_t st) {
     if (n > 0) k_gather_bits<u32><<<(unsigned)((n + 255) / 256), 256, 0, st>>>((const u8*)in_bits, row_idx, n, (u8*)out_bytes);
+}
+
+void launch_gather_or_null(const void* in, int width, const u32* row_idx, i64 n, void* out, cudaStream_t st) {
+    if (n <= 0) return;
+    unsigned blocks = (unsigned)((n + 255) / 256);
+    if (width == 16) k_gather_rows_or_null<ulonglong2><<<blocks, 256, 0, st>>>((const ulonglong2*)in, row_idx, n, (ulonglong2*)out);
+    else if (width == 8) k_gather_rows_or_null<u64><<<blocks, 256, 0, st>>>((const u64*)in, row_idx, n, (u64*)out);
+    else if (width == 4) k_gather_rows_or_null<u32><<<blocks, 256, 0, st>>>((const u32*)in, row_idx, n, (u32*)out);
+    else if (width == 2) k_gather_rows_or_null<u16><<<blocks, 256, 0, st>>>((const u16*)in, row_idx, n, (u16*)out);
+    else k_gather_rows_or_null<u8><<<blocks, 256, 0, st>>>((const u8*)in, row_idx, n, (u8*)out);
+}
+void launch_gather_bits_or_null(const void* in_bits, const u32* row_idx, i64 n, void* out_bytes, cudaStream_t st) {
+    if (n > 0) k_gather_bits_or_null<<<(unsigned)((n + 255) / 256), 256, 0, st>>>((const u8*)in_bits, row_idx, n, (u8*)out_bytes);
 }
 
 // ---- sort: packed row keys, stable LSD radix sort -----------------------------------------------------------------------------------------
@@ -719,36 +743,57 @@ __device__ __forceinline__ i64 join_find(const JoinTable& t, const u64* k) {
         if (eq) return r;
     }
 }
-__global__ void __launch_bounds__(256) k_join_probe(JoinTable t, const u64* keys, i64 n, int mode, u32* counts, u32* run_of, u64* total, u8* keep) {
+__global__ void __launch_bounds__(256) k_join_probe(JoinTable t, const u64* keys, i64 n, int mode, u32* counts, u32* run_of, u64* total, u8* keep,
+                                                    u8* hit) {
     const i64 i = (i64)blockIdx.x * blockDim.x + threadIdx.x;
+    const bool pairs = mode == CB_JOIN_COUNT || mode == CB_JOIN_OUTER;
     u64 c = 0;
     if (i < n) {
         u64 k[SK_MAX_WORDS];
 #pragma unroll
         for (int j = 0; j < SK_MAX_WORDS; j++) k[j] = j < t.words ? keys[i * t.words + j] : 0;
         const i64 r = join_find(t, k);
-        if (mode == CB_JOIN_COUNT) {
-            c = r < 0 ? 0 : t.run_start[r + 1] - t.run_start[r];
+        if (pairs) {
+            c = r < 0 ? (mode == CB_JOIN_OUTER ? 1 : 0) : t.run_start[r + 1] - t.run_start[r];
             counts[i] = (u32)c;
             run_of[i] = r < 0 ? 0xffffffffu : (u32)r;
+            if (hit && r >= 0) hit[r] = 1; // plain stores: every writer stores the same value
         } else keep[i] = (r >= 0) == (mode == CB_JOIN_SEMI);
     }
-    if (mode != CB_JOIN_COUNT) return;
+    if (!pairs) return;
 #pragma unroll
     for (int o = 16; o; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
     if ((threadIdx.x & 31) == 0 && c) atomicAdd((unsigned long long*)total, (unsigned long long)c);
 }
-__global__ void k_join_emit(JoinTable t, const u32* run_of, const u32* offs, const u32* chunk_off, i64 n, i64 o0, i64 o1, u32* probe_idx, u32* build_idx) {
+__global__ void k_join_emit(JoinTable t, const u32* run_of, const u32* offs, const u32* chunk_off, i64 n, i64 o0, i64 o1, int outer, u32* probe_idx,
+                            u32* build_idx) {
     const i64 i = (i64)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const u32 r = run_of[i];
-    if (r == 0xffffffffu) return;
-    const i64 b0 = t.run_start[r], c = (i64)t.run_start[r + 1] - b0, off = (i64)offs[i] + chunk_off[i >> 12];
+    const i64 off = (i64)offs[i] + chunk_off[i >> 12];
+    if (r == 0xffffffffu) { // no match: an outer join's one NULL-extended pair
+        if (outer && off >= o0 && off < o1) { probe_idx[off - o0] = (u32)i; build_idx[off - o0] = CB_NULL_ROW; }
+        return;
+    }
+    const i64 b0 = t.run_start[r], c = (i64)t.run_start[r + 1] - b0;
     const i64 lo = max(off, o0), hi = min(off + c, o1);
     for (i64 p = lo; p < hi; p++) {
         probe_idx[p - o0] = (u32)i;
         build_idx[p - o0] = t.rows[b0 + (p - off)];
     }
+}
+// keep[rows[p]] = the run holding sorted position p was never hit.  The run is found by binary search over run_start, one thread per
+// position: a run may hold most of the build side.
+__global__ void k_join_unmatched(const u32* run_start, i64 n_runs, const u32* rows, const u8* hit, i64 m, u8* keep) {
+    const i64 p = (i64)blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= m) return;
+    i64 lo = 0, hi = n_runs - 1; // the last run starting at or before p
+    while (lo < hi) {
+        const i64 mid = (lo + hi + 1) >> 1;
+        if ((i64)run_start[mid] <= p) lo = mid;
+        else hi = mid - 1;
+    }
+    keep[rows[p]] = !hit[lo];
 }
 void launch_join_heads(const u64* keys, int words, i64 m, u8* head, cudaStream_t st) {
     if (m > 0) k_join_heads<<<(unsigned)((m + 255) / 256), 256, 0, st>>>(keys, words, m, head);
@@ -756,12 +801,15 @@ void launch_join_heads(const u64* keys, int words, i64 m, u8* head, cudaStream_t
 void launch_join_insert(const JoinTable& t, i64 n_runs, cudaStream_t st) {
     if (n_runs > 0) k_join_insert<<<(unsigned)((n_runs + 255) / 256), 256, 0, st>>>(t, n_runs);
 }
-void launch_join_probe(const JoinTable& t, const u64* keys, i64 n, int mode, u32* counts, u32* run_of, u64* total, u8* keep, cudaStream_t st) {
-    if (n > 0) k_join_probe<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(t, keys, n, mode, counts, run_of, total, keep);
+void launch_join_probe(const JoinTable& t, const u64* keys, i64 n, int mode, u32* counts, u32* run_of, u64* total, u8* keep, u8* hit, cudaStream_t st) {
+    if (n > 0) k_join_probe<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(t, keys, n, mode, counts, run_of, total, keep, hit);
 }
-void launch_join_emit(const JoinTable& t, const u32* run_of, const u32* offs, const u32* chunk_off, i64 n, i64 o0, i64 o1, u32* probe_idx, u32* build_idx,
-                      cudaStream_t st) {
-    if (n > 0 && o1 > o0) k_join_emit<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(t, run_of, offs, chunk_off, n, o0, o1, probe_idx, build_idx);
+void launch_join_emit(const JoinTable& t, const u32* run_of, const u32* offs, const u32* chunk_off, i64 n, i64 o0, i64 o1, bool outer, u32* probe_idx,
+                      u32* build_idx, cudaStream_t st) {
+    if (n > 0 && o1 > o0) k_join_emit<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(t, run_of, offs, chunk_off, n, o0, o1, outer, probe_idx, build_idx);
+}
+void launch_join_unmatched(const u32* run_start, i64 n_runs, const u32* rows, const u8* hit, i64 m, u8* keep, cudaStream_t st) {
+    if (m > 0) k_join_unmatched<<<(unsigned)((m + 255) / 256), 256, 0, st>>>(run_start, n_runs, rows, hit, m, keep);
 }
 
 template <int W> static cudaError_t sort_pass(const RadixScratch& s, i64 n, int digit, int from, bool first, cudaStream_t st) {

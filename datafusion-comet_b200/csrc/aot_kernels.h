@@ -56,6 +56,11 @@ void launch_gather(const void* in, int width, const long long* row_idx, long lon
 void launch_gather(const void* in, int width, const unsigned* row_idx, long long n, void* out, cudaStream_t st);
 void launch_gather_bits(const void* in_bits, const long long* row_idx, long long n, void* out_bytes, cudaStream_t st);
 void launch_gather_bits(const void* in_bits, const unsigned* row_idx, long long n, void* out_bytes, cudaStream_t st);
+// the same for NULL-extended join output: row index CB_NULL_ROW gives zero bytes (launch_gather_or_null) or 0 (launch_gather_bits_or_null).
+// in_bits == nullptr (a column without a validity bitmap) reads as all set.
+enum : unsigned { CB_NULL_ROW = 0xffffffffu };
+void launch_gather_or_null(const void* in, int width, const unsigned* row_idx, long long n, void* out, cudaStream_t st);
+void launch_gather_bits_or_null(const void* in_bits, const unsigned* row_idx, long long n, void* out_bytes, cudaStream_t st);
 
 // ---- sort (SortExec / TopK): packed row keys (device/cb_sortkey.h), stable LSD radix sort of (key, row index) ----------------------------
 // k_sort_keys: kc.words 64-bit words per row into keys[n * words]; and_or[0, words) ANDs and and_or[words, 2 * words) ORs them over
@@ -105,15 +110,21 @@ struct JoinTable {
 void launch_join_heads(const unsigned long long* keys, int words, long long m, unsigned char* head, cudaStream_t st);
 // every run r < n_runs whose key has no NULL field gets one slot
 void launch_join_insert(const JoinTable& t, long long n_runs, cudaStream_t st);
-enum { CB_JOIN_COUNT = 0, CB_JOIN_SEMI = 1, CB_JOIN_ANTI = 2 };
+enum { CB_JOIN_COUNT = 0, CB_JOIN_SEMI = 1, CB_JOIN_ANTI = 2, CB_JOIN_OUTER = 3 };
 // one lookup per probe key (NULL fields match nothing).  CB_JOIN_COUNT: counts[i] = matching build rows, run_of[i] = their run (~0 when
-// none), *total += the sum of counts (64-bit; the caller zeroes it).  CB_JOIN_SEMI / ANTI: keep[i] = a match exists / none does.
+// none), *total += the sum of counts (64-bit; the caller zeroes it).  CB_JOIN_OUTER: the same, but a row without a match counts 1.
+// CB_JOIN_SEMI / ANTI: keep[i] = a match exists / none does.  hit (n_runs bytes, or nullptr): hit[run] = 1 for every run found.
 void launch_join_probe(const JoinTable& t, const unsigned long long* keys, long long n, int mode, unsigned* counts, unsigned* run_of,
-                       unsigned long long* total, unsigned char* keep, cudaStream_t st);
-// inner join pairs at output positions [o0, o1): probe row i's matches occupy [off_i, off_i + count_i), off_i = offs[i] + chunk_off[i / 4096]
-// (launch_scan_u32 over the counts); probe_idx[p - o0] = i, build_idx[p - o0] = the build row, in build input order
+                       unsigned long long* total, unsigned char* keep, unsigned char* hit, cudaStream_t st);
+// join pairs at output positions [o0, o1): probe row i's matches occupy [off_i, off_i + count_i), off_i = offs[i] + chunk_off[i / 4096]
+// (launch_scan_u32 over the counts); probe_idx[p - o0] = i, build_idx[p - o0] = the build row, in build input order.  outer: a row
+// without a match gives one pair whose build row is CB_NULL_ROW.
 void launch_join_emit(const JoinTable& t, const unsigned* run_of, const unsigned* offs, const unsigned* chunk_off, long long n, long long o0,
-                      long long o1, unsigned* probe_idx, unsigned* build_idx, cudaStream_t st);
+                      long long o1, bool outer, unsigned* probe_idx, unsigned* build_idx, cudaStream_t st);
+// keep[rows[p]] = 1 for every sorted build position p < m whose run (run_start[0, n_runs)) has no hit: the build rows no probe row matched,
+// NULL keys included (their runs are not in the table)
+void launch_join_unmatched(const unsigned* run_start, long long n_runs, const unsigned* rows, const unsigned char* hit, long long m,
+                           unsigned char* keep, cudaStream_t st);
 
 // device values -> the Arrow layout of their logical type, rows [0, n): what the hand-off (Arrow export, cb200_execute_device) gives out
 enum { CB_SEXT32_TO_128, CB_SEXT64_TO_128, CB_NARROW32_TO_8, CB_NARROW32_TO_16, CB_BITS_TO_BYTES };

@@ -140,7 +140,7 @@ struct ExecContext {
     int64_t agg_range_reruns = 0; // dense launches discarded by value-mask validation
     int64_t sort_rows = 0, sort_passes = 0, sort_pass_rows = 0; // rows Sort operators radix-sorted, the digit passes they ran, rows moved
     int64_t sort_select_rows = 0; // rows TopK's radix select read (one read per digit step)
-    int64_t join_build_rows = 0, join_probe_rows = 0, join_out_rows = 0; // hash joins: rows drained from the build side, rows probed, rows out
+    int64_t join_build_rows = 0, join_probe_rows = 0, join_out_rows = 0; // hash and sort-merge joins: rows drained from the build side, rows probed, rows out
     std::vector<int64_t> partition_starts; // last ShuffleWriter batch: partition p = rows [starts[p], starts[p+1])
     void check_device_errors() { raise_device_errors(take_device_errors()); }
     int take_device_errors();           // synchronises; returns the error flags the kernels raised so far and clears them

@@ -176,7 +176,7 @@ ExecNodeP make_partition_node(const OperatorP& op, const ExecNodeP& child, ExecC
 ExecNodeP make_sort_node(const OperatorP& op, const ExecNodeP& child, ExecContext* ctx);
 ExecNodeP make_join_node(const OperatorP& op, const ExecNodeP& left, const ExecNodeP& right, ExecContext* ctx);
 
-// ---- row primitives shared by repartitioning, Sort and HashJoin (rows.cpp) ------------------------------------------
+// ---- row primitives shared by repartitioning, Sort and the joins (rows.cpp) ------------------------------------------
 // The HK_* kind of a key column (device/cb_sortkey.h).  The logical type decides how Spark hashes a value (utils.rs: i8 / i16 / i32 /
 // date as i32, decimal(p <= 18) as i64, wider decimals as 16 bytes) and how many bits its sort key takes; the stored layout (DESIGN.md,
 // "Data layout in HBM") decides how it is read.
@@ -193,6 +193,10 @@ Batch drain(ExecNode& child, ExecContext* ctx, const char* op, const char* conca
 // (the byte forms are kept: the exchange sends them).  `op` names the operator in the refusal of plain Utf8 columns.  I: long long or
 // unsigned.
 template <typename I> void gather_columns(const Batch& in, const I* row_idx, int64_t n, Batch& out, ExecContext* ctx, const char* op);
+// gather_columns for the columns of a join side that may be NULL-extended: row index CB_NULL_ROW gives a NULL, and every column gets a
+// validity bitmap (byte form kept) whether or not a row is NULL, so its layout is the same in every batch.  Plain Utf8 never gets here
+// (arrive refuses it).
+void gather_columns_or_null(const Batch& in, const unsigned* row_idx, int64_t n, Batch& out, ExecContext* ctx);
 // the rows of bs in one batch (`bs` non-empty, every batch on the device): values and validity appended in order; dictionary-coded strings
 // that carry different Dictionary objects are recoded into one (the first batch's entries, then the others' new entries)
 Batch concat_batches(const std::vector<Batch>& bs, ExecContext* ctx, const char* op);

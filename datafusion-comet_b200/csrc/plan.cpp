@@ -573,6 +573,58 @@ static StructField decode_struct_field(PbReader r) { // SparkStructField operato
     return f;
 }
 
+// one SortOrder expression (expr.proto:385-389): the Sort operator's keys and the sort-merge join's sort options
+static SortKey decode_sort_order(PbReader e) {
+    bool have_order = false;
+    SortKey k;
+    while (e.next()) {
+        if (e.field != 19 || e.wire != 2) { e.skip(); continue; }
+        have_order = true;
+        PbReader so = e.sub();
+        while (so.next()) {
+            if (so.field == 1) k.expr = decode_expr(so.sub());
+            else if (so.field == 2) k.descending = so.i64() == 1;
+            else if (so.field == 3) k.nulls_first = so.i64() == 0;
+            else so.skip();
+        }
+    }
+    if (!have_order || !k.expr) throw PlanError("sort key is not a SortOrder with a child");
+    return k;
+}
+
+// the checks HashJoin and SortMergeJoin share before their own: two children, key lists, join type (`what` names the operator)
+static void decode_join(Operator& op, const std::string& what, int64_t join_type) {
+    if (op.children.size() != 2) throw PlanError(what + " expects two children");
+    if (op.left_keys.empty()) throw PlanError(what + " without keys");
+    if (op.left_keys.size() != op.right_keys.size())
+        throw PlanError(what + " with " + std::to_string(op.left_keys.size()) + " left keys and " + std::to_string(op.right_keys.size()) + " right keys");
+    if (join_type < 0 || join_type > 5) throw PlanError("unknown join type " + std::to_string(join_type));
+    op.join_type = (JoinType)join_type;
+}
+
+// the key pairs resolved against the children's schemas and checked (plain column keys of one type each, at most 8 keys and 256 bits
+// of packed key), and the output schema: the left columns, then the right ones unless the join is a semi / anti join
+static void resolve_join_keys(Operator& op, const std::string& what) {
+    if (op.left_keys.size() > MAX_SORT_KEYS) throw Unsupported("more than 8 " + what + " keys");
+    const auto &ls = op.children[0]->schema, &rs = op.children[1]->schema;
+    int bits = 0;
+    for (size_t i = 0; i < op.left_keys.size(); i++) {
+        Expr &l = *op.left_keys[i], &r = *op.right_keys[i];
+        resolve(l, ls);
+        resolve(r, rs);
+        if (l.kind != ExprKind::Bound || r.kind != ExprKind::Bound)
+            throw Unsupported("computed " + what + " keys (only plain column keys: put a Projection below the join)");
+        if (l.type != r.type) throw PlanError(what + " key " + std::to_string(i) + " is " + l.type.str() + " on the left and " + r.type.str() + " on the right");
+        if (l.type.is_float()) throw Unsupported(what + " key of type " + l.type.str() + " (Spark normalises NaN and -0.0 in float keys)");
+        if (l.type.id == TypeId::Binary) throw Unsupported(what + " key of type binary");
+        bits += sort_key_bits(l.type) + 1; // the sort's key encoding: one null bit per key
+    }
+    if (bits > MAX_SORT_KEY_BITS) throw Unsupported(what + " keys of " + std::to_string(bits) + " bits (at most 256 bits of packed key)");
+    const bool semi_anti = op.join_type == JoinType::LeftSemi || op.join_type == JoinType::LeftAnti;
+    op.schema = ls;
+    if (!semi_anti) op.schema.insert(op.schema.end(), rs.begin(), rs.end());
+}
+
 static OperatorP decode_operator(PbReader r) { // Operator operator.proto:32-86
     auto op = std::make_shared<Operator>();
     bool have = false;
@@ -753,22 +805,7 @@ static OperatorP decode_operator(PbReader r) { // Operator operator.proto:32-86
         op->kind = OpKind::Sort;
         while (b.next()) {
             if (b.field == 1 && b.wire == 2) {
-                PbReader e = b.sub();
-                bool have_order = false;
-                SortKey k;
-                while (e.next()) {
-                    if (e.field != 19 || e.wire != 2) { e.skip(); continue; } // SortOrder expr.proto:385-389
-                    have_order = true;
-                    PbReader so = e.sub();
-                    while (so.next()) {
-                        if (so.field == 1) k.expr = decode_expr(so.sub());
-                        else if (so.field == 2) k.descending = so.i64() == 1;
-                        else if (so.field == 3) k.nulls_first = so.i64() == 0;
-                        else so.skip();
-                    }
-                }
-                if (!have_order || !k.expr) throw PlanError("sort key is not a SortOrder with a child");
-                op->sort_keys.push_back(k);
+                op->sort_keys.push_back(decode_sort_order(b.sub()));
             } else if (b.field == 3 || b.field == 4) {
                 const int32_t v = (int32_t)b.i64(); // optional int32
                 if (v < 0) throw PlanError(std::string("sort ") + (b.field == 3 ? "fetch" : "skip") + " is negative");
@@ -789,6 +826,31 @@ static OperatorP decode_operator(PbReader r) { // Operator operator.proto:32-86
         have = true;
         break;
     }
+    case 108: { // SortMergeJoin operator.proto:765-771 (planner.rs:2126-2190: SortMergeJoinExec with NullEqualsNothing)
+        // Run by the hash join's node: the side whose order the output keeps is probed, so RightOuter builds the left side and every
+        // other type the right one.  The sort options must match the keys in number; the operator needs no sorted input, so their
+        // directions do not change the result.
+        op->kind = OpKind::HashJoin;
+        bool condition = false;
+        int64_t join_type = 0;
+        size_t n_sort_options = 0;
+        while (b.next()) {
+            if (b.field == 1 && b.wire == 2) op->left_keys.push_back(decode_expr(b.sub()));
+            else if (b.field == 2 && b.wire == 2) op->right_keys.push_back(decode_expr(b.sub()));
+            else if (b.field == 3) join_type = b.i64();
+            else if (b.field == 4 && b.wire == 2) { decode_sort_order(b.sub()); n_sort_options++; }
+            else if (b.field == 5) { condition = true; b.skip(); }
+            else b.skip();
+        }
+        decode_join(*op, "sort-merge join", join_type);
+        if (n_sort_options != op->left_keys.size())
+            throw PlanError("sort-merge join with " + std::to_string(n_sort_options) + " sort options for " + std::to_string(op->left_keys.size()) + " keys");
+        op->build_left = op->join_type == JoinType::RightOuter;
+        if (condition) throw Unsupported("sort-merge join with a join condition");
+        resolve_join_keys(*op, "sort-merge join");
+        have = true;
+        break;
+    }
     case 109: { // HashJoin operator.proto:754-763 (planner.rs:2192-2266: HashJoinExec with NullEqualsNothing; BuildRight swaps the inputs)
         op->kind = OpKind::HashJoin;
         bool condition = false, null_aware = false;
@@ -802,36 +864,15 @@ static OperatorP decode_operator(PbReader r) { // Operator operator.proto:32-86
             else if (b.field == 6) null_aware = b.i64() != 0;
             else b.skip();
         }
-        if (op->children.size() != 2) throw PlanError("hash join expects two children");
-        if (op->left_keys.empty()) throw PlanError("hash join without keys");
-        if (op->left_keys.size() != op->right_keys.size())
-            throw PlanError("hash join with " + std::to_string(op->left_keys.size()) + " left keys and " + std::to_string(op->right_keys.size()) + " right keys");
-        if (join_type < 0 || join_type > 5) throw PlanError("unknown join type " + std::to_string(join_type));
+        decode_join(*op, "hash join", join_type);
         if (build_side != 0 && build_side != 1) throw PlanError("unknown build side " + std::to_string(build_side));
-        op->join_type = (JoinType)join_type;
         op->build_left = build_side == 0;
         const bool semi_anti = op->join_type == JoinType::LeftSemi || op->join_type == JoinType::LeftAnti;
         if (op->join_type != JoinType::Inner && !semi_anti) throw Unsupported("outer hash joins (only inner, left semi and left anti)");
         if (semi_anti && op->build_left) throw Unsupported("left semi / anti hash join with BuildLeft (only BuildRight)");
         if (condition) throw Unsupported("hash join with a join condition");
         if (null_aware) throw Unsupported("null-aware anti join (NOT IN)");
-        if (op->left_keys.size() > MAX_SORT_KEYS) throw Unsupported("more than 8 hash join keys");
-        const auto &ls = op->children[0]->schema, &rs = op->children[1]->schema;
-        int bits = 0;
-        for (size_t i = 0; i < op->left_keys.size(); i++) {
-            Expr &l = *op->left_keys[i], &r = *op->right_keys[i];
-            resolve(l, ls);
-            resolve(r, rs);
-            if (l.kind != ExprKind::Bound || r.kind != ExprKind::Bound)
-                throw Unsupported("computed hash join keys (only plain column keys: put a Projection below the join)");
-            if (l.type != r.type) throw PlanError("hash join key " + std::to_string(i) + " is " + l.type.str() + " on the left and " + r.type.str() + " on the right");
-            if (l.type.is_float()) throw Unsupported("hash join key of type " + l.type.str() + " (Spark normalises NaN and -0.0 in float keys)");
-            if (l.type.id == TypeId::Binary) throw Unsupported("hash join key of type binary");
-            bits += sort_key_bits(l.type) + 1; // the sort's key encoding: one null bit per key
-        }
-        if (bits > MAX_SORT_KEY_BITS) throw Unsupported("hash join keys of " + std::to_string(bits) + " bits (at most 256 bits of packed key)");
-        op->schema = ls;
-        if (!semi_anti) op->schema.insert(op->schema.end(), rs.begin(), rs.end());
+        resolve_join_keys(*op, "hash join");
         have = true;
         break;
     }

@@ -105,6 +105,7 @@ struct AggExpr {
     int state_at = -1;
 };
 
+// HashJoin: both HashJoin (operator field 109) and SortMergeJoin (108) plans, which one join node runs
 enum class OpKind { Scan, ShuffleScan, NativeScan, Projection, Filter, HashAgg, ShuffleWriter, Sort, HashJoin };
 
 // operator.proto JoinType / BuildSide
@@ -155,8 +156,9 @@ struct Operator {
     // -1 = the field is absent
     std::vector<SortKey> sort_keys;
     int64_t fetch = -1, skip = -1;
-    // HashJoin (operator.proto:754-763): equi-join on Bound key columns of children[0] (left) and children[1] (right).  Inner: the
-    // output is the left columns, then the right ones; LeftSemi / LeftAnti: the left columns.
+    // HashJoin (operator.proto:754-763) and SortMergeJoin (:765-771): equi-join on Bound key columns of children[0] (left) and
+    // children[1] (right).  Inner and the outer types: the output is the left columns, then the right ones; LeftSemi / LeftAnti: the
+    // left columns.  A sort-merge join's build side follows from its type: the left one for RightOuter, else the right one.
     std::vector<ExprP> left_keys, right_keys;
     JoinType join_type = JoinType::Inner;
     bool build_left = false; // BuildLeft: the left child is the build side (the hash table), the right one is probed

@@ -109,6 +109,34 @@ template <typename I> void gather_columns(const Batch& in, const I* row_idx, int
 template void gather_columns<long long>(const Batch&, const long long*, int64_t, Batch&, ExecContext*, const char*);
 template void gather_columns<unsigned>(const Batch&, const unsigned*, int64_t, Batch&, ExecContext*, const char*);
 
+void gather_columns_or_null(const Batch& in, const unsigned* row_idx, int64_t n, Batch& out, ExecContext* ctx) {
+    cudaStream_t st = ctx->stream;
+    out.n_rows = n;
+    out.cols.clear();
+    for (auto& c : in.cols) {
+        Column o = c;
+        const int w = phys_bytes(c.phys);
+        if (w == 0) {
+            auto bytes = std::make_shared<DeviceBuf>((size_t)n + 16);
+            launch_gather_bits_or_null(c.data->ptr, row_idx, n, bytes->ptr, st);
+            o.data = bytes_to_bitmap(bytes, n, ctx);
+            o.bool_bytes = bytes;
+        } else {
+            o.data = std::make_shared<DeviceBuf>((size_t)std::max<int64_t>(n, 1) * w);
+            launch_gather_or_null(c.data->ptr, w, row_idx, n, o.data->ptr, st);
+            if (c.type.id == TypeId::Bool) o.bool_bytes = o.data;
+        }
+        auto bytes = std::make_shared<DeviceBuf>((size_t)n + 16);
+        launch_gather_bits_or_null(c.validity ? c.validity->ptr : nullptr, row_idx, n, bytes->ptr, st);
+        ctx->kernel_launches += 2;
+        o.validity = bytes_to_bitmap(bytes, n, ctx);
+        o.valid_bytes = bytes;
+        o.null_count = -1;
+        out.cols.push_back(o);
+    }
+    cuda_check(cudaGetLastError(), "gathers");
+}
+
 // A non-dictionary column whose batches store it in different layouts -- a Partial aggregate that migrates from dense to hash emits
 // its booleans first as a bitmap (the host flush), then one byte per row (kernel output) -- is brought to the Arrow layout of its type
 // in every batch first, the conversion export makes (to_arrow_layout).  Dictionary columns of different dictionaries are remapped to

@@ -202,7 +202,7 @@ typedef struct cb200_stats {
     int64_t sort_passes;       /* radix passes they ran: one per 8-bit key digit that is not the same in every row */
     int64_t sort_pass_rows;    /* rows those passes moved, summed over the passes */
     int64_t sort_select_rows;  /* rows TopK's radix select read, summed over its digit steps */
-    int64_t join_build_rows;   /* rows HashJoin operators drained from their build side into the hash table's input */
+    int64_t join_build_rows;   /* rows HashJoin and SortMergeJoin operators drained from their build side into the hash table's input */
     int64_t join_probe_rows;   /* probe-side rows they looked up */
     int64_t join_out_rows;     /* rows they emitted */
     int64_t agg_range_levels;  /* OR of CB200_RANGE_* over the dense aggregate launches that were kept: which value-range assumptions ran */
