@@ -67,7 +67,7 @@ class Stats(C.Structure):
                 ("scan_pruned_pages", C.c_int64), ("scan_page_pruned_rows", C.c_int64), ("sort_rows", C.c_int64),
                 ("sort_passes", C.c_int64), ("sort_pass_rows", C.c_int64), ("sort_select_rows", C.c_int64),
                 ("join_build_rows", C.c_int64), ("join_probe_rows", C.c_int64), ("join_out_rows", C.c_int64),
-                ("agg_range_levels", C.c_int64), ("agg_range_reruns", C.c_int64)]
+                ("agg_range_levels", C.c_int64), ("agg_range_reruns", C.c_int64), ("join_cond_pairs", C.c_int64)]
 AGG_DENSE, AGG_TABLE, AGG_STREAM, AGG_MIGRATED = 1, 2, 4, 8  # cb200_stats.agg_strategies bits (CB200_AGG_*)
 RANGE_TIGHT, RANGE_TYPE, RANGE_SAFE = 1, 2, 4  # cb200_stats.agg_range_levels bits (CB200_RANGE_*)
 

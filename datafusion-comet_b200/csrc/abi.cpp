@@ -359,6 +359,7 @@ int cb200_plan_stats(cb200_plan* plan, cb200_stats* out) {
     out->join_out_rows = c.join_out_rows;
     out->agg_range_levels = c.agg_range_levels;
     out->agg_range_reruns = c.agg_range_reruns;
+    out->join_cond_pairs = c.join_cond_pairs;
     return 0;
 }
 

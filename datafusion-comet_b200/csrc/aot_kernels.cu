@@ -795,6 +795,60 @@ __global__ void k_join_unmatched(const u32* run_start, i64 n_runs, const u32* ro
     }
     keep[rows[p]] = !hit[lo];
 }
+// ---- join conditions: from one pass bit per candidate pair to the rows the join type keeps ---------------------------------------------------
+// One thread per pair of a slice whose first pair is a multiple of 32, so each warp owns whole words of the pass bits.  A pair whose build
+// row is CB_NULL_ROW is no candidate (an outer join's slot of a probe row without a match): its bit is cleared, whatever the condition
+// gave on its NULLs.  A passing pair sets its probe row's `passed` byte and, with build_hit, its build row's: plain stores, every writer
+// stores 1.
+__global__ void __launch_bounds__(256) k_join_cond_mark(u32* bits, const u32* probe_idx, const u32* build_idx, i64 k, u8* passed, u8* build_hit,
+                                                        u64* candidates) {
+    const i64 j = (i64)blockIdx.x * blockDim.x + threadIdx.x;
+    if ((j & ~(i64)31) >= k) return; // whole warps only: the ballots below take every lane
+    const bool in = j < k;
+    const u32 b = in ? build_idx[j] : CB_NULL_ROW;
+    const bool cand = b != CB_NULL_ROW;
+    const bool pass = cand && ((bits[j >> 5] >> (j & 31)) & 1u);
+    const u32 word = __ballot_sync(0xffffffffu, pass), n_cand = __popc(__ballot_sync(0xffffffffu, cand));
+    if ((threadIdx.x & 31) == 0) {
+        bits[j >> 5] = word;
+        if (n_cand) atomicAdd((unsigned long long*)candidates, (unsigned long long)n_cand);
+    }
+    if (pass) {
+        passed[probe_idx[j]] = 1;
+        if (build_hit) build_hit[b] = 1;
+    }
+}
+// pairs [o0, o0 + k) of a probe batch after its pass bits are final: keep[j] = the pair passed, or (outer) it is the first pair of a probe
+// row that passed nothing, which becomes that row's NULL-extended row (build_idx[j] = CB_NULL_ROW)
+__global__ void __launch_bounds__(256) k_join_cond_resolve(const u32* bits, i64 o0, const u32* probe_idx, u32* build_idx, i64 k, const u32* offs,
+                                                           const u32* chunk_off, const u8* passed, int outer, u8* keep) {
+    const i64 j = (i64)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= k) return;
+    const i64 p = o0 + j;
+    const bool pass = (bits[p >> 5] >> (p & 31)) & 1u;
+    bool kept = pass;
+    if (!pass && outer) {
+        const u32 i = probe_idx[j];
+        if (!passed[i] && p == (i64)offs[i] + chunk_off[i >> 12]) { kept = true; build_idx[j] = CB_NULL_ROW; }
+    }
+    keep[j] = kept;
+}
+__global__ void k_flags_not(const u8* flags, i64 n, u8* out) {
+    const i64 i = (i64)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) out[i] = !flags[i];
+}
+void launch_join_cond_mark(unsigned* bits, const unsigned* probe_idx, const unsigned* build_idx, i64 k, u8* passed, u8* build_hit,
+                           unsigned long long* candidates, cudaStream_t st) {
+    if (k > 0) k_join_cond_mark<<<(unsigned)((k + 255) / 256), 256, 0, st>>>(bits, probe_idx, build_idx, k, passed, build_hit, (u64*)candidates);
+}
+void launch_join_cond_resolve(const unsigned* bits, i64 o0, const unsigned* probe_idx, unsigned* build_idx, i64 k, const unsigned* offs,
+                              const unsigned* chunk_off, const u8* passed, bool outer, u8* keep, cudaStream_t st) {
+    if (k > 0)
+        k_join_cond_resolve<<<(unsigned)((k + 255) / 256), 256, 0, st>>>(bits, o0, probe_idx, build_idx, k, offs, chunk_off, passed, outer, keep);
+}
+void launch_flags_not(const u8* flags, i64 n, u8* out, cudaStream_t st) {
+    if (n > 0) k_flags_not<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(flags, n, out);
+}
 void launch_join_heads(const u64* keys, int words, i64 m, u8* head, cudaStream_t st) {
     if (m > 0) k_join_heads<<<(unsigned)((m + 255) / 256), 256, 0, st>>>(keys, words, m, head);
 }

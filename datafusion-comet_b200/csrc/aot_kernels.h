@@ -125,6 +125,18 @@ void launch_join_emit(const JoinTable& t, const unsigned* run_of, const unsigned
 // NULL keys included (their runs are not in the table)
 void launch_join_unmatched(const unsigned* run_start, long long n_runs, const unsigned* rows, const unsigned char* hit, long long m,
                            unsigned char* keep, cudaStream_t st);
+// Join conditions.  bits: one pass bit per pair of a probe batch (bit p & 31 of word p >> 5).  mark: the pairs of a slice whose first
+// pair is a multiple of 32 (bits points at its first word): clears the bit of every pair whose build row is CB_NULL_ROW, then for every
+// pair still set stores passed[probe row] = 1 and, if build_hit is given, build_hit[build row] = 1; *candidates += its pairs whose build
+// row is not CB_NULL_ROW.
+void launch_join_cond_mark(unsigned* bits, const unsigned* probe_idx, const unsigned* build_idx, long long k, unsigned char* passed,
+                           unsigned char* build_hit, unsigned long long* candidates, cudaStream_t st);
+// resolve: pairs [o0, o0 + k) once `passed` is final: keep[j] = pair o0 + j passed, or (outer) it is the first pair of a probe row that
+// passed nothing -- offs / chunk_off as in launch_join_emit -- whose build_idx[j] then becomes CB_NULL_ROW
+void launch_join_cond_resolve(const unsigned* bits, long long o0, const unsigned* probe_idx, unsigned* build_idx, long long k, const unsigned* offs,
+                              const unsigned* chunk_off, const unsigned char* passed, bool outer, unsigned char* keep, cudaStream_t st);
+// out[i] = !flags[i], i < n
+void launch_flags_not(const unsigned char* flags, long long n, unsigned char* out, cudaStream_t st);
 
 // device values -> the Arrow layout of their logical type, rows [0, n): what the hand-off (Arrow export, cb200_execute_device) gives out
 enum { CB_SEXT32_TO_128, CB_SEXT64_TO_128, CB_NARROW32_TO_8, CB_NARROW32_TO_16, CB_BITS_TO_BYTES };

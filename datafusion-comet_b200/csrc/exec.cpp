@@ -621,20 +621,7 @@ struct SelectNode : FusedBase {
         return s;
     }
     // pass 1: the predicates alone over the columns they read; same tile / warp geometry as pass 2
-    PipelineSpec make_count_spec(const Batch* b) const {
-        PipelineSpec s;
-        s.cols = stage_cols_of(b, pred_cols);
-        s.predicates = to_slots(predicates, pred_slot_of);
-        s.sink = SinkKind::Count;
-        s.threads = 512;
-        s.ltile = 1024;
-        for (int tile : {4096, 2048, 1024}) { // the widest stage that still leaves a 3-deep ring (wide predicate columns: decimals)
-            s.tile = tile;
-            if (stage_bytes_for(s) * 3 + 1024 <= (int)SMEM_BUDGET) break;
-        }
-        s.stages = stages_for(s);
-        return s;
-    }
+    PipelineSpec make_count_spec(const Batch* b) const { return count_pass_spec(stage_cols_of(b, pred_cols), to_slots(predicates, pred_slot_of)); }
     std::vector<PipelineSpec> build_specs() const override {
         std::vector<PipelineSpec> out{make_spec(nullptr)};
         if (!predicates.empty()) out.push_back(make_count_spec(nullptr));
@@ -721,6 +708,21 @@ struct SelectNode : FusedBase {
         // boolean outputs were written one byte per row; repack lazily at export
     }
 };
+
+PipelineSpec count_pass_spec(std::vector<SourceCol> cols, std::vector<ExprP> predicates) {
+    PipelineSpec s;
+    s.cols = std::move(cols);
+    s.predicates = std::move(predicates);
+    s.sink = SinkKind::Count;
+    s.threads = 512;
+    s.ltile = 1024;
+    for (int tile : {4096, 2048, 1024}) { // the widest stage that still leaves a 3-deep ring (wide predicate columns: decimals)
+        s.tile = tile;
+        if (SelectNode::stage_bytes_for(s) * 3 + 1024 <= (int)SMEM_BUDGET) break;
+    }
+    s.stages = SelectNode::stages_for(s);
+    return s;
+}
 
 // =================================================================================================
 // plan -> executor tree

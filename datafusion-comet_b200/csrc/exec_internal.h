@@ -167,6 +167,11 @@ struct FusedBase : ExecNode {
     }
 };
 
+// The predicate-only pass of a filter (SinkKind::Count) over staged columns `cols`: per (1024-row logical tile, warp) the rows every
+// predicate keeps in PipeParams::sel_off, and with PipeParams::sel_mask one keep bit per row (bit r & 31 of word r >> 5, whole words up
+// to the last row's).  A filter's first pass; a join condition's evaluation over its candidate pairs.
+PipelineSpec count_pass_spec(std::vector<SourceCol> cols, std::vector<ExprP> predicates);
+
 // agg.cpp: the aggregate `agg_op` over `src`, whose columns pass through the fused filters `preds` and projections `cols`.
 // `assume_bits`: build-time value-range assumptions per source column (see cb200_compile_plan_assume); empty at run time.
 ExecNodeP make_agg_node(const OperatorP& agg_op, const ExecNodeP& src, const std::vector<ExprP>& preds, const std::vector<ExprP>& cols, ExecContext* ctx,

@@ -34,6 +34,17 @@ static std::vector<uint32_t> canonical_codes(const Dictionary& d, const Dictiona
 // bit, whatever a batch's validity) and a string field holds a canonical code rather than the dictionary code: the code of the first
 // equal entry of the build side's dictionary, or that dictionary's size (which no build key has) for a probe string it lacks.
 //
+// Join conditions.  A condition is evaluated on candidate pairs only -- (probe row, build row) with equal keys -- and a pair passes when
+// it gives TRUE.  A probe batch with a condition is resolved in two phases, because one probe row's candidates may straddle slices:
+//  1. its pairs are enumerated in slices of at most chunkRows; for each slice the columns the condition reads are gathered through the
+//     pair indices (each in its stored layout), a generated predicate-only pass (count_pass_spec) leaves one pass bit per pair in the
+//     batch's bit array, and launch_join_cond_mark sets the probe row's `passed` byte (and FullOuter's per-build-row hit byte);
+//  2. semi / anti joins compact the probe rows by `passed`; inner and outer joins re-enumerate the pairs slice by slice and keep the
+//     passing ones, plus, for a probe row that passed nothing, its first pair (an outer join's sentinel pair when it has no candidate)
+//     as its NULL-extended row.  FullOuter's unmatched build rows are those whose hit byte no passing pair set.
+// An outer join's sentinel pairs take part in phase 1 with NULLs on both sides and their bits cleared: the condition never sees a
+// NULL-extended row, so an ANSI error comes from a candidate or from nowhere.
+//
 // NULL columns of type t, n rows: the layout (and dictionary) of `like`, or without one the Arrow layout of t and an empty dictionary
 static Column null_column(const DType& t, const Column* like, int64_t n, ExecContext* ctx) {
     Column o;
@@ -50,6 +61,46 @@ static Column null_column(const DType& t, const Column* like, int64_t n, ExecCon
     return o;
 }
 
+// The condition's evaluator: a fused node over the left columns followed by the right ones, whose child produces nothing
+struct JoinCondition : FusedBase {
+    struct Columns : ExecNode { bool next(Batch&) override { return false; } };
+    int n_left = 0;
+    DeviceBufP sel_off;                      // the count pass's per-(tile, warp) counts: written, not read
+
+    bool next(Batch&) override { return false; }
+    PipelineSpec spec(const Batch* b) const { return count_pass_spec(stage_cols(b), to_slots(predicates, slot_of)); }
+
+    // pass bits of the k pairs (probe_idx[j], build_idx[j]) into bits[0, (k + 31) / 32); or_null: a row index may be CB_NULL_ROW
+    void eval(const Batch& probe, const Batch& build, bool build_left, const unsigned* probe_idx, const unsigned* build_idx, int64_t k, bool or_null,
+              cb::u32* bits) {
+        Batch in;
+        in.n_rows = k;
+        in.cols.resize(child->schema.size());
+        for (int c : used_cols) {
+            const bool left = c < n_left, from_probe = left != build_left;
+            const Batch& side = from_probe ? probe : build;
+            const unsigned* idx = from_probe ? probe_idx : build_idx;
+            Batch one, g;
+            one.n_rows = side.n_rows;
+            one.cols = {side.cols.at((size_t)(left ? c : c - n_left))};
+            if (or_null) gather_columns_or_null(one, idx, k, g, ctx);
+            else gather_columns(one, idx, k, g, ctx, "joining");
+            in.cols[(size_t)c] = std::move(g.cols[0]);
+        }
+        const PipelineSpec s = spec(&in);
+        const GeneratedKernel g = generate_pipeline(s);
+        auto mod = jit_get(g, true);
+        cb::PipeParams p;
+        fill_inputs(p, in, g.tile);
+        bind_str_masks(p, s, in);
+        const size_t m = (size_t)((k + 1023) / 1024) * (size_t)(g.threads / 32);
+        if (!sel_off || sel_off->bytes < m * 4) sel_off = std::make_shared<DeviceBuf>(m * 4 + m / 2);
+        p.sel_off = (cb::u32*)sel_off->ptr;
+        p.sel_mask = bits;
+        launch(mod->kernel(g.entry), dim3(std::min(ctx->num_sms, p.n_tiles)), dim3(g.threads + 32), g.dyn_smem(0), &p);
+    }
+};
+
 struct JoinNode : ExecNode {
     ExecContext* ctx;
     ExecNodeP build_child, probe_child;
@@ -63,6 +114,8 @@ struct JoinNode : ExecNode {
     Batch build;                             // the build side's rows, concatenated
     DeviceBufP keys, rows, run_start, slots; // sorted build keys and their rows, run starts (+ the end), the table
     DeviceBufP hit;                          // FullOuter: one byte per run, set when a probe row finds it
+    std::shared_ptr<JoinCondition> cond;     // the join condition, or null
+    DeviceBufP row_hit;                      // FullOuter with a condition: one byte per build row, set when a pair of it passes
     int64_t n_runs = 0;
     JoinTable table{};
     uint32_t h_build_rows = 0;
@@ -71,14 +124,22 @@ struct JoinNode : ExecNode {
     bool probe_done = false;
 
     // what the rows being emitted are: (probe, build) pairs, probe rows (kept_rows), or FullOuter's unmatched build rows (kept_rows)
-    enum class Emit { Pairs, ProbeRows, BuildRows } src = Emit::Pairs;
+    // what the rows being emitted are: (probe, build) pairs, probe rows (kept_rows), FullOuter's unmatched build rows (kept_rows), or
+    // the pairs a condition kept from one slice (kept_probe, kept_build)
+    enum class Emit { Pairs, ProbeRows, BuildRows, KeptPairs } src = Emit::Pairs;
     Batch probe;                             // the probe batch being emitted ...
     DeviceBufP run_of, offs, chunk_off, kept_rows;
     int64_t total = 0, pos = 0;              // ... its output rows, and those emitted
+    // a probe batch with a condition: the pass bit of each pair, the probe rows with a passing pair, the pairs, those resolved (phase 2)
+    DeviceBufP pass_bits, passed, kept_probe, kept_build;
+    int64_t cand_total = 0, cand_pos = 0;
 
     bool outer() const { return type == JoinType::LeftOuter || type == JoinType::RightOuter || type == JoinType::FullOuter; }
     bool semi_anti() const { return type == JoinType::LeftSemi || type == JoinType::LeftAnti; }
     std::vector<ExecNodeP> children() const override { return {build_left ? build_child : probe_child, build_left ? probe_child : build_child}; }
+    std::vector<PipelineSpec> build_specs() const override { return cond ? std::vector<PipelineSpec>{cond->spec(nullptr)} : std::vector<PipelineSpec>{}; }
+    // pairs per condition slice: at most chunkRows, a multiple of 32 so that each slice's pass bits start on a word
+    int64_t cond_slice() const { return std::max<int64_t>(32, ctx->chunk_rows / 32 * 32); }
     // the key layout from the declared key types: the last key is the least significant field, each with a null bit above its value
     void set_layout(const std::vector<DType>& key_types) {
         bits = 0;
@@ -147,7 +208,10 @@ struct JoinNode : ExecNode {
         launch_join_insert(table, n_runs, st);
         cuda_check(cudaGetLastError(), "k_join_insert launch");
         ctx->kernel_launches++;
-        if (type == JoinType::FullOuter) {
+        if (type == JoinType::FullOuter && cond) {
+            row_hit = std::make_shared<DeviceBuf>((size_t)n + 16);
+            cuda_check(cudaMemsetAsync(row_hit->ptr, 0, (size_t)n, st), "memset join row hits");
+        } else if (type == JoinType::FullOuter) {
             hit = std::make_shared<DeviceBuf>((size_t)n_runs);
             cuda_check(cudaMemsetAsync(hit->ptr, 0, (size_t)n_runs, st), "memset join hits");
         }
@@ -172,7 +236,7 @@ struct JoinNode : ExecNode {
         }
         const DeviceBufP pk = pack_row_keys(key_cols(in, probe_keys, false), n, bits, ctx).keys;
         probe = std::move(in);
-        if (!semi_anti()) {
+        if (!semi_anti() || cond) {
             const size_t n_chunks = (size_t)(n + CB_SCAN_CHUNK - 1) / CB_SCAN_CHUNK;
             run_of = std::make_shared<DeviceBuf>((size_t)n * 4);
             offs = std::make_shared<DeviceBuf>((size_t)n * 4);
@@ -188,7 +252,9 @@ struct JoinNode : ExecNode {
             ctx->check_device_errors();
             // the scan's offsets are 32-bit
             if (total >= ((int64_t)1 << 32))
-                throw Unsupported(std::string("a probe batch whose ") + (outer() ? "outer" : "inner") + " join output has 2^32 rows or more (lower spark.comet.b200.chunkRows)");
+                throw Unsupported(std::string("a probe batch whose ") + (cond ? "join condition candidates number" : outer() ? "outer join output has" : "inner join output has") +
+                                  " 2^32 rows or more (lower spark.comet.b200.chunkRows)");
+            if (cond) { evaluate_condition(); return; }
             src = Emit::Pairs;
         } else {
             auto keep = std::make_shared<DeviceBuf>((size_t)n + 16);
@@ -202,13 +268,89 @@ struct JoinNode : ExecNode {
         }
     }
 
+    // phase 1 of a probe batch with a condition (total = its pairs): the pass bits and `passed`; semi / anti joins then compact the probe
+    // rows they keep, inner and outer ones resolve the pairs slice by slice (resolve_slice)
+    void evaluate_condition() {
+        TraceSpan ts("join.condition");
+        cudaStream_t st = ctx->stream;
+        const int64_t n = probe.n_rows, S = cond_slice();
+        pass_bits = std::make_shared<DeviceBuf>((size_t)(total + 31) / 32 * 4 + 8);
+        passed = std::make_shared<DeviceBuf>((size_t)n + 16);
+        auto n_cand = std::make_shared<DeviceBuf>(8);
+        cuda_check(cudaMemsetAsync(passed->ptr, 0, (size_t)n, st), "memset join passed");
+        cuda_check(cudaMemsetAsync(n_cand->ptr, 0, 8, st), "memset join candidates");
+        const size_t cap = (size_t)std::max<int64_t>(std::min(S, total), 1) * 4;
+        auto pidx = std::make_shared<DeviceBuf>(cap), bidx = std::make_shared<DeviceBuf>(cap);
+        for (int64_t s = 0; s < total; s += S) {
+            const int64_t k = std::min(S, total - s);
+            if (outer()) { // the sentinel pairs' slots stay (CB_NULL_ROW, CB_NULL_ROW): all NULLs
+                cuda_check(cudaMemsetAsync(pidx->ptr, 0xff, (size_t)k * 4, st), "memset join pairs");
+                cuda_check(cudaMemsetAsync(bidx->ptr, 0xff, (size_t)k * 4, st), "memset join pairs");
+            }
+            launch_join_emit(table, (const unsigned*)run_of->ptr, (const unsigned*)offs->ptr, (const unsigned*)chunk_off->ptr, n, s, s + k, false,
+                             (unsigned*)pidx->ptr, (unsigned*)bidx->ptr, st);
+            cuda_check(cudaGetLastError(), "k_join_emit launch");
+            cb::u32* bits = (cb::u32*)pass_bits->ptr + s / 32;
+            cond->eval(probe, build, build_left, (const unsigned*)pidx->ptr, (const unsigned*)bidx->ptr, k, outer(), bits);
+            launch_join_cond_mark(bits, (const unsigned*)pidx->ptr, (const unsigned*)bidx->ptr, k, (unsigned char*)passed->ptr,
+                                  row_hit ? (unsigned char*)row_hit->ptr : nullptr, (unsigned long long*)n_cand->ptr, st);
+            cuda_check(cudaGetLastError(), "k_join_cond_mark launch");
+            ctx->kernel_launches += 2;
+        }
+        int64_t* h_cand = (int64_t*)ctx->h_err + 1; // pinned scratch next to the error flag
+        cuda_check(cudaMemcpyAsync(h_cand, n_cand->ptr, 8, cudaMemcpyDeviceToHost, st), "D2H join candidates");
+        ctx->check_device_errors(); // also synchronises: the condition's ANSI errors are raised here
+        ctx->join_cond_pairs += *h_cand;
+        pos = 0;
+        if (semi_anti()) {
+            DeviceBufP keep = passed;
+            if (type == JoinType::LeftAnti) {
+                keep = std::make_shared<DeviceBuf>((size_t)n + 16);
+                launch_flags_not((const unsigned char*)passed->ptr, n, (unsigned char*)keep->ptr, st);
+                ctx->kernel_launches++;
+            }
+            Compacted c = compact_rows(keep, n, n, ctx);
+            kept_rows = c.rows;
+            total = c.n;
+            src = Emit::ProbeRows;
+            pass_bits.reset(); passed.reset(); run_of.reset(); offs.reset(); chunk_off.reset();
+        } else {
+            cand_total = total;
+            cand_pos = 0;
+            total = 0;
+            src = Emit::KeptPairs;
+        }
+    }
+
+    // phase 2, inner and outer joins: the kept pairs of the next slice (possibly none)
+    void resolve_slice() {
+        TraceSpan ts("join.condition.resolve");
+        cudaStream_t st = ctx->stream;
+        const int64_t k = std::min(cond_slice(), cand_total - cand_pos);
+        auto pidx = std::make_shared<DeviceBuf>((size_t)k * 4), bidx = std::make_shared<DeviceBuf>((size_t)k * 4);
+        auto keep = std::make_shared<DeviceBuf>((size_t)k + 16);
+        launch_join_emit(table, (const unsigned*)run_of->ptr, (const unsigned*)offs->ptr, (const unsigned*)chunk_off->ptr, probe.n_rows, cand_pos,
+                         cand_pos + k, outer(), (unsigned*)pidx->ptr, (unsigned*)bidx->ptr, st);
+        launch_join_cond_resolve((const unsigned*)pass_bits->ptr, cand_pos, (const unsigned*)pidx->ptr, (unsigned*)bidx->ptr, k, (const unsigned*)offs->ptr,
+                                 (const unsigned*)chunk_off->ptr, (const unsigned char*)passed->ptr, outer(), (unsigned char*)keep->ptr, st);
+        cuda_check(cudaGetLastError(), "join condition resolve");
+        ctx->kernel_launches += 2;
+        Compacted c = compact_rows(keep, k, k, ctx, {{pidx, 4}, {bidx, 4}});
+        kept_probe = c.extra_out[0];
+        kept_build = c.extra_out[1];
+        total = c.n;
+        pos = 0;
+        cand_pos += k;
+    }
+
     // FullOuter, once the probe side has ended: the build rows no probe row matched, in build input order
     void unmatched_build_rows() {
         TraceSpan ts("join.unmatched");
         const int64_t n = build.n_rows;
         auto keep = std::make_shared<DeviceBuf>((size_t)n + 16);
-        launch_join_unmatched((const unsigned*)run_start->ptr, n_runs, (const unsigned*)rows->ptr, (const unsigned char*)hit->ptr, n,
-                              (unsigned char*)keep->ptr, ctx->stream);
+        if (row_hit) launch_flags_not((const unsigned char*)row_hit->ptr, n, (unsigned char*)keep->ptr, ctx->stream);
+        else launch_join_unmatched((const unsigned*)run_start->ptr, n_runs, (const unsigned*)rows->ptr, (const unsigned char*)hit->ptr, n,
+                                   (unsigned char*)keep->ptr, ctx->stream);
         cuda_check(cudaGetLastError(), "k_join_unmatched launch");
         ctx->kernel_launches++;
         Compacted c = compact_rows(keep, n, n, ctx);
@@ -233,16 +375,26 @@ struct JoinNode : ExecNode {
         const int64_t k = std::min<int64_t>(total - pos, std::max<int64_t>(ctx->chunk_rows, 1));
         const bool null_probe = type == JoinType::FullOuter; // the probe side may be NULL-extended
         Batch pb, bb;
-        if (src == Emit::Pairs) {
-            auto pidx = std::make_shared<DeviceBuf>((size_t)k * 4), bidx = std::make_shared<DeviceBuf>((size_t)k * 4);
-            launch_join_emit(table, (const unsigned*)run_of->ptr, (const unsigned*)offs->ptr, (const unsigned*)chunk_off->ptr, probe.n_rows, pos, pos + k,
-                             outer(), (unsigned*)pidx->ptr, (unsigned*)bidx->ptr, ctx->stream);
-            cuda_check(cudaGetLastError(), "k_join_emit launch");
-            ctx->kernel_launches++;
-            if (null_probe) gather_columns_or_null(probe, (const unsigned*)pidx->ptr, k, pb, ctx);
-            else gather_columns(probe, (const unsigned*)pidx->ptr, k, pb, ctx, "joining");
-            if (outer()) gather_columns_or_null(build, (const unsigned*)bidx->ptr, k, bb, ctx);
-            else gather_columns(build, (const unsigned*)bidx->ptr, k, bb, ctx, "joining");
+        if (src == Emit::Pairs || src == Emit::KeptPairs) {
+            DeviceBufP pidx, bidx;
+            const unsigned *pi, *bi;
+            if (src == Emit::Pairs) {
+                pidx = std::make_shared<DeviceBuf>((size_t)k * 4);
+                bidx = std::make_shared<DeviceBuf>((size_t)k * 4);
+                launch_join_emit(table, (const unsigned*)run_of->ptr, (const unsigned*)offs->ptr, (const unsigned*)chunk_off->ptr, probe.n_rows, pos, pos + k,
+                                 outer(), (unsigned*)pidx->ptr, (unsigned*)bidx->ptr, ctx->stream);
+                cuda_check(cudaGetLastError(), "k_join_emit launch");
+                ctx->kernel_launches++;
+                pi = (const unsigned*)pidx->ptr;
+                bi = (const unsigned*)bidx->ptr;
+            } else {
+                pi = (const unsigned*)kept_probe->ptr + pos;
+                bi = (const unsigned*)kept_build->ptr + pos;
+            }
+            if (null_probe) gather_columns_or_null(probe, pi, k, pb, ctx);
+            else gather_columns(probe, pi, k, pb, ctx, "joining");
+            if (outer()) gather_columns_or_null(build, bi, k, bb, ctx);
+            else gather_columns(build, bi, k, bb, ctx, "joining");
         } else if (src == Emit::ProbeRows) {
             const unsigned* idx = (const unsigned*)kept_rows->ptr + pos;
             if (null_probe) gather_columns_or_null(probe, idx, k, pb, ctx);
@@ -263,7 +415,10 @@ struct JoinNode : ExecNode {
         pos += k;
         ctx->join_out_rows += k;
         ctx->check_device_errors();
-        if (pos >= total) { probe = Batch(); run_of.reset(); offs.reset(); chunk_off.reset(); kept_rows.reset(); }
+        if (pos >= total && cand_pos >= cand_total) {
+            probe = Batch(); run_of.reset(); offs.reset(); chunk_off.reset(); kept_rows.reset();
+            pass_bits.reset(); passed.reset(); kept_probe.reset(); kept_build.reset();
+        }
     }
 
     // Empty sides: an empty build side gives no rows for inner and semi joins, every probe row for anti and outer joins; an empty probe
@@ -274,6 +429,7 @@ struct JoinNode : ExecNode {
         if (empty_build && (type == JoinType::Inner || type == JoinType::LeftSemi)) return false; // nothing matches
         for (;;) {
             if (pos < total) { emit(out); return true; }
+            if (cand_pos < cand_total) { resolve_slice(); continue; }
             if (probe_done) return false;
             Batch in;
             if (!probe_child->next(in)) {
@@ -319,6 +475,22 @@ ExecNodeP make_join_node(const OperatorP& op, const ExecNodeP& left, const ExecN
     n->build_keys = op->build_left ? lk : rk;
     n->probe_keys = op->build_left ? rk : lk;
     n->set_layout(key_types);
+    if (op->join_condition) {
+        auto c = std::make_shared<JoinCondition>();
+        auto cols = std::make_shared<JoinCondition::Columns>();
+        cols->schema = left->schema;
+        cols->schema.insert(cols->schema.end(), right->schema.begin(), right->schema.end());
+        c->ctx = ctx;
+        c->child = cols;
+        c->n_left = (int)left->schema.size();
+        c->predicates = {op->join_condition};
+        c->assign_slots(c->predicates);
+        if (c->used_cols.empty()) { // a condition of literals alone: the pass still needs a staged column, the first left key
+            c->used_cols.push_back(lk[0]);
+            c->slot_of[lk[0]] = 0;
+        }
+        n->cond = c;
+    }
     return n;
 }
 

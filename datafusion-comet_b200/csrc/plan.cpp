@@ -625,6 +625,31 @@ static void resolve_join_keys(Operator& op, const std::string& what) {
     if (!semi_anti) op.schema.insert(op.schema.end(), rs.begin(), rs.end());
 }
 
+// the join condition resolved against the left columns followed by the right ones (operators.scala:2634-2640), for every join type.
+// What the expression layer refuses stays refused, its message naming the condition.
+static void resolve_join_condition(Operator& op) {
+    if (!op.join_condition) return;
+    std::vector<DType> both = op.children[0]->schema;
+    both.insert(both.end(), op.children[1]->schema.begin(), op.children[1]->schema.end());
+    try {
+        resolve(*op.join_condition, both);
+    } catch (const Unsupported& e) {
+        throw Unsupported(std::string("join condition: ") + e.what());
+    } catch (const PlanError& e) {
+        throw PlanError(std::string("join condition: ") + e.what());
+    }
+    if (op.join_condition->type.id != TypeId::Bool) throw PlanError("join condition is " + op.join_condition->type.str() + ", not boolean");
+}
+
+// a join condition's expression (Unsupported -> a refusal naming the condition)
+static ExprP decode_join_condition(PbReader r) {
+    try {
+        return decode_expr(r);
+    } catch (const Unsupported& e) {
+        throw Unsupported(std::string("join condition: ") + e.what());
+    }
+}
+
 static OperatorP decode_operator(PbReader r) { // Operator operator.proto:32-86
     auto op = std::make_shared<Operator>();
     bool have = false;
@@ -831,7 +856,6 @@ static OperatorP decode_operator(PbReader r) { // Operator operator.proto:32-86
         // other type the right one.  The sort options must match the keys in number; the operator needs no sorted input, so their
         // directions do not change the result.
         op->kind = OpKind::HashJoin;
-        bool condition = false;
         int64_t join_type = 0;
         size_t n_sort_options = 0;
         while (b.next()) {
@@ -839,27 +863,27 @@ static OperatorP decode_operator(PbReader r) { // Operator operator.proto:32-86
             else if (b.field == 2 && b.wire == 2) op->right_keys.push_back(decode_expr(b.sub()));
             else if (b.field == 3) join_type = b.i64();
             else if (b.field == 4 && b.wire == 2) { decode_sort_order(b.sub()); n_sort_options++; }
-            else if (b.field == 5) { condition = true; b.skip(); }
+            else if (b.field == 5 && b.wire == 2) op->join_condition = decode_join_condition(b.sub());
             else b.skip();
         }
         decode_join(*op, "sort-merge join", join_type);
         if (n_sort_options != op->left_keys.size())
             throw PlanError("sort-merge join with " + std::to_string(n_sort_options) + " sort options for " + std::to_string(op->left_keys.size()) + " keys");
         op->build_left = op->join_type == JoinType::RightOuter;
-        if (condition) throw Unsupported("sort-merge join with a join condition");
         resolve_join_keys(*op, "sort-merge join");
+        resolve_join_condition(*op);
         have = true;
         break;
     }
     case 109: { // HashJoin operator.proto:754-763 (planner.rs:2192-2266: HashJoinExec with NullEqualsNothing; BuildRight swaps the inputs)
         op->kind = OpKind::HashJoin;
-        bool condition = false, null_aware = false;
+        bool null_aware = false;
         int64_t join_type = 0, build_side = 0;
         while (b.next()) {
             if (b.field == 1 && b.wire == 2) op->left_keys.push_back(decode_expr(b.sub()));
             else if (b.field == 2 && b.wire == 2) op->right_keys.push_back(decode_expr(b.sub()));
             else if (b.field == 3) join_type = b.i64();
-            else if (b.field == 4) { condition = true; b.skip(); }
+            else if (b.field == 4 && b.wire == 2) op->join_condition = decode_join_condition(b.sub());
             else if (b.field == 5) build_side = b.i64();
             else if (b.field == 6) null_aware = b.i64() != 0;
             else b.skip();
@@ -870,9 +894,9 @@ static OperatorP decode_operator(PbReader r) { // Operator operator.proto:32-86
         const bool semi_anti = op->join_type == JoinType::LeftSemi || op->join_type == JoinType::LeftAnti;
         if (op->join_type != JoinType::Inner && !semi_anti) throw Unsupported("outer hash joins (only inner, left semi and left anti)");
         if (semi_anti && op->build_left) throw Unsupported("left semi / anti hash join with BuildLeft (only BuildRight)");
-        if (condition) throw Unsupported("hash join with a join condition");
         if (null_aware) throw Unsupported("null-aware anti join (NOT IN)");
         resolve_join_keys(*op, "hash join");
+        resolve_join_condition(*op);
         have = true;
         break;
     }

@@ -162,6 +162,9 @@ struct Operator {
     std::vector<ExprP> left_keys, right_keys;
     JoinType join_type = JoinType::Inner;
     bool build_left = false; // BuildLeft: the left child is the build side (the hash table), the right one is probed
+    // the join condition (JoinFilter, planner.rs:2462-2542), or null: a boolean over the left columns followed by the right ones
+    // (Bound.index = left column, or left column count + right column), whatever the build side and join type
+    ExprP join_condition;
 };
 
 // Sort keys at most: 8 keys, 256 bits of packed key (value bits by declared type plus one null bit per key, sort_key_bits)

@@ -207,6 +207,7 @@ typedef struct cb200_stats {
     int64_t join_out_rows;     /* rows they emitted */
     int64_t agg_range_levels;  /* OR of CB200_RANGE_* over the dense aggregate launches that were kept: which value-range assumptions ran */
     int64_t agg_range_reruns;  /* dense aggregate launches discarded because their input broke the value range the kernel assumed */
+    int64_t join_cond_pairs;   /* candidate pairs (equal keys) of HashJoin and SortMergeJoin operators their join condition was evaluated on */
 } cb200_stats;
 #define CB200_AGG_DENSE 1      /* thread-private accumulators over dictionary / bool key codes (and ungrouped aggregates) */
 #define CB200_AGG_TABLE 2      /* global key table */
