@@ -379,6 +379,7 @@ struct AggNode : FusedBase {
 
     // keys
     std::vector<bool> key_has_null;               // per key: some batch so far had a validity buffer
+    std::vector<bool> col_nullable;               // per child column: some batch so far had a validity buffer (SourceCol::layout_nullable)
     std::vector<DictionaryP> key_dicts;           // strings per key (dict columns); empty for bool keys
     // device string dictionaries for plain Utf8 keys
     struct DevDict { StringDictDev d; std::vector<DeviceBufP> bufs; int host_known = 0; };
@@ -386,7 +387,7 @@ struct AggNode : FusedBase {
 
     // accumulator layout of the kernels launched so far, and the last of them (finalize runs from its module)
     int n_words = 0, key_words = 1;   // key_words: 64-bit words per packed group key (hkey_of_gid stride)
-    std::vector<int> word_kinds;
+    std::vector<int> word_kinds, role_words;
     Kernel last;                      // the last kernel whose launch was kept: the node holds state once there is one
     bool have_totals() const { return last.mod != nullptr; }
 
@@ -416,7 +417,10 @@ struct AggNode : FusedBase {
         const bool hash = st == Strategy::Table || st == Strategy::Stream;
         PipelineSpec s;
         s.cols = stage_cols(b);
-        for (auto& c : s.cols) c.assume_bits = assume_for(c.src_index, lv);
+        for (auto& c : s.cols) {
+            c.assume_bits = assume_for(c.src_index, lv);
+            c.layout_nullable = b && col_nullable[(size_t)c.src_index];
+        }
         s.predicates = to_slots(predicates, slot_of);
         s.sink = SinkKind::Agg;
         s.mode = mode;
@@ -468,16 +472,38 @@ struct AggNode : FusedBase {
         return out;
     }
 
-    // generate and load the kernel of `spec` and adopt its accumulator layout, which must not change once state exists
+    // generate and load the kernel of `spec` and adopt its accumulator layout; state that exists moves to it when it is wider
     Kernel compile(const PipelineSpec& spec) {
         Kernel k{spec, generate_pipeline(spec), nullptr};
         k.mod = jit_get(k.g, true);
-        if (have_totals() && (k.g.n_words != n_words || k.g.word_kinds != word_kinds)) throw ExecError(15, "", "internal: accumulator layout changed between launches");
         if (have_totals() && k.g.key_words != key_words) throw ExecError(15, "", "internal: group key packing changed between launches");
+        if (have_totals() && (k.g.n_words != n_words || k.g.word_kinds != word_kinds || k.g.role_words != role_words)) widen(k);
         n_words = k.g.n_words;
         word_kinds = k.g.word_kinds;
+        role_words = k.g.role_words;
         key_words = k.g.key_words;
         return k;
+    }
+
+    // A batch gave validity to an input whose row count the layout shared so far (COUNT(x) beside COUNT(*), say): move the totals to
+    // the wider layout of `k`.  Each word starts as the word it was split from (widen_word_map).  Totals are group-major -- dense:
+    // one row per group, id rows: max_groups + 2 rows -- so the move is one strided copy per word.
+    void widen(const Kernel& k) {
+        GeneratedKernel from;
+        from.n_words = n_words;
+        from.word_kinds = word_kinds;
+        from.role_words = role_words;
+        const std::vector<int> map = widen_word_map(from, k.g);
+        if (map.empty()) throw ExecError(15, "", "internal: accumulator layout changed between launches");
+        const bool is_dense = strategy == Strategy::Dense;
+        DeviceBufP& t = is_dense ? dense.totals : rows.htotals;
+        const size_t n_rows = is_dense ? (size_t)dense.groups : (size_t)rows.max_groups + 2;
+        auto nt = std::make_shared<DeviceBuf>(n_rows * (size_t)k.g.n_words * 16);
+        for (int w = 0; w < k.g.n_words; w++)
+            cuda_check(cudaMemcpy2DAsync((char*)nt->ptr + (size_t)w * 16, (size_t)k.g.n_words * 16, (const char*)t->ptr + (size_t)map[(size_t)w] * 16,
+                                         (size_t)n_words * 16, 16, n_rows, cudaMemcpyDeviceToDevice, ctx->stream), "widen totals");
+        cuda_check(cudaStreamSynchronize(ctx->stream), "widen totals"); // the old buffer dies below
+        t = nt;
     }
 
     // ---- value masks: per staged column, the OR of (v ^ sign) over the valid rows of one launch --------------------------------------
@@ -568,6 +594,7 @@ struct AggNode : FusedBase {
     }
 
     void consume(Batch& b) {
+        for (int ci : used_cols) if (b.cols[(size_t)ci].validity) col_nullable[(size_t)ci] = true;
         std::vector<int> nc(keys.size());
         std::vector<bool> hn(keys.size());
         for (size_t k = 0; k < keys.size(); k++) {
@@ -649,7 +676,7 @@ struct AggNode : FusedBase {
         }
         last = Kernel();
         dense = DenseState();
-        n_words = 0; word_kinds.clear(); rows_scanned = 0;
+        n_words = 0; word_kinds.clear(); role_words.clear(); rows_scanned = 0;
     }
 
     // one (possibly split) launch over rows [row0,row1) at assumption level lv, escalating on violated assumptions
@@ -808,7 +835,7 @@ struct AggNode : FusedBase {
         IdRows::init_totals(ctx, k, (cb::u64*)rows.htotals->ptr, rows.max_groups, 2);
         if (stream.ratio <= ctx->stream_agg_max_ratio) return true;
         rows = IdRows();
-        n_words = 0; word_kinds.clear();
+        n_words = 0; word_kinds.clear(); role_words.clear();
         return false;
     }
     void consume_stream(Batch& b) {
@@ -880,6 +907,7 @@ struct AggNode : FusedBase {
     void aggregate_input() {
         if (keys.size() > CB_MAX_KEYS) throw Unsupported("more than 4 group keys");
         key_has_null.assign(keys.size(), false);
+        col_nullable.assign(child->schema.size(), false);
         key_dicts.assign(keys.size(), nullptr);
         dev_dicts.assign(keys.size(), nullptr);
         Batch in;

@@ -7,9 +7,11 @@
 #include "device/cb_params.h"
 #include "ranges.h"
 
+#include <algorithm>
 #include <climits>
 #include <cstring>
 #include <functional>
+#include <memory>
 #include <set>
 #include <sstream>
 
@@ -766,7 +768,7 @@ void sig_expr(std::ostringstream& o, const Expr& e) {
 std::string spec_signature(const PipelineSpec& s) {
     std::ostringstream o;
     o << (int)s.sink << ';' << (int)s.mode << ';' << s.ungrouped << ';' << s.hash << (s.stream ? "s" : "") << (s.masked ? "m" : "") << ';' << s.tile << ';' << s.stages << ';' << s.threads << ';' << s.ltile << ";C";
-    for (auto& c : s.cols) o << c.src_index << ':' << c.type.str() << ':' << (int)c.phys << ':' << c.has_validity << ':' << c.assume_bits << ',';
+    for (auto& c : s.cols) o << c.src_index << ':' << c.type.str() << ':' << (int)c.phys << ':' << c.has_validity << ':' << c.assume_bits << (c.layout_nullable && !c.has_validity ? "L" : "") << ',';
     o << ";P";
     for (auto& e : s.predicates) { sig_expr(o, *e); o << ';'; }
     o << ";O";
@@ -791,6 +793,26 @@ GeneratedKernel generate_pipeline_uncached(const PipelineSpec& spec);
 } // namespace
 
 std::string pipeline_signature(const PipelineSpec& spec) { return spec_signature(spec); }
+
+std::vector<int> widen_word_map(const GeneratedKernel& from, const GeneratedKernel& to) {
+    if (from.role_words.size() != to.role_words.size()) return {};
+    std::vector<int> map((size_t)to.n_words, -1);
+    auto set = [&](int w, int o) {
+        if (map[(size_t)w] >= 0 && map[(size_t)w] != o) return false; // two words of `from` would merge into one
+        map[(size_t)w] = o;
+        return true;
+    };
+    for (size_t r = 0; r < to.role_words.size(); r++) {
+        const int w = to.role_words[r], o = from.role_words[r];
+        if ((w < 0) != (o < 0)) return {};
+        if (w < 0) continue;
+        if (!set(w, o)) return {};
+        if (to.word_kinds[(size_t)w] == W_DD_HI && !set(w + 1, o + 1)) return {};
+    }
+    for (int w = 0; w < to.n_words; w++)
+        if (map[(size_t)w] < 0 || from.word_kinds.at((size_t)map[(size_t)w]) != to.word_kinds[(size_t)w]) return {};
+    return map;
+}
 
 std::string str_pred_key(const Expr& e) {
     std::ostringstream o;
@@ -1048,22 +1070,40 @@ GeneratedKernel generate_pipeline_uncached(const PipelineSpec& spec) {
         if (!spec.hash) em.body << "    const int g = " << gid << ";\n";
         int w_rows = slots.add(W_WRAP64, "cnt|true"); // rows passing the filter == COUNT(*) == non-null count of never-null inputs
         upd("count", "true", w_rows);
+        // Which inputs share a word is decided by the null tests of every column that ever carried validity (layout_nullable), not
+        // by this batch's alone, so a later batch without validity keeps the layout.  `km` emits the aggregate inputs as if those
+        // columns had validity; only the strings it returns -- the slot dedup keys -- are used.  A spec where the two agree keys
+        // the slots by `em`'s own strings.
+        PipelineSpec lspec;
+        std::unique_ptr<Emitter> km;
+        if (std::any_of(spec.cols.begin(), spec.cols.end(), [](const SourceCol& c) { return c.layout_nullable && !c.has_validity; })) {
+            lspec = spec;
+            for (auto& c : lspec.cols) c.has_validity = c.has_validity || c.layout_nullable;
+            km.reset(new Emitter(lspec));
+            km->base_guard = em.base_guard;
+        }
+        // the FILTER clause, then the children: `cond` = the row passes the filter and every child is non-NULL
+        auto input_cond = [](Emitter& e, const AggExpr& a, std::vector<Val>& cv) {
+            std::string cond = "true";
+            if (a.filter) {
+                Val f = e.emit(*a.filter);
+                cond = f.n.empty() ? f.v : "(!" + f.n + " && " + f.v + ")";
+            }
+            for (auto& c : a.children) cv.push_back(e.emit(*c));
+            for (auto& v : cv) if (v.nullable()) cond += " && !" + v.n;
+            return cond;
+        };
 
         for (size_t ai = 0; ai < spec.aggs.size(); ai++) {
             const AggExpr& a = spec.aggs[ai];
             AggLayout& L = layout[ai];
             if (a.mode == AggMode::Partial) {
                 // per-aggregate FILTER clause: NULL/FALSE excludes the row (sum_decimal.rs:452-458)
-                std::string cond = "true";
-                if (a.filter) {
-                    Val f = em.emit(*a.filter);
-                    cond = f.n.empty() ? f.v : "(!" + f.n + " && " + f.v + ")";
-                }
-                std::vector<Val> cv;
-                for (auto& c : a.children) cv.push_back(em.emit(*c));
-                for (auto& v : cv) if (v.nullable()) cond += " && !" + v.n;
-                std::string condkey = cond;
+                std::vector<Val> cv, kcv;
+                const std::string cond = input_cond(em, a, cv);
+                const std::string condkey = km ? input_cond(*km, a, kcv) : cond;
                 const Val& v = cv[0];
+                const std::string vkey = km ? kcv[0].v : v.v; // the value's name in the slot keys
                 std::string use = cond == "true" ? "true" : em.declb(cond);
                 // non-null (and filter-passing) row count of this input: COUNT, AVG count, !is_empty
                 auto cnt_slot = [&]() {
@@ -1082,8 +1122,8 @@ GeneratedKernel generate_pipeline_uncached(const PipelineSpec& spec) {
                     bool f64 = !dec && (a.kind == AggKind::Avg || a.datatype.is_float());
                     L.w_cnt = cnt_slot();
                     if (dec) {
-                        bool first = slots.dedup.count(std::to_string((int)W_SUM128) + "|sum|" + v.v + "|" + condkey) == 0;
-                        L.w_sum = slots.add(W_SUM128, "sum|" + v.v + "|" + condkey);
+                        bool first = slots.dedup.count(std::to_string((int)W_SUM128) + "|sum|" + vkey + "|" + condkey) == 0;
+                        L.w_sum = slots.add(W_SUM128, "sum|" + vkey + "|" + condkey);
                         if (first) {
                             // per-thread 64-bit partials are exact while rows/thread * |v| < 2^63 (host caps rows/thread at 2^CB_RPT_LOG2)
                             u128r vb = em.bound_of(*a.children[0]);
@@ -1095,8 +1135,8 @@ GeneratedKernel generate_pipeline_uncached(const PipelineSpec& spec) {
                     } else if (f64) {
                         L.is_f64_sum = true;
                         std::string dv = v.type.id == TypeId::Float64 ? v.v : "(double)" + v.v;
-                        bool first = slots.dedup.count(std::to_string((int)W_DD_HI) + "|dd|" + dv + "|" + condkey) == 0;
-                        L.w_sum = slots.add(W_DD_HI, "dd|" + dv + "|" + condkey, 2);
+                        bool first = slots.dedup.count(std::to_string((int)W_DD_HI) + "|dd|" + vkey + "|" + condkey) == 0;
+                        L.w_sum = slots.add(W_DD_HI, "dd|" + vkey + "|" + condkey, 2);
                         if (first) upd("f64", use, L.w_sum, dv);
                     } else if (a.eval_mode != EvalMode::Legacy) {
                         // SumInt ANSI / TRY (sum_int.rs:176-390): the reference adds row by row with add_checked, so whether it
@@ -1104,13 +1144,13 @@ GeneratedKernel generate_pipeline_uncached(const PipelineSpec& spec) {
                         // EVERY order: sum|v| <= i64::MAX => no prefix of any order can overflow; total out of range => every
                         // order overflows (the last prefix is the total); anything else is order-dependent (finalize raises it).
                         std::string iv = "(cb::i64)" + v.v;
-                        bool first = slots.dedup.count(std::to_string((int)W_SUM128) + "|csum|" + v.v + "|" + condkey) == 0;
-                        L.w_sum = slots.add(W_SUM128, "csum|" + v.v + "|" + condkey);
-                        L.w_abs = slots.add(W_SUM128, "cabs|" + v.v + "|" + condkey);
+                        bool first = slots.dedup.count(std::to_string((int)W_SUM128) + "|csum|" + vkey + "|" + condkey) == 0;
+                        L.w_sum = slots.add(W_SUM128, "csum|" + vkey + "|" + condkey);
+                        L.w_abs = slots.add(W_SUM128, "cabs|" + vkey + "|" + condkey);
                         if (first) { upd("wide", use, L.w_sum, iv); upd("i128", use, L.w_abs, absval(iv)); }
                     } else { // SumInt Legacy: wrapping i64 (sum_int.rs:432)
-                        bool first = slots.dedup.count(std::to_string((int)W_WRAP64) + "|isum|" + v.v + "|" + condkey) == 0;
-                        L.w_sum = slots.add(W_WRAP64, "isum|" + v.v + "|" + condkey);
+                        bool first = slots.dedup.count(std::to_string((int)W_WRAP64) + "|isum|" + vkey + "|" + condkey) == 0;
+                        L.w_sum = slots.add(W_WRAP64, "isum|" + vkey + "|" + condkey);
                         if (first) upd("wrap", use, L.w_sum, "(cb::i64)" + v.v);
                     }
                     break;
@@ -1123,7 +1163,7 @@ GeneratedKernel generate_pipeline_uncached(const PipelineSpec& spec) {
                     // the words hold 64-bit keys: a decimal(p <= 18) value outside them (invalid input) is refused, never compared by its low word
                     if (v.type.is_decimal() && !v.narrow) em.raise(use + " && !cb::i128_fits_i64(" + v.v + ")", 6);
                     bool mn = a.kind == AggKind::Min;
-                    std::string sk = std::string(mn ? "min|" : "max|") + v.v + "|" + condkey;
+                    std::string sk = std::string(mn ? "min|" : "max|") + vkey + "|" + condkey;
                     bool first = slots.dedup.count(std::to_string((int)(mn ? W_MIN : W_MAX)) + "|" + sk) == 0;
                     L.w_minmax = slots.add(mn ? W_MIN : W_MAX, sk);
                     if (first) upd(mn ? "min" : "max", use, L.w_minmax, key);
@@ -1227,6 +1267,9 @@ GeneratedKernel generate_pipeline_uncached(const PipelineSpec& spec) {
         }
         g.n_words = (int)slots.kinds.size();
         g.word_kinds = slots.kinds;
+        g.role_words.push_back(w_rows);
+        for (const AggLayout& L : layout)
+            for (int w : {L.w_sum, L.w_cnt, L.w_bits, L.w_bad, L.w_minmax, L.w_abs}) g.role_words.push_back(w);
 
         // ---------------- finalize program: totals -> state columns (Partial) / results (Final) -------
         std::ostringstream fin;

@@ -20,6 +20,9 @@ struct SourceCol {
     Phys phys;
     bool has_validity;
     int assume_bits = 0; // decimal columns: kernel may assume |v| < 2^assume_bits (validated by the value masks); 0 = no assumption
+    // aggregate sinks: an earlier batch of the same aggregate carried validity for this column.  The accumulator layout keeps the
+    // column's null tests apart (as if has_validity) so that it never narrows again; the null tests emitted are this batch's own.
+    bool layout_nullable = false;
 };
 
 // thread-private 64-bit partial sums are exact while rows/thread <= 2^CB_RPT_LOG2 (host enforces it per launch)
@@ -64,6 +67,9 @@ struct GeneratedKernel {
     int stage_bytes = 0;
     int n_words = 0;           // agg: accumulator words per group
     std::vector<int> word_kinds;
+    // agg: the word of each accumulator role: [0] the row count (CB_W_ROWS), then per aggregate its sum, count, bits, bad, min / max
+    // and abs words (-1: unused).  Two layouts of one aggregate correspond role by role (see widen_word_map).
+    std::vector<int> role_words;
     std::vector<OutCol> out_cols;     // select: outputs; agg: finalize outputs (excluding key columns)
     std::vector<int> out_bytes;       // element bytes of each output column (1 for bool-as-byte)
     int threads = 256, tile = 512, stages = 3;
@@ -75,6 +81,11 @@ struct GeneratedKernel {
 };
 
 GeneratedKernel generate_pipeline(const PipelineSpec& spec);
+
+// For each accumulator word of layout `to`, the word of layout `from` it starts as: both are layouts of one aggregate, `to` with at
+// least the nullable inputs of `from`.  Words that shared a row count in `from` and are apart in `to` both start from it, which is
+// exact: every row seen so far counted toward each.  Empty when `to` does not refine `from` role by role.
+std::vector<int> widen_word_map(const GeneratedKernel& from, const GeneratedKernel& to);
 
 // The distinct string predicates (ExprKind::StrPred) of a pipeline in mask-slot order: PipeParams::smask[i] holds the mask of entry i.
 // Order: predicates, outputs, group keys, then the arguments and FILTER clauses of Partial-mode aggregates, each depth first.  Throws
