@@ -67,7 +67,7 @@ EXPR_FIELD = dict(literal=2, bound=3, add=4, subtract=5, multiply=6, divide=7, c
                   scalarFunc=31, caseWhen=38, **{"in": 39, "not": 40}, unary_minus=41, **{"if": 44}, unbound=51)  # expr.proto:30-109
 AGG_FIELD = dict(count=2, sum=3, min=4, max=5, avg=6)  # expr.proto:143-176
 OP_FIELD = dict(scan=100, projection=101, filter=102, sort=103, hash_agg=104, limit=105, shuffle_writer=106, sort_merge_join=108, hash_join=109,
-                native_scan=111, shuffle_scan=116)  # operator.proto:32-86
+                native_scan=111, shuffle_scan=116, broadcast_nested_loop_join=117)  # operator.proto:32-86
 LITERAL_FIELD = dict(bool_val=1, byte_val=2, short_val=3, int_val=4, long_val=5, float_val=6, double_val=7,
                      string_val=8, bytes_val=9, decimal_val=10, datatype=12, is_null=13)  # literal.proto:26-47
 LEGACY, TRY, ANSI = 0, 1, 2  # expr.proto:324 EvalMode
@@ -351,6 +351,14 @@ def sort_merge_join(left, right, left_keys, right_keys, join_type, sort_options,
     if condition is not None:
         body += f_len(5, condition)
     return _op("sort_merge_join", body, (left, right), plan_id)
+
+
+def broadcast_nested_loop_join(left, right, join_type, build_side, condition=None, plan_id=0):
+    """BroadcastNestedLoopJoin operator.proto:773-777: children (left, right), no keys; the condition is field 3."""
+    body = f_varint(1, join_type) + f_varint(2, build_side)
+    if condition is not None:
+        body += f_len(3, condition)
+    return _op("broadcast_nested_loop_join", body, (left, right), plan_id)
 
 
 def struct_field(name, dt, nullable=True):  # SparkStructField operator.proto:97

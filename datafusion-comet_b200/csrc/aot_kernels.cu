@@ -833,6 +833,48 @@ __global__ void __launch_bounds__(256) k_join_cond_resolve(const u32* bits, i64 
     }
     keep[j] = kept;
 }
+// ---- nested-loop join: pair position p of a group is (probe row row0 + p / m, build row p % m) -------------------------------------------
+// p / m without a 64-bit divide: inv = floor((2^64 - 1) / m) gives inv * m in (2^64 - 1 - m, 2^64), so mulhi(p, inv) is p / m or one less;
+// one compare of the remainder corrects it.  Exact for every p < 2^64 and 0 < m < 2^32.
+__device__ __forceinline__ u32 nlj_divmod(u64 p, u32 m, u64 inv, u32& r) {
+    u64 q = __umul64hi(p, inv);
+    u64 rem = p - q * m;
+    if (rem >= m) { q++; rem -= m; }
+    r = (u32)rem;
+    return (u32)q;
+}
+__global__ void __launch_bounds__(256) k_nlj_pairs(i64 p0, i64 k, u32 row0, u32 m, u64 inv, u32* probe_idx, u32* build_idx) {
+    const i64 j = (i64)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= k) return;
+    u32 r;
+    const u32 q = nlj_divmod((u64)(p0 + j), m, inv, r);
+    probe_idx[j] = row0 + q;
+    build_idx[j] = r;
+}
+// k_join_cond_resolve's arithmetic sibling, which also writes the pairs: keep[j] = pair p0 + j passed, or (outer) it is the first pair
+// (build row 0) of a probe row that passed nothing, whose build row then becomes CB_NULL_ROW
+__global__ void __launch_bounds__(256) k_nlj_cond_resolve(const u32* bits, i64 p0, i64 k, u32 row0, u32 m, u64 inv, const u8* passed, int outer,
+                                                          u32* probe_idx, u32* build_idx, u8* keep) {
+    const i64 j = (i64)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= k) return;
+    const i64 p = p0 + j;
+    u32 r;
+    const u32 i = row0 + nlj_divmod((u64)p, m, inv, r);
+    const bool pass = (bits[p >> 5] >> (p & 31)) & 1u;
+    bool kept = pass;
+    if (!pass && outer && r == 0 && !passed[i]) { kept = true; r = CB_NULL_ROW; }
+    probe_idx[j] = i;
+    build_idx[j] = r;
+    keep[j] = kept;
+}
+void launch_nlj_pairs(i64 p0, i64 k, unsigned row0, unsigned m, unsigned long long inv, unsigned* probe_idx, unsigned* build_idx, cudaStream_t st) {
+    if (k > 0) k_nlj_pairs<<<(unsigned)((k + 255) / 256), 256, 0, st>>>(p0, k, row0, m, (u64)inv, probe_idx, build_idx);
+}
+void launch_nlj_cond_resolve(const unsigned* bits, i64 p0, i64 k, unsigned row0, unsigned m, unsigned long long inv, const u8* passed, bool outer,
+                             unsigned* probe_idx, unsigned* build_idx, u8* keep, cudaStream_t st) {
+    if (k > 0)
+        k_nlj_cond_resolve<<<(unsigned)((k + 255) / 256), 256, 0, st>>>(bits, p0, k, row0, m, (u64)inv, passed, outer, probe_idx, build_idx, keep);
+}
 __global__ void k_flags_not(const u8* flags, i64 n, u8* out) {
     const i64 i = (i64)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) out[i] = !flags[i];

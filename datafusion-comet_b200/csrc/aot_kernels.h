@@ -135,6 +135,16 @@ void launch_join_cond_mark(unsigned* bits, const unsigned* probe_idx, const unsi
 // passed nothing -- offs / chunk_off as in launch_join_emit -- whose build_idx[j] then becomes CB_NULL_ROW
 void launch_join_cond_resolve(const unsigned* bits, long long o0, const unsigned* probe_idx, unsigned* build_idx, long long k, const unsigned* offs,
                               const unsigned* chunk_off, const unsigned char* passed, bool outer, unsigned char* keep, cudaStream_t st);
+// Nested-loop join.  The pairs of a group of probe rows from row0 against m build rows (0 < m < 2^32) are numbered probe-row major:
+// position p is (row0 + p / m, p % m).  inv = floor((2^64 - 1) / m) replaces the divide.  pairs: probe_idx[j], build_idx[j] = pair p0 + j,
+// j < k.
+void launch_nlj_pairs(long long p0, long long k, unsigned row0, unsigned m, unsigned long long inv, unsigned* probe_idx, unsigned* build_idx,
+                      cudaStream_t st);
+// resolve (launch_join_cond_resolve for the arithmetic pairs, writing them too): pairs [p0, p0 + k) of the group once `passed` is final;
+// bits: the group's pass bits from bit 0.  keep[j] = pair p0 + j passed, or (outer) it is build row 0 of a probe row that passed nothing,
+// whose build_idx[j] then becomes CB_NULL_ROW.
+void launch_nlj_cond_resolve(const unsigned* bits, long long p0, long long k, unsigned row0, unsigned m, unsigned long long inv,
+                             const unsigned char* passed, bool outer, unsigned* probe_idx, unsigned* build_idx, unsigned char* keep, cudaStream_t st);
 // out[i] = !flags[i], i < n
 void launch_flags_not(const unsigned char* flags, long long n, unsigned char* out, cudaStream_t st);
 

@@ -1,5 +1,7 @@
-// join.cpp -- the equi-join node of HashJoin (HashJoinExec with NullEquality::NullEqualsNothing, planner.rs:2192-2266: inner, left semi
-// and left anti) and SortMergeJoin (SortMergeJoinExec with NullEqualsNothing, planner.rs:2126-2190: those and left / right / full outer).
+// join.cpp -- the join node of HashJoin (HashJoinExec with NullEquality::NullEqualsNothing, planner.rs:2192-2266: inner, left semi and
+// left anti), SortMergeJoin (SortMergeJoinExec with NullEqualsNothing, planner.rs:2126-2190: those and left / right / full outer) and
+// BroadcastNestedLoopJoin (NestedLoopJoinExec, planner.rs:1386-1436: inner, left / right outer, left semi and left anti, the shapes whose
+// output follows the streamed side, operators.scala:2258-2266).
 #include "exec_internal.h"
 
 namespace cb200 {
@@ -44,6 +46,16 @@ static std::vector<uint32_t> canonical_codes(const Dictionary& d, const Dictiona
 //     as its NULL-extended row.  FullOuter's unmatched build rows are those whose hit byte no passing pair set.
 // An outer join's sentinel pairs take part in phase 1 with NULLs on both sides and their bits cleared: the condition never sees a
 // NULL-extended row, so an ANSI error comes from a candidate or from nowhere.
+//
+// Nested-loop joins.  A join without keys is run by the same node: every (probe row, build row) pair is a candidate.  The build side is
+// drained and concatenated, with no key, sort or table.  Pairs are numbered probe-row major -- pair p of a group starting at probe row g0
+// is (g0 + p / m, p % m) for m build rows -- and computed by launch_nlj_pairs, so the output order is the hash join's: probe rows in input
+// order, each one's pairs in build input order.  Without a condition an inner / outer join emits all n * m pairs of a probe batch in
+// chunkRows windows, and a semi / anti join passes or drops the whole batch by whether the build side is empty.  With a condition a probe
+// batch is resolved in groups of max(1, chunkRows / m) whole probe rows, so that a group's pass bits and pair indices take O(chunkRows + m)
+// memory however many pairs the batch has: phase 1 runs group by group (semi / anti joins run every group, then compact), and an inner
+// / outer join resolves each group's pairs (launch_nlj_cond_resolve: a probe row that passed nothing keeps its pair with build row 0,
+// NULL-extended) before the next group's phase 1.
 //
 // NULL columns of type t, n rows: the layout (and dictionary) of `like`, or without one the Arrow layout of t and an empty dictionary
 static Column null_column(const DType& t, const Column* like, int64_t n, ExecContext* ctx) {
@@ -107,6 +119,8 @@ struct JoinNode : ExecNode {
     std::vector<int> build_keys, probe_keys; // key columns of each side, in key order
     JoinType type = JoinType::Inner;
     bool build_left = false;
+    bool nested = false;                     // a nested-loop join: no keys, every pair is a candidate
+    unsigned long long nlj_inv = 0;          // nested-loop join: floor((2^64 - 1) / build rows), launch_nlj_pairs' divisor
     int bits = 0, W = 1;                     // packed key bits (fixed per plan) and words
     cb::u64 nullmask[cb::SK_MAX_WORDS] = {0, 0, 0, 0};
 
@@ -133,6 +147,7 @@ struct JoinNode : ExecNode {
     // a probe batch with a condition: the pass bit of each pair, the probe rows with a passing pair, the pairs, those resolved (phase 2)
     DeviceBufP pass_bits, passed, kept_probe, kept_build;
     int64_t cand_total = 0, cand_pos = 0;
+    int64_t grp0 = 0, grp_end = 0;           // nested-loop join with a condition: the probe rows of the current group, [grp0, grp_end)
 
     bool outer() const { return type == JoinType::LeftOuter || type == JoinType::RightOuter || type == JoinType::FullOuter; }
     bool semi_anti() const { return type == JoinType::LeftSemi || type == JoinType::LeftAnti; }
@@ -140,6 +155,11 @@ struct JoinNode : ExecNode {
     std::vector<PipelineSpec> build_specs() const override { return cond ? std::vector<PipelineSpec>{cond->spec(nullptr)} : std::vector<PipelineSpec>{}; }
     // pairs per condition slice: at most chunkRows, a multiple of 32 so that each slice's pass bits start on a word
     int64_t cond_slice() const { return std::max<int64_t>(32, ctx->chunk_rows / 32 * 32); }
+    // nested-loop join with a condition: probe rows per group, at most chunkRows pairs (one row when m exceeds it)
+    int64_t group_rows() const { return std::max<int64_t>(1, std::max<int64_t>(ctx->chunk_rows, 1) / build.n_rows); }
+    // a nested-loop inner / outer join with a condition has probe rows left in the batch after the current group (with an empty build
+    // side an outer join's probe rows are NULL-extended whole, without groups)
+    bool more_groups() const { return nested && cond && !semi_anti() && build.n_rows > 0 && grp_end < probe.n_rows; }
     // the key layout from the declared key types: the last key is the least significant field, each with a null bit above its value
     void set_layout(const std::vector<DType>& key_types) {
         bits = 0;
@@ -176,9 +196,14 @@ struct JoinNode : ExecNode {
 
     void build_table() {
         built = true;
-        build = drain(*build_child, ctx, "joining", "hash join build");
+        build = drain(*build_child, ctx, "joining", nested ? "nested-loop join build" : "hash join build");
         ctx->join_build_rows += build.n_rows;
         if (build.n_rows == 0) return;
+        if (nested) {
+            if (build.n_rows >= ((int64_t)1 << 32)) throw Unsupported("a nested-loop join build side of 2^32 rows or more");
+            nlj_inv = ~0ull / (unsigned long long)build.n_rows;
+            return;
+        }
         TraceSpan ts("join.build");
         const int64_t n = build.n_rows;
         if (n >= ((int64_t)1 << 32)) throw Unsupported("a hash join build side of 2^32 rows or more");
@@ -234,6 +259,11 @@ struct JoinNode : ExecNode {
             total = n;
             return;
         }
+        if (nested) {
+            probe = std::move(in);
+            nested_batch();
+            return;
+        }
         const DeviceBufP pk = pack_row_keys(key_cols(in, probe_keys, false), n, bits, ctx).keys;
         probe = std::move(in);
         if (!semi_anti() || cond) {
@@ -272,26 +302,49 @@ struct JoinNode : ExecNode {
     // rows they keep, inner and outer ones resolve the pairs slice by slice (resolve_slice)
     void evaluate_condition() {
         TraceSpan ts("join.condition");
-        cudaStream_t st = ctx->stream;
-        const int64_t n = probe.n_rows, S = cond_slice();
+        const int64_t n = probe.n_rows;
         pass_bits = std::make_shared<DeviceBuf>((size_t)(total + 31) / 32 * 4 + 8);
         passed = std::make_shared<DeviceBuf>((size_t)n + 16);
+        cuda_check(cudaMemsetAsync(passed->ptr, 0, (size_t)n, ctx->stream), "memset join passed");
+        mark_pairs(total);
+        pos = 0;
+        if (semi_anti()) keep_passed_rows();
+        else {
+            cand_total = total;
+            cand_pos = 0;
+            total = 0;
+            src = Emit::KeptPairs;
+        }
+    }
+
+    // the pairs at positions [p0, p0 + k): of the probe batch (sentinels: an outer join's pair of a probe row without a match), or of
+    // the current group of a nested-loop join
+    void pairs_at(int64_t p0, int64_t k, bool sentinels, unsigned* pidx, unsigned* bidx) {
+        if (nested) launch_nlj_pairs(p0, k, (unsigned)grp0, (unsigned)build.n_rows, nlj_inv, pidx, bidx, ctx->stream);
+        else launch_join_emit(table, (const unsigned*)run_of->ptr, (const unsigned*)offs->ptr, (const unsigned*)chunk_off->ptr, probe.n_rows, p0,
+                              p0 + k, sentinels, pidx, bidx, ctx->stream);
+        cuda_check(cudaGetLastError(), nested ? "k_nlj_pairs launch" : "k_join_emit launch");
+    }
+
+    // phase 1 over `count` pairs (pairs_at): their pass bits from bit 0 of pass_bits, `passed`, and the candidates counted.  A hash
+    // join's outer sentinel pairs take part with NULLs on both sides; a nested-loop join has none.
+    void mark_pairs(int64_t count) {
+        cudaStream_t st = ctx->stream;
+        const int64_t S = cond_slice();
+        const bool sentinels = outer() && !nested;
         auto n_cand = std::make_shared<DeviceBuf>(8);
-        cuda_check(cudaMemsetAsync(passed->ptr, 0, (size_t)n, st), "memset join passed");
         cuda_check(cudaMemsetAsync(n_cand->ptr, 0, 8, st), "memset join candidates");
-        const size_t cap = (size_t)std::max<int64_t>(std::min(S, total), 1) * 4;
+        const size_t cap = (size_t)std::max<int64_t>(std::min(S, count), 1) * 4;
         auto pidx = std::make_shared<DeviceBuf>(cap), bidx = std::make_shared<DeviceBuf>(cap);
-        for (int64_t s = 0; s < total; s += S) {
-            const int64_t k = std::min(S, total - s);
-            if (outer()) { // the sentinel pairs' slots stay (CB_NULL_ROW, CB_NULL_ROW): all NULLs
+        for (int64_t s = 0; s < count; s += S) {
+            const int64_t k = std::min(S, count - s);
+            if (sentinels) { // the sentinel pairs' slots stay (CB_NULL_ROW, CB_NULL_ROW): all NULLs
                 cuda_check(cudaMemsetAsync(pidx->ptr, 0xff, (size_t)k * 4, st), "memset join pairs");
                 cuda_check(cudaMemsetAsync(bidx->ptr, 0xff, (size_t)k * 4, st), "memset join pairs");
             }
-            launch_join_emit(table, (const unsigned*)run_of->ptr, (const unsigned*)offs->ptr, (const unsigned*)chunk_off->ptr, n, s, s + k, false,
-                             (unsigned*)pidx->ptr, (unsigned*)bidx->ptr, st);
-            cuda_check(cudaGetLastError(), "k_join_emit launch");
+            pairs_at(s, k, false, (unsigned*)pidx->ptr, (unsigned*)bidx->ptr);
             cb::u32* bits = (cb::u32*)pass_bits->ptr + s / 32;
-            cond->eval(probe, build, build_left, (const unsigned*)pidx->ptr, (const unsigned*)bidx->ptr, k, outer(), bits);
+            cond->eval(probe, build, build_left, (const unsigned*)pidx->ptr, (const unsigned*)bidx->ptr, k, sentinels, bits);
             launch_join_cond_mark(bits, (const unsigned*)pidx->ptr, (const unsigned*)bidx->ptr, k, (unsigned char*)passed->ptr,
                                   row_hit ? (unsigned char*)row_hit->ptr : nullptr, (unsigned long long*)n_cand->ptr, st);
             cuda_check(cudaGetLastError(), "k_join_cond_mark launch");
@@ -301,25 +354,58 @@ struct JoinNode : ExecNode {
         cuda_check(cudaMemcpyAsync(h_cand, n_cand->ptr, 8, cudaMemcpyDeviceToHost, st), "D2H join candidates");
         ctx->check_device_errors(); // also synchronises: the condition's ANSI errors are raised here
         ctx->join_cond_pairs += *h_cand;
-        pos = 0;
-        if (semi_anti()) {
-            DeviceBufP keep = passed;
-            if (type == JoinType::LeftAnti) {
-                keep = std::make_shared<DeviceBuf>((size_t)n + 16);
-                launch_flags_not((const unsigned char*)passed->ptr, n, (unsigned char*)keep->ptr, st);
-                ctx->kernel_launches++;
-            }
-            Compacted c = compact_rows(keep, n, n, ctx);
-            kept_rows = c.rows;
-            total = c.n;
-            src = Emit::ProbeRows;
-            pass_bits.reset(); passed.reset(); run_of.reset(); offs.reset(); chunk_off.reset();
-        } else {
-            cand_total = total;
-            cand_pos = 0;
-            total = 0;
-            src = Emit::KeptPairs;
+    }
+
+    // semi / anti joins once `passed` is final: the probe rows they keep
+    void keep_passed_rows() {
+        const int64_t n = probe.n_rows;
+        DeviceBufP keep = passed;
+        if (type == JoinType::LeftAnti) {
+            keep = std::make_shared<DeviceBuf>((size_t)n + 16);
+            launch_flags_not((const unsigned char*)passed->ptr, n, (unsigned char*)keep->ptr, ctx->stream);
+            ctx->kernel_launches++;
         }
+        Compacted c = compact_rows(keep, n, n, ctx);
+        kept_rows = c.rows;
+        total = c.n;
+        pos = 0;
+        src = Emit::ProbeRows;
+        pass_bits.reset(); passed.reset(); run_of.reset(); offs.reset(); chunk_off.reset();
+    }
+
+    // a nested-loop join's probe batch, the build side not empty (semi / anti joins without a condition never get here): without a
+    // condition every pair is output; with one, semi / anti joins run phase 1 over every group, inner / outer ones start the first group
+    void nested_batch() {
+        const int64_t n = probe.n_rows, m = build.n_rows;
+        pos = 0;
+        grp0 = grp_end = 0;
+        if (!cond) {
+            total = n * m;
+            src = Emit::Pairs;
+            return;
+        }
+        pass_bits = std::make_shared<DeviceBuf>((size_t)((std::min(n, group_rows()) * m + 31) / 32) * 4 + 8);
+        passed = std::make_shared<DeviceBuf>((size_t)n + 16);
+        cuda_check(cudaMemsetAsync(passed->ptr, 0, (size_t)n, ctx->stream), "memset join passed");
+        if (semi_anti()) {
+            while (grp_end < n) nested_group();
+            keep_passed_rows();
+        } else nested_group();
+    }
+
+    // phase 1 over the next group's pairs; an inner / outer join then resolves them slice by slice (resolve_slice)
+    void nested_group() {
+        TraceSpan ts("join.condition");
+        grp0 = grp_end;
+        grp_end = std::min(probe.n_rows, grp0 + group_rows());
+        const int64_t count = (grp_end - grp0) * build.n_rows;
+        mark_pairs(count);
+        if (semi_anti()) return;
+        cand_total = count;
+        cand_pos = 0;
+        total = 0;
+        pos = 0;
+        src = Emit::KeptPairs;
     }
 
     // phase 2, inner and outer joins: the kept pairs of the next slice (possibly none)
@@ -329,12 +415,18 @@ struct JoinNode : ExecNode {
         const int64_t k = std::min(cond_slice(), cand_total - cand_pos);
         auto pidx = std::make_shared<DeviceBuf>((size_t)k * 4), bidx = std::make_shared<DeviceBuf>((size_t)k * 4);
         auto keep = std::make_shared<DeviceBuf>((size_t)k + 16);
-        launch_join_emit(table, (const unsigned*)run_of->ptr, (const unsigned*)offs->ptr, (const unsigned*)chunk_off->ptr, probe.n_rows, cand_pos,
-                         cand_pos + k, outer(), (unsigned*)pidx->ptr, (unsigned*)bidx->ptr, st);
-        launch_join_cond_resolve((const unsigned*)pass_bits->ptr, cand_pos, (const unsigned*)pidx->ptr, (unsigned*)bidx->ptr, k, (const unsigned*)offs->ptr,
-                                 (const unsigned*)chunk_off->ptr, (const unsigned char*)passed->ptr, outer(), (unsigned char*)keep->ptr, st);
+        if (nested) {
+            launch_nlj_cond_resolve((const unsigned*)pass_bits->ptr, cand_pos, k, (unsigned)grp0, (unsigned)build.n_rows, nlj_inv,
+                                    (const unsigned char*)passed->ptr, outer(), (unsigned*)pidx->ptr, (unsigned*)bidx->ptr, (unsigned char*)keep->ptr, st);
+            ctx->kernel_launches++;
+        } else {
+            launch_join_emit(table, (const unsigned*)run_of->ptr, (const unsigned*)offs->ptr, (const unsigned*)chunk_off->ptr, probe.n_rows, cand_pos,
+                             cand_pos + k, outer(), (unsigned*)pidx->ptr, (unsigned*)bidx->ptr, st);
+            launch_join_cond_resolve((const unsigned*)pass_bits->ptr, cand_pos, (const unsigned*)pidx->ptr, (unsigned*)bidx->ptr, k, (const unsigned*)offs->ptr,
+                                     (const unsigned*)chunk_off->ptr, (const unsigned char*)passed->ptr, outer(), (unsigned char*)keep->ptr, st);
+            ctx->kernel_launches += 2;
+        }
         cuda_check(cudaGetLastError(), "join condition resolve");
-        ctx->kernel_launches += 2;
         Compacted c = compact_rows(keep, k, k, ctx, {{pidx, 4}, {bidx, 4}});
         kept_probe = c.extra_out[0];
         kept_build = c.extra_out[1];
@@ -381,9 +473,7 @@ struct JoinNode : ExecNode {
             if (src == Emit::Pairs) {
                 pidx = std::make_shared<DeviceBuf>((size_t)k * 4);
                 bidx = std::make_shared<DeviceBuf>((size_t)k * 4);
-                launch_join_emit(table, (const unsigned*)run_of->ptr, (const unsigned*)offs->ptr, (const unsigned*)chunk_off->ptr, probe.n_rows, pos, pos + k,
-                                 outer(), (unsigned*)pidx->ptr, (unsigned*)bidx->ptr, ctx->stream);
-                cuda_check(cudaGetLastError(), "k_join_emit launch");
+                pairs_at(pos, k, outer(), (unsigned*)pidx->ptr, (unsigned*)bidx->ptr);
                 ctx->kernel_launches++;
                 pi = (const unsigned*)pidx->ptr;
                 bi = (const unsigned*)bidx->ptr;
@@ -415,7 +505,7 @@ struct JoinNode : ExecNode {
         pos += k;
         ctx->join_out_rows += k;
         ctx->check_device_errors();
-        if (pos >= total && cand_pos >= cand_total) {
+        if (pos >= total && cand_pos >= cand_total && !more_groups()) {
             probe = Batch(); run_of.reset(); offs.reset(); chunk_off.reset(); kept_rows.reset();
             pass_bits.reset(); passed.reset(); kept_probe.reset(); kept_build.reset();
         }
@@ -430,6 +520,7 @@ struct JoinNode : ExecNode {
         for (;;) {
             if (pos < total) { emit(out); return true; }
             if (cand_pos < cand_total) { resolve_slice(); continue; }
+            if (more_groups()) { nested_group(); continue; }
             if (probe_done) return false;
             Batch in;
             if (!probe_child->next(in)) {
@@ -452,6 +543,12 @@ struct JoinNode : ExecNode {
                 out = std::move(in);
                 return true;
             }
+            if (nested && !cond && semi_anti()) { // the build side is not empty and every pair passes: LeftSemi keeps the batch, LeftAnti none of it
+                if (type == JoinType::LeftAnti) continue;
+                ctx->join_out_rows += in.n_rows;
+                out = std::move(in);
+                return true;
+            }
             probe_batch(in);
         }
     }
@@ -463,6 +560,7 @@ ExecNodeP make_join_node(const OperatorP& op, const ExecNodeP& left, const ExecN
     n->schema = op->schema;
     n->type = op->join_type;
     n->build_left = op->build_left;
+    n->nested = op->left_keys.empty();
     std::vector<int> lk, rk;
     std::vector<DType> key_types;
     for (size_t i = 0; i < op->left_keys.size(); i++) {
@@ -485,9 +583,11 @@ ExecNodeP make_join_node(const OperatorP& op, const ExecNodeP& left, const ExecN
         c->n_left = (int)left->schema.size();
         c->predicates = {op->join_condition};
         c->assign_slots(c->predicates);
-        if (c->used_cols.empty()) { // a condition of literals alone: the pass still needs a staged column, the first left key
-            c->used_cols.push_back(lk[0]);
-            c->slot_of[lk[0]] = 0;
+        if (c->used_cols.empty()) { // a condition of literals alone: the pass still needs a staged column, the first left key (without
+                                    // keys, the probe side's first column)
+            const int staged = lk.empty() ? (op->build_left ? c->n_left : 0) : lk[0];
+            c->used_cols.push_back(staged);
+            c->slot_of[staged] = 0;
         }
         n->cond = c;
     }

@@ -900,6 +900,39 @@ static OperatorP decode_operator(PbReader r) { // Operator operator.proto:32-86
         have = true;
         break;
     }
+    case 117: { // BroadcastNestedLoopJoin operator.proto:773-777 (planner.rs:1386-1436: NestedLoopJoinExec, BuildRight swaps the inputs)
+        // Run by the hash join's node without keys: every pair is a candidate, the streamed side is probed.  Comet's serde sends the
+        // shapes whose output follows the streamed side (operators.scala:2258-2266); the others would need the build side's rows merged
+        // across partitions.
+        op->kind = OpKind::HashJoin;
+        int64_t join_type = 0, build_side = 0;
+        while (b.next()) {
+            if (b.field == 1) join_type = b.i64();
+            else if (b.field == 2) build_side = b.i64();
+            else if (b.field == 3 && b.wire == 2) op->join_condition = decode_join_condition(b.sub());
+            else b.skip();
+        }
+        if (op->children.size() != 2) throw PlanError("nested-loop join expects two children");
+        if (join_type < 0 || join_type > 5) throw PlanError("unknown join type " + std::to_string(join_type));
+        if (build_side != 0 && build_side != 1) throw PlanError("unknown build side " + std::to_string(build_side));
+        op->join_type = (JoinType)join_type;
+        op->build_left = build_side == 0;
+        const JoinType jt = op->join_type;
+        const bool accepted = jt == JoinType::Inner || (jt == JoinType::LeftOuter && !op->build_left) || (jt == JoinType::RightOuter && op->build_left) ||
+                              ((jt == JoinType::LeftSemi || jt == JoinType::LeftAnti) && !op->build_left);
+        if (!accepted) {
+            static const char* names[] = {"inner", "left outer", "right outer", "full outer", "left semi", "left anti"};
+            throw Unsupported(std::string(names[join_type]) + " nested-loop join with " + (op->build_left ? "BuildLeft" : "BuildRight") +
+                              " (only inner, left outer / semi / anti with BuildRight and right outer with BuildLeft: the output follows the streamed side)");
+        }
+        const auto &ls = op->children[0]->schema, &rs = op->children[1]->schema;
+        if (ls.empty() || rs.empty()) throw Unsupported("a nested-loop join side without columns");
+        op->schema = ls;
+        if (jt != JoinType::LeftSemi && jt != JoinType::LeftAnti) op->schema.insert(op->schema.end(), rs.begin(), rs.end());
+        resolve_join_condition(*op);
+        have = true;
+        break;
+    }
     default:
         throw Unsupported("operator field " + std::to_string(f) + " is outside the GPU hot path");
     }

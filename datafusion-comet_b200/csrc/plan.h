@@ -159,6 +159,7 @@ struct Operator {
     // HashJoin (operator.proto:754-763) and SortMergeJoin (:765-771): equi-join on Bound key columns of children[0] (left) and
     // children[1] (right).  Inner and the outer types: the output is the left columns, then the right ones; LeftSemi / LeftAnti: the
     // left columns.  A sort-merge join's build side follows from its type: the left one for RightOuter, else the right one.
+    // BroadcastNestedLoopJoin (:773-777) is the same operator without keys: every (left row, right row) pair is a candidate.
     std::vector<ExprP> left_keys, right_keys;
     JoinType join_type = JoinType::Inner;
     bool build_left = false; // BuildLeft: the left child is the build side (the hash table), the right one is probed

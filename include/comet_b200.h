@@ -202,12 +202,13 @@ typedef struct cb200_stats {
     int64_t sort_passes;       /* radix passes they ran: one per 8-bit key digit that is not the same in every row */
     int64_t sort_pass_rows;    /* rows those passes moved, summed over the passes */
     int64_t sort_select_rows;  /* rows TopK's radix select read, summed over its digit steps */
-    int64_t join_build_rows;   /* rows HashJoin and SortMergeJoin operators drained from their build side into the hash table's input */
-    int64_t join_probe_rows;   /* probe-side rows they looked up */
+    int64_t join_build_rows;   /* rows HashJoin, SortMergeJoin and BroadcastNestedLoopJoin operators drained from their build side */
+    int64_t join_probe_rows;   /* probe-side (streamed-side) rows they looked up or paired */
     int64_t join_out_rows;     /* rows they emitted */
     int64_t agg_range_levels;  /* OR of CB200_RANGE_* over the dense aggregate launches that were kept: which value-range assumptions ran */
     int64_t agg_range_reruns;  /* dense aggregate launches discarded because their input broke the value range the kernel assumed */
-    int64_t join_cond_pairs;   /* candidate pairs (equal keys) of HashJoin and SortMergeJoin operators their join condition was evaluated on */
+    int64_t join_cond_pairs;   /* candidate pairs their join condition was evaluated on: pairs with equal keys (HashJoin, SortMergeJoin), every
+                                  (probe row, build row) pair (BroadcastNestedLoopJoin: n * m per probe batch when the build side has rows) */
 } cb200_stats;
 #define CB200_AGG_DENSE 1      /* thread-private accumulators over dictionary / bool key codes (and ungrouped aggregates) */
 #define CB200_AGG_TABLE 2      /* global key table */
