@@ -144,6 +144,18 @@ def literal(value, dt):
     return _expr("literal", body)
 
 
+def literal_bits(bits, dt):
+    """a FLOAT / DOUBLE literal given by its own 32 / 64 bits: every NaN sign and payload, and -0.0, exactly as written (a Python
+    float would pass a float32 NaN through a double)"""
+    if dt.name == "FLOAT":
+        body = _tag(LITERAL_FIELD["float_val"], FIXED32) + struct.pack("<I", bits & 0xFFFFFFFF)
+    elif dt.name == "DOUBLE":
+        body = _tag(LITERAL_FIELD["double_val"], FIXED64) + struct.pack("<Q", bits & 0xFFFFFFFFFFFFFFFF)
+    else:
+        raise ValueError(dt)
+    return _expr("literal", body + f_len(LITERAL_FIELD["datatype"], dt.encode()))
+
+
 def _math(kind, l, r, ret, eval_mode=LEGACY):  # MathExpr expr.proto:330
     return _expr(kind, f_len(1, l) + f_len(2, r) + f_len(4, ret.encode()) + f_varint(5, eval_mode))
 
@@ -313,6 +325,26 @@ def hash_agg(child, grouping, aggs, mode=PARTIAL, plan_id=0, expr_modes=None, in
 
 def hash_partitioning(exprs, num_partitions):  # partitioning.proto:38
     return f_len(1, b"".join(f_len(1, e) for e in exprs) + f_varint(2, num_partitions))
+
+
+PARTITIONING_FIELD = dict(hash_partition=1, single_partition=2, range_partition=3, round_robin_partition=4)  # partitioning.proto:29-36
+
+
+def single_partitioning():  # partitioning.proto:43
+    return f_len(PARTITIONING_FIELD["single_partition"], b"")
+
+
+def range_partitioning(sort_orders, num_partitions, boundary_rows):  # RangePartition partitioning.proto:49-53
+    """sort_orders: sort_order(...) expressions; boundary_rows: lists of literal(...) / literal_bits(...) expressions, one per
+    (deduplicated) sort order, in ascending order of the sort orders"""
+    body = b"".join(f_len(1, o) for o in sort_orders) + f_varint(2, num_partitions)
+    body += b"".join(f_len(4, b"".join(f_len(1, e) for e in row)) for row in boundary_rows)  # BoundaryRow { partition_bounds = 1 }
+    return f_len(PARTITIONING_FIELD["range_partition"], body)
+
+
+def round_robin_partitioning(num_partitions, max_hash_columns=0):  # RoundRobinPartition partitioning.proto:55-59
+    """murmur3 over the first max_hash_columns columns (<= 0: all of them), pmod num_partitions"""
+    return f_len(PARTITIONING_FIELD["round_robin_partition"], f_varint(1, num_partitions) + f_varint(2, max_hash_columns))
 
 
 def shuffle_writer(child, partitioning, plan_id=0):  # operator.proto:688

@@ -360,6 +360,9 @@ int cb200_plan_stats(cb200_plan* plan, cb200_stats* out) {
     out->agg_range_levels = c.agg_range_levels;
     out->agg_range_reruns = c.agg_range_reruns;
     out->join_cond_pairs = c.join_cond_pairs;
+    out->partition_ids_ms = c.partition_ids_ms;
+    out->partition_place_ms = c.partition_place_ms;
+    out->partition_gather_ms = c.partition_gather_ms;
     return 0;
 }
 

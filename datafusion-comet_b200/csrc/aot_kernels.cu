@@ -4,6 +4,7 @@
 // codes.  (Plan-dependent kernels are JIT-specialised: device/cb_kernels.cuh.)
 #include "aot_kernels.h"
 #include "device/cb_math.h"
+#include "device/cb_rangepart.h"
 #include "device/cb_strpred.h"
 
 #include <algorithm>
@@ -250,10 +251,8 @@ using namespace cb;
 
 __device__ __forceinline__ bool bit_at(const u8* bm, i64 i) { return (bm[i >> 3] >> (i & 7)) & 1; }
 
-__global__ void k_partition_ids(HashKeyCols kc, i64 n, u32 n_parts, u32* hashes, u32* pids) {
-    i64 i = (i64)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    u32 h = 42u; // spark seed (multi_partition.rs:298)
+// h chained over row i's key columns by Spark's murmur3 rules
+__device__ __forceinline__ u32 hash_key_cols(const HashKeyCols& kc, i64 i, u32 h) {
     for (int c = 0; c < kc.n; c++) {
         const HashKeyCol& k = kc.col[c];
         if (k.validity && !bit_at(k.validity, i)) continue; // NULL leaves the running hash unchanged (utils.rs:38-42)
@@ -284,8 +283,40 @@ __global__ void k_partition_ids(HashKeyCols kc, i64 n, u32 n_parts, u32* hashes,
         }
         }
     }
+    return h;
+}
+
+__global__ void k_partition_ids(HashKeyCols kc, i64 n, u32 n_parts, u32* hashes, u32* pids) {
+    i64 i = (i64)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const u32 h = hash_key_cols(kc, i, 42u); // spark seed (multi_partition.rs:298)
     if (hashes) hashes[i] = h;
     pids[i] = pmod_u32(h, n_parts);
+}
+
+// one group of at most 8 columns of a longer hash chain (round-robin partitioning over more columns): the first group starts from the
+// seed, the others from hashes[i]; the last writes pids[i] = pmod, the others the running hash back to hashes[i]
+__global__ void k_partition_ids_chain(HashKeyCols kc, i64 n, u32 n_parts, int first, int last, u32* hashes, u32* pids) {
+    i64 i = (i64)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const u32 h = hash_key_cols(kc, i, first ? 42u : hashes[i]);
+    if (last) pids[i] = pmod_u32(h, n_parts);
+    else hashes[i] = h;
+}
+
+// Range partitioning: pids[i] = the number of boundary rows <= row i's packed key (device/cb_rangepart.h).  The key has W words, a
+// template constant, so it is built and compared in registers.  The top level of the search (all boundary rows, or every 2^shift-th)
+// is staged in shared memory once per CTA of a grid-stride loop; with shift > 0 the search ends in `bounds`, which stays in L2.
+template <int W>
+__global__ void __launch_bounds__(256) k_range_pids(SortKeyCols kc, i64 n, const u64* top, u32 n_top, int shift, const u64* bounds, u32 nb, u32* pids) {
+    extern __shared__ u64 s_top[];
+    for (u32 j = threadIdx.x; j < n_top * (u32)W; j += blockDim.x) s_top[j] = top[j];
+    __syncthreads();
+    for (i64 i = (i64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (i64)gridDim.x * blockDim.x) {
+        u64 w[W] = {};
+        if (!sk_row_reg<W>(kc, i, w)) atomicOr(kc.err, 1 << 5);
+        pids[i] = rp_pid<W>(s_top, n_top, shift, bounds, nb, w);
+    }
 }
 
 // per-1024-row-block histogram of partition ids -> block_hist[block][n_parts]
@@ -393,26 +424,64 @@ __global__ void k_gather_bits_or_null(const u8* in_bits, const u32* row_idx, i64
 }
 
 i64 partition_chunks(i64 n) { const i64 nb = (n + 1023) / 1024; return (nb + PID_CHUNK - 1) / PID_CHUNK; }
-cudaError_t launch_partition(const HashKeyCols& kc, i64 n, u32 n_parts, u32* hashes, u32* pids, i32* block_hist, i64* block_base, i64* chunk_tmp,
-                             i64* starts, i64* row_idx, cudaStream_t st) {
-    if (n <= 0) return cudaSuccess;
+// one counter per partition in shared memory: above the default 48 KB a kernel has to opt in
+static cudaError_t partition_smem_setup(u32 n_parts, int& smem32, int& smem64) {
     if (n_parts == 0 || n_parts > (u32)CB_MAX_HASH_PARTITIONS) return cudaErrorInvalidValue;
-    // one counter per partition in shared memory: above the default 48 KB a kernel has to opt in
-    const int smem32 = (int)(n_parts * sizeof(i32)), smem64 = (int)(n_parts * sizeof(i64));
+    smem32 = (int)(n_parts * sizeof(i32)), smem64 = (int)(n_parts * sizeof(i64));
     cudaError_t e = cudaSuccess;
     if (smem32 > 48 * 1024) e = cudaFuncSetAttribute((const void*)k_pid_block_hist, cudaFuncAttributeMaxDynamicSharedMemorySize, smem32);
     if (smem64 > 48 * 1024 && e == cudaSuccess) e = cudaFuncSetAttribute((const void*)k_pid_chunk_scan, cudaFuncAttributeMaxDynamicSharedMemorySize, smem64);
     if (smem64 > 48 * 1024 && e == cudaSuccess) e = cudaFuncSetAttribute((const void*)k_pid_place, cudaFuncAttributeMaxDynamicSharedMemorySize, smem64);
-    if (e != cudaSuccess) return e;
-    i64 nb = (n + 1023) / 1024;
-    const i64 nc = partition_chunks(n);
+    return e;
+}
+cudaError_t launch_partition_ids(const HashKeyCols& kc, i64 n, u32 n_parts, u32* hashes, u32* pids, cudaStream_t st) {
+    if (n <= 0) return cudaSuccess;
+    if (n_parts == 0 || n_parts > (u32)CB_MAX_HASH_PARTITIONS) return cudaErrorInvalidValue;
     k_partition_ids<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(kc, n, n_parts, hashes, pids);
+    return cudaGetLastError();
+}
+cudaError_t launch_partition_place(const u32* pids, i64 n, u32 n_parts, i32* block_hist, i64* block_base, i64* chunk_tmp, i64* starts, i64* row_idx,
+                                   cudaStream_t st) {
+    if (n <= 0) return cudaSuccess;
+    int smem32 = 0, smem64 = 0;
+    cudaError_t e = partition_smem_setup(n_parts, smem32, smem64);
+    if (e != cudaSuccess) return e;
+    const i64 nb = (n + 1023) / 1024, nc = partition_chunks(n);
     k_pid_block_hist<<<(unsigned)nb, 256, smem32, st>>>(pids, n, n_parts, block_hist);
     k_pid_chunk_totals<<<(unsigned)nc, 256, 0, st>>>(block_hist, nb, n_parts, chunk_tmp);
     k_pid_chunk_scan<<<1, 256, smem64, st>>>(chunk_tmp, nc, n_parts, starts);
     k_pid_block_bases<<<(unsigned)nc, 256, 0, st>>>(block_hist, nb, n_parts, chunk_tmp, block_base);
     k_pid_place<<<(unsigned)nb, 64, smem64, st>>>(pids, n, n_parts, block_base, row_idx);
     return cudaGetLastError();
+}
+cudaError_t launch_partition_ids_chain(const HashKeyCols& kc, i64 n, u32 n_parts, bool first, bool last, u32* hashes, u32* pids, cudaStream_t st) {
+    if (n <= 0) return cudaSuccess;
+    k_partition_ids_chain<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(kc, n, n_parts, first, last, hashes, pids);
+    return cudaGetLastError();
+}
+template <int W> static cudaError_t range_pids(const SortKeyCols& kc, i64 n, const u64* top, u32 n_top, int shift, const u64* bounds, u32 nb, u32* pids,
+                                               cudaStream_t st) {
+    const size_t smem = (size_t)n_top * W * 8;
+    // grid-stride over one wave: as many CTAs as fit on the device at once with this much shared memory each
+    int dev = 0, sms = 0, per_sm = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_range_pids<W>, 256, smem);
+    if (e != cudaSuccess) return e;
+    const i64 blocks = std::min<i64>((n + 255) / 256, (i64)std::max(1, sms * per_sm));
+    k_range_pids<W><<<(unsigned)blocks, 256, smem, st>>>(kc, n, top, n_top, shift, bounds, nb, pids);
+    return cudaGetLastError();
+}
+cudaError_t launch_range_pids(const SortKeyCols& kc, i64 n, const u64* top, u32 n_top, int shift, const u64* bounds, u32 nb, u32* pids, cudaStream_t st) {
+    if (n <= 0) return cudaSuccess;
+    if ((size_t)n_top * kc.words * 8 > CB_RANGE_TOP_BYTES) return cudaErrorInvalidValue;
+    switch (kc.words) {
+    case 1: return range_pids<1>(kc, n, top, n_top, shift, bounds, nb, pids, st);
+    case 2: return range_pids<2>(kc, n, top, n_top, shift, bounds, nb, pids, st);
+    case 3: return range_pids<3>(kc, n, top, n_top, shift, bounds, nb, pids, st);
+    case 4: return range_pids<4>(kc, n, top, n_top, shift, bounds, nb, pids, st);
+    default: return cudaErrorInvalidValue;
+    }
 }
 template <typename I> static void gather_rows(const void* in, int width, const I* row_idx, i64 n, void* out, cudaStream_t st) {
     if (n <= 0) return;

@@ -45,12 +45,26 @@ struct HashKeyCols {
     int n;
     HashKeyCol col[8];
 };
-long long partition_chunks(long long n); // entries per partition of launch_partition's chunk_tmp scratch
+long long partition_chunks(long long n); // entries per partition of launch_partition_place's chunk_tmp scratch
 // n_parts <= CB_MAX_HASH_PARTITIONS: three of the kernels keep one counter per partition in shared memory (8 bytes each at most)
 enum { CB_MAX_HASH_PARTITIONS = 16384 };
-// returns the first error of the launches (a launch the device refuses is reported here, not by a later synchronisation)
-cudaError_t launch_partition(const HashKeyCols& kc, long long n, unsigned n_parts, unsigned* hashes, unsigned* pids, int* block_hist, long long* block_base,
-                      long long* chunk_tmp, long long* starts, long long* row_idx, cudaStream_t st);
+// Each launcher returns the first error of its launches (a launch the device refuses is reported here, not by a later synchronisation).
+// pids[i] = pmod(murmur3 seed 42 chained over the key columns, n_parts), hashes[i] the hash when hashes is not null
+cudaError_t launch_partition_ids(const HashKeyCols& kc, long long n, unsigned n_parts, unsigned* hashes, unsigned* pids, cudaStream_t st);
+// the stable counting sort by partition id (pids[i] < n_parts): starts[n_parts + 1] and row_idx[n], the rows in partition order
+cudaError_t launch_partition_place(const unsigned* pids, long long n, unsigned n_parts, int* block_hist, long long* block_base, long long* chunk_tmp,
+                                   long long* starts, long long* row_idx, cudaStream_t st);
+// murmur3 chained over more than 8 key columns, one launch per group of at most 8 (kc): the first group starts from seed 42, the
+// others from hashes[i]; the last writes pids[i] = pmod(h, n_parts), the others write the running hash to hashes[i]
+cudaError_t launch_partition_ids_chain(const HashKeyCols& kc, long long n, unsigned n_parts, bool first, bool last, unsigned* hashes, unsigned* pids,
+                                       cudaStream_t st);
+// range partitioning (device/cb_rangepart.h): pids[i] = the number of the nb boundary rows (kc.words words each, non-decreasing) <= row
+// i's key packed by kc.  top / n_top / shift: the top level of the search, staged in shared memory (n_top * words * 8 <=
+// CB_RANGE_TOP_BYTES): the boundary rows themselves with shift 0, else every 2^shift-th of them (rp_shift).  A dictionary code outside
+// its rank table sets error bit 5.
+enum { CB_RANGE_TOP_BYTES = 48 * 1024 };
+cudaError_t launch_range_pids(const cb::SortKeyCols& kc, long long n, const unsigned long long* top, unsigned n_top, int shift,
+                              const unsigned long long* bounds, unsigned nb, unsigned* pids, cudaStream_t st);
 // out[i] = in[row_idx[i]] (width bytes per row), i < n; 64-bit (partitioning) or 32-bit (sort) row indices
 void launch_gather(const void* in, int width, const long long* row_idx, long long n, void* out, cudaStream_t st);
 void launch_gather(const void* in, int width, const unsigned* row_idx, long long n, void* out, cudaStream_t st);

@@ -78,26 +78,42 @@ CB_HD bool sk_value(const SortKeyCol& k, i64 i, u64& hi, u64& lo) {
     return true;
 }
 
-// OR row i's fields into w[0, kc.words) (zeroed by the caller); false if a dictionary code was out of range
-CB_HD bool sk_row(const SortKeyCols& kc, i64 i, u64* w) {
+// row i's fields as put(off, v, nb) calls (OR nb <= 64 bits of v at bit offset off); false if a dictionary code was out of range
+template <typename Put> CB_HD bool sk_fields(const SortKeyCols& kc, i64 i, Put put) {
     bool ok = true;
     for (int c = 0; c < kc.n; c++) {
         const SortKeyCol& k = kc.col[c];
         const bool valid = !k.validity || ((k.validity[i >> 3] >> (i & 7)) & 1);
-        if (k.has_null) sk_put(w, kc.words, k.off + k.bits, (valid == (bool)k.nulls_first) ? 1u : 0u, 1); // valid rows after NULLs iff nulls_first
+        if (k.has_null) put(k.off + k.bits, (valid == (bool)k.nulls_first) ? 1u : 0u, 1); // valid rows after NULLs iff nulls_first
         if (!valid) continue;
         u64 hi, lo;
         if (!sk_value(k, i, hi, lo)) ok = false;
         if (k.bits > 64) {
             if (k.desc) { hi = ~hi; lo = ~lo; }
-            sk_put(w, kc.words, k.off, lo, 64);
-            sk_put(w, kc.words, k.off + 64, hi & sk_mask(k.bits - 64), k.bits - 64);
+            put(k.off, lo, 64);
+            put(k.off + 64, hi & sk_mask(k.bits - 64), k.bits - 64);
         } else {
             if (k.desc) lo = ~lo & sk_mask(k.bits);
-            sk_put(w, kc.words, k.off, lo, k.bits);
+            put(k.off, lo, k.bits);
         }
     }
     return ok;
+}
+
+// OR row i's fields into w[0, kc.words) (zeroed by the caller); false if a dictionary code was out of range
+CB_HD bool sk_row(const SortKeyCols& kc, i64 i, u64* w) {
+    return sk_fields(kc, i, [&](int off, u64 v, int nb) { sk_put(w, kc.words, off, v, nb); });
+}
+
+// sk_row for a key of W words (W == kc.words) kept in registers: every word is addressed by a constant index
+template <int W> CB_HD bool sk_row_reg(const SortKeyCols& kc, i64 i, u64 (&w)[W]) {
+    return sk_fields(kc, i, [&](int off, u64 v, int nb) {
+        const int lw = off >> 6, sh = off & 63;
+        for (int j = 0; j < W; j++) {
+            if (j == W - 1 - lw) w[j] |= v << sh;
+            if (sh && sh + nb > 64 && j == W - 2 - lw) w[j] |= v >> (64 - sh);
+        }
+    });
 }
 
 } // namespace cb

@@ -3,9 +3,12 @@
 // partitioning}.proto (cited inline).  Type rules: native/core/src/execution/planner.rs.
 #include "plan.h"
 #include "proto_wire.h"
+#include "device/cb_rangepart.h"
+#include "device/cb_sortkey.h"
 #include "device/cb_strpred.h"
 
 #include <algorithm>
+#include <cstring>
 #include <sstream>
 
 namespace cb200 {
@@ -88,8 +91,8 @@ static ExprP decode_literal(PbReader r) {
     while (r.next()) {
         switch (r.field) {
         case 1: case 2: case 3: case 4: case 5: e->lit_i64 = r.i64(); have_value = true; break;
-        case 6: e->lit_f64 = (double)r.f32(); have_value = true; break;
-        case 7: e->lit_f64 = r.f64(); have_value = true; break;
+        case 6: { const uint32_t u = r.fixed32(); float f; memcpy(&f, &u, 4); e->lit_f64 = (double)f; e->lit_bits = u; have_value = true; break; }
+        case 7: { const uint64_t u = r.fixed64(); memcpy(&e->lit_f64, &u, 8); e->lit_bits = u; have_value = true; break; }
         case 8: case 9: e->lit_str = r.bytes(); have_value = true; break;
         case 10: dec_bytes = r.bytes(); have_value = true; break;
         case 11: throw Unsupported("list literals are outside the GPU hot path");
@@ -650,6 +653,126 @@ static ExprP decode_join_condition(PbReader r) {
     }
 }
 
+// RangePartition (planner.rs:3298-3358): the sort orders resolved against the child and deduplicated by column, as DataFusion's
+// LexOrdering drops a repeated expression (the JVM sends every sort order but boundary rows of the deduplicated ones,
+// CometNativeShuffleWriter.scala:263-326), and the first k entries of each boundary row, k the deduplicated key count, packed once as
+// row keys.  A row's partition is then the number of packed bounds <= its packed key (multi_partition.rs:333-380 partition_point).
+static void decode_range_partitioning(Operator& op, const std::vector<DType>& cs, std::vector<PbReader>& rows) {
+    if (op.range_keys.empty()) throw PlanError("range partitioning without sort orders");
+    std::vector<SortKey> keys;
+    for (auto& k : op.range_keys) {
+        resolve(*k.expr, cs);
+        if (k.expr->kind != ExprKind::Bound) throw Unsupported("computed range-partition keys (only plain column keys: put a Projection below the shuffle writer)");
+        bool seen = false;
+        for (auto& q : keys) seen = seen || q.expr->index == k.expr->index;
+        if (!seen) keys.push_back(k);
+    }
+    op.range_keys = keys;
+    const size_t K = keys.size();
+    if (K > MAX_SORT_KEYS) throw Unsupported("more than 8 range-partition keys");
+    int bits = 0;
+    for (auto& k : keys) {
+        if (k.expr->type.id == TypeId::Binary) throw Unsupported("range-partition key of type binary");
+        try {
+            bits += sort_key_bits(k.expr->type) + 1; // every field carries a null bit
+        } catch (const Unsupported&) {
+            throw Unsupported("range-partition key of type " + k.expr->type.str());
+        }
+    }
+    if (bits > MAX_SORT_KEY_BITS) throw Unsupported("range-partition keys of " + std::to_string(bits) + " bits (at most 256 bits of packed key)");
+    if ((int64_t)rows.size() >= op.num_partitions)
+        throw PlanError(std::to_string(rows.size()) + " range boundary rows for " + std::to_string(op.num_partitions) + " partitions (at most " +
+                        std::to_string(op.num_partitions - 1) + ")");
+    // the boundary entries: literals of their key's type
+    std::vector<std::vector<ExprP>> bound(rows.size());
+    for (size_t r = 0; r < rows.size(); r++) {
+        PbReader br = rows[r];
+        while (br.next()) {
+            if (br.field == 1 && br.wire == 2) bound[r].push_back(decode_expr(br.sub()));
+            else br.skip();
+        }
+        if (bound[r].size() < K)
+            throw PlanError("range boundary row " + std::to_string(r) + " has " + std::to_string(bound[r].size()) + " entries for " + std::to_string(K) + " keys");
+        for (size_t k = 0; k < K; k++) {
+            const Expr& e = *bound[r][k];
+            if (e.kind != ExprKind::Literal) throw PlanError("range boundary row " + std::to_string(r) + " entry " + std::to_string(k) + " is not a literal");
+            if (e.type != keys[k].expr->type)
+                throw PlanError("range boundary row " + std::to_string(r) + " entry " + std::to_string(k) + " is " + e.type.str() + ", its key " + keys[k].expr->type.str());
+        }
+    }
+    op.range_strs.assign(K, {});
+    for (size_t k = 0; k < K; k++) {
+        if (keys[k].expr->type.id != TypeId::String) continue;
+        auto& v = op.range_strs[k];
+        for (auto& row : bound)
+            if (!row[k]->lit_null) v.push_back(row[k]->lit_str);
+        std::sort(v.begin(), v.end());
+        v.erase(std::unique(v.begin(), v.end()), v.end());
+    }
+    // pack each row with the row-key encoder itself: a one-row column per key in the layout the encoder reads for its type
+    const int W = op.range_words = std::max(1, (bits + 63) / 64);
+    op.n_bounds = (int64_t)rows.size();
+    op.range_bounds.assign((size_t)op.n_bounds * W, 0);
+    struct Cell { uint64_t v[2]; uint8_t valid; uint32_t rank; };
+    std::vector<Cell> cells(K);
+    cb::SortKeyCols kc;
+    memset(&kc, 0, sizeof(kc));
+    kc.n = (int)K;
+    kc.words = W;
+    int off = 0;
+    for (size_t k = K; k-- > 0;) { // the last key is the least significant field
+        const DType& t = keys[k].expr->type;
+        cb::SortKeyCol& f = kc.col[k];
+        f.bits = sort_key_bits(t);
+        switch (t.id) {
+        case TypeId::Bool: f.kind = HK_BOOL8; break;
+        case TypeId::Int8: f.kind = HK_I8; break;
+        case TypeId::Int16: f.kind = HK_I16; break;
+        case TypeId::Int32: case TypeId::Date: f.kind = HK_I32; break;
+        case TypeId::Float32: f.kind = HK_F32; break;
+        case TypeId::Float64: f.kind = HK_F64; break;
+        case TypeId::Decimal: f.kind = t.precision <= 18 ? HK_DEC_SMALL_64 : HK_DEC_LARGE_128; break;
+        case TypeId::String: f.kind = HK_DICT32; f.rank = &cells[k].rank; f.n_rank = 1; break;
+        default: f.kind = HK_I64; break; // int64, timestamps
+        }
+        f.off = off;
+        off += f.bits + 1;
+        f.desc = keys[k].descending;
+        f.nulls_first = keys[k].nulls_first;
+        f.has_null = 1;
+        f.data = cells[k].v;
+        f.validity = &cells[k].valid;
+    }
+    for (size_t r = 0; r < rows.size(); r++) {
+        for (size_t k = 0; k < K; k++) {
+            const Expr& e = *bound[r][k];
+            Cell& c = cells[k];
+            c.v[0] = c.v[1] = 0;
+            c.valid = e.lit_null ? 0 : 1;
+            c.rank = 0;
+            switch (e.type.id) {
+            case TypeId::Bool: c.v[0] = e.lit_i64 != 0; break;
+            case TypeId::Int8: { const int8_t x = (int8_t)e.lit_i64; memcpy(c.v, &x, 1); break; }
+            case TypeId::Int16: { const int16_t x = (int16_t)e.lit_i64; memcpy(c.v, &x, 2); break; }
+            case TypeId::Int32: case TypeId::Date: { const int32_t x = (int32_t)e.lit_i64; memcpy(c.v, &x, 4); break; }
+            case TypeId::Float32: { const uint32_t x = (uint32_t)e.lit_bits; memcpy(c.v, &x, 4); break; }
+            case TypeId::Float64: c.v[0] = e.lit_bits; break;
+            case TypeId::Decimal: c.v[0] = (uint64_t)e.lit_dec; c.v[1] = (uint64_t)(e.lit_dec >> 64); break;
+            case TypeId::String: {
+                const auto& v = op.range_strs[k];
+                if (!e.lit_null) c.rank = 2 * (uint32_t)(std::lower_bound(v.begin(), v.end(), e.lit_str) - v.begin()) + 1;
+                break;
+            }
+            default: c.v[0] = (uint64_t)e.lit_i64; break;
+            }
+        }
+        cb::u64* w = (cb::u64*)&op.range_bounds[r * (size_t)W];
+        cb::sk_row(kc, 0, w);
+        if (r > 0 && std::lexicographical_compare(w, w + W, w - W, w))
+            throw PlanError("range boundary row " + std::to_string(r) + " sorts before row " + std::to_string(r - 1) + " (boundary rows must be in ascending order of the sort orders)");
+    }
+}
+
 static OperatorP decode_operator(PbReader r) { // Operator operator.proto:32-86
     auto op = std::make_shared<Operator>();
     bool have = false;
@@ -802,8 +925,9 @@ static OperatorP decode_operator(PbReader r) { // Operator operator.proto:32-86
         have = true;
         break;
     }
-    case 106: { // ShuffleWriter operator.proto:688 (hash partitioning only)
+    case 106: { // ShuffleWriter operator.proto:688
         op->kind = OpKind::ShuffleWriter;
+        std::vector<PbReader> bound_rows;
         while (b.next()) {
             if (b.field == 1) { // Partitioning
                 PbReader pt = b.sub();
@@ -816,13 +940,41 @@ static OperatorP decode_operator(PbReader r) { // Operator operator.proto:32-86
                             else hp.skip();
                         }
                     } else if (pt.field == 2) { pt.skip(); op->num_partitions = 1; }
-                    else throw Unsupported("range / round-robin partitioning is outside the GPU hot path");
+                    else if (pt.field == 3) { // RangePartition partitioning.proto:49-53
+                        op->part_kind = PartKind::Range;
+                        PbReader rp = pt.sub();
+                        while (rp.next()) {
+                            if (rp.field == 1 && rp.wire == 2) op->range_keys.push_back(decode_sort_order(rp.sub()));
+                            else if (rp.field == 2) op->num_partitions = (int32_t)rp.i64();
+                            else if (rp.field == 4 && rp.wire == 2) bound_rows.push_back(rp.sub());
+                            else rp.skip();
+                        }
+                    } else if (pt.field == 4) { // RoundRobinPartition partitioning.proto:55-59
+                        op->part_kind = PartKind::RoundRobin;
+                        PbReader rr = pt.sub();
+                        while (rr.next()) {
+                            if (rr.field == 1) op->num_partitions = (int32_t)rr.i64();
+                            else if (rr.field == 2) op->max_hash_columns = (int32_t)rr.i64();
+                            else rr.skip();
+                        }
+                    } else throw Unsupported("partitioning field " + std::to_string(pt.field) + " is outside the GPU hot path");
                 }
             } else b.skip();
         }
-        for (auto& e : op->hash_exprs) resolve(*e, child_schema());
+        const auto& cs = child_schema();
+        for (auto& e : op->hash_exprs) resolve(*e, cs);
         if (op->num_partitions <= 0) throw PlanError("shuffle writer without partitions");
-        op->schema = child_schema();
+        if (op->part_kind == PartKind::RoundRobin) { // planner.rs:3360-3370, multi_partition.rs:386-430: murmur3 over the first columns
+            const size_t k = op->max_hash_columns <= 0 ? cs.size() : std::min(cs.size(), (size_t)op->max_hash_columns);
+            for (size_t i = 0; i < k; i++) {
+                auto e = mk(ExprKind::Bound);
+                e->index = (int)i;
+                e->type = cs[i];
+                op->hash_exprs.push_back(e);
+            }
+        }
+        if (op->part_kind == PartKind::Range) decode_range_partitioning(*op, cs, bound_rows);
+        op->schema = cs;
         have = true;
         break;
     }

@@ -67,6 +67,7 @@ struct Expr {
     bool lit_null = false;
     int64_t lit_i64 = 0;   // bool/int/date/timestamp
     double lit_f64 = 0;    // float/double
+    uint64_t lit_bits = 0; // float/double: the value's own 32 / 64 bits as sent (NaN payloads kept)
     unsigned __int128 lit_dec = 0; // decimal unscaled (two's complement)
     std::string lit_str;
     // Bound / Unbound
@@ -111,6 +112,9 @@ enum class OpKind { Scan, ShuffleScan, NativeScan, Projection, Filter, HashAgg, 
 // operator.proto JoinType / BuildSide
 enum class JoinType : int { Inner = 0, LeftOuter = 1, RightOuter = 2, FullOuter = 3, LeftSemi = 4, LeftAnti = 5 };
 
+// ShuffleWriter partitioning (partitioning.proto Partitioning): SinglePartition runs as a hash partitioning without keys
+enum class PartKind { Hash, Range, RoundRobin };
+
 // one ORDER BY key (SortOrder expr.proto:385-389, planner.rs:927-950 create_sort_expr): arrow SortOptions{descending, nulls_first}
 struct SortKey {
     ExprP expr;               // a Bound column reference of the child
@@ -149,9 +153,20 @@ struct Operator {
     std::vector<ExprP> grouping;
     std::vector<AggExpr> aggs;
     AggMode mode = AggMode::Partial; // the operator's mode (each aggregate's own: AggExpr::mode)
-    // ShuffleWriter (hash partitioning only)
+    // ShuffleWriter.  Hash: hash_exprs.  RoundRobin: hash_exprs are Bound columns 0 .. k-1 (max_hash_columns as the reference reads it),
+    // which may be more than 8.  Range: range_keys are the sort orders with repeated columns dropped (the first occurrence kept), and
+    // range_bounds the n_bounds boundary rows packed as row keys of range_words words (device/cb_sortkey.h; every field has a null bit,
+    // the last key at bit 0), non-decreasing.  A string key's field is its rank against range_strs[key], that key's distinct
+    // boundary strings in byte order (device/cb_rangepart.h).
+    PartKind part_kind = PartKind::Hash;
     std::vector<ExprP> hash_exprs;
     int num_partitions = 0;
+    int max_hash_columns = 0;
+    std::vector<SortKey> range_keys;
+    std::vector<uint64_t> range_bounds;
+    int64_t n_bounds = 0;
+    int range_words = 1;
+    std::vector<std::vector<std::string>> range_strs;
     // Sort (operator.proto:641-645): the output is sorted[skip : fetch] (SortExec::with_fetch, then GlobalLimitExec(skip));
     // -1 = the field is absent
     std::vector<SortKey> sort_keys;

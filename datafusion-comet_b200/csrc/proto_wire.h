@@ -67,6 +67,20 @@ struct PbReader {
         p += 4;
         return f;
     }
+    uint32_t fixed32() { // a float's bits as sent
+        if (wire != 5 || end - p < 4) throw PbError("protobuf: bad fixed32");
+        uint32_t u;
+        memcpy(&u, p, 4);
+        p += 4;
+        return u;
+    }
+    uint64_t fixed64() { // a double's bits as sent
+        if (wire != 1 || end - p < 8) throw PbError("protobuf: bad fixed64");
+        uint64_t u;
+        memcpy(&u, p, 8);
+        p += 8;
+        return u;
+    }
     int64_t i64() { // int32/int64/bool/enum fields
         if (wire != 0) throw PbError("protobuf: expected varint field");
         return (int64_t)varint();

@@ -115,10 +115,16 @@ const char* cb200_plan_dict_value(cb200_plan* plan, int32_t col, int32_t i, int3
  * plan).  Returns rows, -1 at end, -2 on error. */
 int64_t cb200_execute_device(cb200_plan* plan, cb200_device_column* cols, int32_t n_cols, cb200_error* err);
 
-/* Plans rooted at a ShuffleWriter with HashPartition (at most 8 key columns and 16 384 partitions; cb200_supports refuses more)
- * (operator.proto:688, partitioning.proto:38) return their
- * child's rows reordered by partition id = pmod(murmur3(keys, seed 42), num_partitions) -- the reference's
- * multi_partition.rs:265-330 -- stable within a partition.  After each cb200_execute / cb200_execute_device
+/* Plans rooted at a ShuffleWriter (operator.proto:688, partitioning.proto; at most 16 384 partitions, cb200_supports refuses more)
+ * return their child's rows reordered by partition id, stable within a partition.  The partition id of a row is:
+ *   HashPartition (at most 8 key columns):  pmod(murmur3(keys, seed 42), num_partitions) -- multi_partition.rs:265-330
+ *   SinglePartition:                        0
+ *   RoundRobinPartition:                    pmod(murmur3(first max_hash_columns columns, all when <= 0), num_partitions)
+ *                                           -- multi_partition.rs:386-430
+ *   RangePartition:                         the number of boundary rows <= the row under the sort orders (repeated sort
+ *                                           columns dropped) -- multi_partition.rs:333-380; with fewer than num_partitions - 1
+ *                                           boundary rows the last partitions are empty.
+ * After each cb200_execute / cb200_execute_device
  * this returns the num_partitions+1 row offsets of that batch (the map-side of the exchange; the reference writes
  * the same segments as per-partition IPC blocks).  Returns the number of entries. */
 int32_t cb200_plan_partition_starts(cb200_plan* plan, int64_t* starts, int32_t cap);
@@ -142,8 +148,10 @@ typedef struct cb200_exchange_stats {
     int64_t bytes_sent, bytes_received; /* payload bytes incl. the segment this rank keeps */
     double payload_ms;                  /* CUDA-event duration of the grouped send/recv on the communicator's stream */
 } cb200_exchange_stats;
-/* The exchange itself.  `map_plan` is a ShuffleWriter(HashPartitioning(keys, world)) plan whose last cb200_execute /
- * cb200_execute_device batch is still alive: its rows are ordered by partition id = pmod(murmur3(keys, 42), world).  Every rank calls
+/* The exchange itself.  `map_plan` is a ShuffleWriter plan with num_partitions = world whose last cb200_execute /
+ * cb200_execute_device batch is still alive: its rows are ordered by partition id (cb200_plan_partition_starts: pmod(murmur3(keys,
+ * 42), world) for HashPartitioning, the number of boundary rows <= the row for RangePartitioning, so that rank r receives the r-th
+ * range of a global order, and murmur3 over the first columns for RoundRobinPartitioning).  Every rank calls
  * this exactly once per map plan, collectively -- also when its map plan produced no batch (an empty partition, a filter that removed
  * every row): that rank takes part with zero rows of the plan's output schema.  Rank r gets back a device table (owned by the
  * library, release with cb200_table_release) holding partition r of every rank, sources in rank order, rows in their map-side order
@@ -209,6 +217,9 @@ typedef struct cb200_stats {
     int64_t agg_range_reruns;  /* dense aggregate launches discarded because their input broke the value range the kernel assumed */
     int64_t join_cond_pairs;   /* candidate pairs their join condition was evaluated on: pairs with equal keys (HashJoin, SortMergeJoin), every
                                   (probe row, build row) pair (BroadcastNestedLoopJoin: n * m per probe batch when the build side has rows) */
+    double partition_ids_ms;    /* ShuffleWriter stages, device time between CUDA events on the plan's stream, summed over batches: */
+    double partition_place_ms;  /*   the partition ids, their stable counting sort (histogram, scan, placement) */
+    double partition_gather_ms; /*   and the gather of the columns into partition order */
 } cb200_stats;
 #define CB200_AGG_DENSE 1      /* thread-private accumulators over dictionary / bool key codes (and ungrouped aggregates) */
 #define CB200_AGG_TABLE 2      /* global key table */
