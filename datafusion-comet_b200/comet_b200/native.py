@@ -68,7 +68,8 @@ class Stats(C.Structure):
                 ("sort_passes", C.c_int64), ("sort_pass_rows", C.c_int64), ("sort_select_rows", C.c_int64),
                 ("join_build_rows", C.c_int64), ("join_probe_rows", C.c_int64), ("join_out_rows", C.c_int64),
                 ("agg_range_levels", C.c_int64), ("agg_range_reruns", C.c_int64), ("join_cond_pairs", C.c_int64),
-                ("partition_ids_ms", C.c_double), ("partition_place_ms", C.c_double), ("partition_gather_ms", C.c_double)]
+                ("partition_ids_ms", C.c_double), ("partition_place_ms", C.c_double), ("partition_gather_ms", C.c_double),
+                ("agg_table_grows", C.c_int64), ("agg_stream_reruns", C.c_int64)]
 AGG_DENSE, AGG_TABLE, AGG_STREAM, AGG_MIGRATED = 1, 2, 4, 8  # cb200_stats.agg_strategies bits (CB200_AGG_*)
 RANGE_TIGHT, RANGE_TYPE, RANGE_SAFE = 1, 2, 4  # cb200_stats.agg_range_levels bits (CB200_RANGE_*)
 

@@ -363,6 +363,8 @@ int cb200_plan_stats(cb200_plan* plan, cb200_stats* out) {
     out->partition_ids_ms = c.partition_ids_ms;
     out->partition_place_ms = c.partition_place_ms;
     out->partition_gather_ms = c.partition_gather_ms;
+    out->agg_table_grows = c.agg_table_grows;
+    out->agg_stream_reruns = c.agg_stream_reruns;
     return 0;
 }
 

@@ -224,6 +224,7 @@ struct IdRows {
         if (zero_fill) init_totals(ctx, k, tp, 0, nm + 2);
         else if (!htotals) init_totals(ctx, k, tp, nm, 2);
         if (htotals) {
+            if (std::any_of(cnt, cnt + GK, [](int64_t c) { return c > 0; })) ctx->agg_table_grows++;
             for (int r = 0; r < GK; r++) {
                 if (cnt[r] <= 0) continue;
                 cuda_check(cudaMemcpyAsync(tp + (size_t)r * Rn * n_words * 2, (cb::u64*)htotals->ptr + (size_t)r * Ro * n_words * 2, (size_t)cnt[r] * n_words * 16,
@@ -457,7 +458,8 @@ struct AggNode : FusedBase {
             acc /= 2;
         }
         if (acc + 2 * (size_t)probe.stage_bytes + 1024 > SMEM_BUDGET)
-            throw Unsupported("too many groups x aggregates for the thread-private accumulators of the dense path");
+            throw Unsupported(hash ? "too many state / input columns to stage in shared memory for the hash aggregate kernel"
+                                   : "too many groups x aggregates for the thread-private accumulators of the dense path");
         s.stages = (int)std::max<size_t>(2, std::min<size_t>(6, (SMEM_BUDGET - 1024 - acc) / (size_t)probe.stage_bytes));
         return s;
     }
@@ -857,6 +859,7 @@ struct AggNode : FusedBase {
             handed_out = stream_launch(b, 0, b.n_rows, k, hf, cnt);
             if (!(hf.w[0] & CB_HF_FULL)) break;
             // more runs than state rows: nothing of this launch is kept (its rows only touched ids past the old counts and the shared group)
+            ctx->agg_stream_reruns++;
             stream.snapshot_reserved(ctx, rows, n_words, true);
             for (int r = 0; r < GK; r++) before.w[CB_HFLAG_CTR + r] = (int)cnt0[r];
             rows.write_flags(ctx, before);

@@ -143,6 +143,8 @@ struct ExecContext {
     int64_t join_build_rows = 0, join_probe_rows = 0, join_out_rows = 0; // hash, sort-merge and nested-loop joins: rows drained from the build side, rows probed, rows out
     int64_t join_cond_pairs = 0;  // candidate (probe row, build row) pairs a join condition was evaluated on
     double partition_ids_ms = 0, partition_place_ms = 0, partition_gather_ms = 0; // ShuffleWriter stages, device time by CUDA events
+    int64_t agg_table_grows = 0;  // IdRows::grow calls that moved groups already handed out to a larger array
+    int64_t agg_stream_reruns = 0; // stream launches discarded because their runs outnumbered the state rows, then repeated
     std::vector<int64_t> partition_starts; // last ShuffleWriter batch: partition p = rows [starts[p], starts[p+1])
     void check_device_errors() { raise_device_errors(take_device_errors()); }
     int take_device_errors();           // synchronises; returns the error flags the kernels raised so far and clears them

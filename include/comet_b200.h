@@ -220,6 +220,10 @@ typedef struct cb200_stats {
     double partition_ids_ms;    /* ShuffleWriter stages, device time between CUDA events on the plan's stream, summed over batches: */
     double partition_place_ms;  /*   the partition ids, their stable counting sort (histogram, scan, placement) */
     double partition_gather_ms; /*   and the gather of the columns into partition order */
+    int64_t agg_table_grows;    /* hash aggregates' id-addressed state rows regrown while some group id was handed out (each range moved to
+                                   its new offset, the two reserved rows to the new tail; the key table path then re-inserts every key) */
+    int64_t agg_stream_reruns;  /* stream-strategy launches discarded because their runs outnumbered the state rows (the reserved rows
+                                   restored from their snapshot, the arrays grown, the launch repeated) */
 } cb200_stats;
 #define CB200_AGG_DENSE 1      /* thread-private accumulators over dictionary / bool key codes (and ungrouped aggregates) */
 #define CB200_AGG_TABLE 2      /* global key table */
