@@ -760,24 +760,8 @@ i64 sort_tiles(i64 n) { return (n + SORT_TILE - 1) / SORT_TILE; }
 // ---- hash join ------------------------------------------------------------------------------------------------------------------------------
 // The build side's row keys are radix-sorted, so equal keys form runs in build input order.  Each distinct key (run) owns one slot of an
 // open-addressing table, found by linear probing from its hash; a slot stores a 32-bit tag of the hash and the run, and a tag hit is
-// confirmed against the run's key words, so two keys are never merged and no collision can fail the query.
-__device__ __forceinline__ u64 join_hash(const u64* k, int W) {
-    u64 h = 0x9E3779B97F4A7C15ull;
-#pragma unroll
-    for (int j = 0; j < SK_MAX_WORDS; j++) {
-        if (j >= W) break;
-        h ^= k[j];
-        h ^= h >> 33; h *= 0xff51afd7ed558ccdull; h ^= h >> 33; h *= 0xc4ceb9fe1a85ec53ull; h ^= h >> 33; // murmur3 fmix64
-    }
-    return h;
-}
-__device__ __forceinline__ bool join_no_null(const JoinTable& t, const u64* k) {
-    bool ok = true;
-#pragma unroll
-    for (int j = 0; j < SK_MAX_WORDS; j++)
-        if (j < t.words) ok &= (k[j] & t.nullmask[j]) == t.nullmask[j];
-    return ok;
-}
+// confirmed against the run's key words, so two keys are never merged and no collision can fail the query.  The hash and the NULL test
+// are join_hash / join_no_null (device/cb_sortkey.h).
 __global__ void k_join_heads(const u64* keys, int W, i64 m, u8* head) {
     const i64 i = (i64)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= m) return;
@@ -789,14 +773,14 @@ __global__ void k_join_insert(JoinTable t, i64 n_runs) {
     const i64 r = (i64)blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= n_runs) return;
     const u64* k = t.keys + (i64)t.run_start[r] * t.words;
-    if (!join_no_null(t, k)) return;
+    if (!join_no_null(k, t.nullmask, t.words)) return;
     const u64 h = join_hash(k, t.words), v = ((h >> 32) << 32) | (u64)(r + 1);
     for (u64 s = h & t.mask;; s = (s + 1) & t.mask) // capacity >= 2 x runs: a free slot exists
         if (atomicCAS((unsigned long long*)&t.slots[s], 0ull, (unsigned long long)v) == 0ull) return;
 }
 // the run of key k, or -1
 __device__ __forceinline__ i64 join_find(const JoinTable& t, const u64* k) {
-    if (!join_no_null(t, k)) return -1;
+    if (!join_no_null(k, t.nullmask, t.words)) return -1;
     const u64 h = join_hash(k, t.words);
     const u32 tag = (u32)(h >> 32);
     for (u64 s = h & t.mask;; s = (s + 1) & t.mask) {

@@ -1,5 +1,6 @@
 // cb_sortkey.h -- the packed row key of a Sort: key values turned into unsigned bits whose lexicographic order is the reference's
-// order, shared by the key kernel k_sort_keys (aot_kernels.cu) and the host test driver sortkey_test.cpp.
+// order, shared by the key kernel k_sort_keys (aot_kernels.cu) and the host test driver sortkey_test.cpp; and the hash join's hash of
+// that key.
 //
 // Value order is arrow-rs's (arrow-ord, which DataFusion's SortExec uses): signed integers, dates, timestamps and decimals (their
 // unscaled value, any precision) numerically; booleans false < true; strings by unsigned bytes (here the dense byte-order rank of the
@@ -20,6 +21,12 @@
 // HK_DICT* are dictionary codes of 1, 2 or 4 bytes, HK_UTF8 plain offsets + chars.
 enum { HK_BOOL, HK_I8, HK_I16, HK_I32, HK_I64, HK_F32, HK_F64, HK_DEC_SMALL_128, HK_DEC_LARGE_128, HK_DEC_SMALL_64 = HK_I64, HK_DEC_LARGE_64 = 9,
        HK_DICT8 = 10, HK_DICT16, HK_DICT32, HK_UTF8, HK_DEC_SMALL_32, HK_BOOL8 };
+
+#ifdef __CUDACC__
+#define CB_SK_UNROLL _Pragma("unroll")
+#else
+#define CB_SK_UNROLL
+#endif
 
 namespace cb {
 
@@ -114,6 +121,28 @@ template <int W> CB_HD bool sk_row_reg(const SortKeyCols& kc, i64 i, u64 (&w)[W]
             if (sh && sh + nb > 64 && j == W - 2 - lw) w[j] |= v >> (64 - sh);
         }
     });
+}
+
+// The join table's hash of a row key of W <= SK_MAX_WORDS words (k_join_insert / k_join_probe, aot_kernels.cu): each word in turn,
+// word 0 first, XORed into the state and mixed by murmur3's fmix64.  A run's home slot is hash & (capacity - 1), its tag hash >> 32.
+CB_HD u64 join_hash(const u64* k, int W) {
+    u64 h = 0x9E3779B97F4A7C15ull;
+CB_SK_UNROLL
+    for (int j = 0; j < SK_MAX_WORDS; j++) {
+        if (j >= W) break;
+        h ^= k[j];
+        h ^= h >> 33; h *= 0xff51afd7ed558ccdull; h ^= h >> 33; h *= 0xc4ceb9fe1a85ec53ull; h ^= h >> 33; // murmur3 fmix64
+    }
+    return h;
+}
+
+// a join key has no NULL field: every field's null bit (nullmask, set on a valid value) is set
+CB_HD bool join_no_null(const u64* k, const u64* nullmask, int W) {
+    bool ok = true;
+CB_SK_UNROLL
+    for (int j = 0; j < SK_MAX_WORDS; j++)
+        if (j < W) ok &= (k[j] & nullmask[j]) == nullmask[j];
+    return ok;
 }
 
 } // namespace cb

@@ -52,4 +52,9 @@ long long cb_sk_encode(int n_keys, const int* kind, const int* bits, const int* 
     return bad;
 }
 
+// join_hash of n row keys of `words` words each (keys[i * words + j], word 0 first) into out[i]
+void cb_join_hash(const unsigned long long* keys, long long n, int words, unsigned long long* out) {
+    for (long long i = 0; i < n; i++) out[i] = cb::join_hash(keys + i * words, words);
+}
+
 } // extern "C"
